@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Benchmark of the mPLUG-Video pre-training hot path (BASELINE.json configs[1]).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's B200 path
+  python bench.py --gpus N --steps K --warmup W            # this repo's H100 path
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as .npy
   python bench.py --impl reference --gpus N --steps K ...   # the reference's algorithm on host cores
 
 A step = one pre-training iteration through the public model API: forward (TimeSformer ->
@@ -36,14 +37,16 @@ GCFG = {"1.3B": dict(vocab_size=51200, hidden_size=2048, ffn_hidden_size=8192, n
                      max_position_embeddings=2048, layernorm_epsilon=1e-5, init_method_std=0.02),
         "2.7B": dict(vocab_size=51200, hidden_size=2560, ffn_hidden_size=10240, num_hidden_layers=32, num_attention_heads=32,
                      max_position_embeddings=2048, layernorm_epsilon=1e-5, init_method_std=0.02)}
-# --config: (model class, decoder, frames, text length, batch/GPU, metric)
+# --config: (model class, decoder, frames, text length, batch/GPU, metric).  Batches are sized for one 80 GB H100: the
+# timed CUDA-graph step keeps its activations in the graph's memory pool while the untimed eager step of the same batch
+# (launch count, GEMM roofline) allocates its own.
 CONFIGS = {
     "pretrain": dict(cls="DistributedGPT3_Pretrain", gpt="1.3B", frames=8, text_len=128, batch=32, metric=METRIC,
                      workload="mPLUG-Video GPT-3 1.3B pretrain step (BASELINE configs[1])"),
-    "caption27b": dict(cls="DistributedGPT3_Caption", gpt="2.7B", frames=16, text_len=256, batch=32,
+    "caption27b": dict(cls="DistributedGPT3_Caption", gpt="2.7B", frames=16, text_len=256, batch=8,
                        metric="video-text samples/sec (caption fine-tuning 2.7B, 16f x 224^2, text 256)",
                        workload="mPLUG-Video GPT-3 2.7B caption fine-tuning step (BASELINE configs[3])"),
-    "retrieval": dict(cls="DistributedGPT3_Retrieval", gpt="1.3B", frames=8, text_len=80, batch=96,
+    "retrieval": dict(cls="DistributedGPT3_Retrieval", gpt="1.3B", frames=8, text_len=80, batch=24,
                       metric="video-text samples/sec (contrastive retrieval 1.3B, 8f x 224^2, text 80)",
                       workload="mPLUG-Video GPT-3 1.3B contrastive retrieval step, feature all-gather across ranks (BASELINE configs[2])"),
 }
@@ -76,7 +79,8 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA's H100 SXM data sheet (dense bf16, 700 W): an upper bound, not a measured rate
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, source="fallback (H100 SXM data sheet)")
 
 
 class ClockSampler:
@@ -284,6 +288,8 @@ def run_ymp(args, rank, local_rank, world):
     if rank == 0:
         sampler.start()
     ms, last_loss = timed(step_resident, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss, eng)
     # kernels of ours enqueued per timed step: counted on one eager step (a graph replay re-launches the
     # same kernels without going through the library's host entry points)
     n0 = lib.launch_count()
@@ -318,7 +324,7 @@ def run_ymp(args, rank, local_rank, world):
         step_e2e_u8()
     ms_e2e_u8, _ = timed(step_e2e_u8, args.steps)
 
-    # ---- roofline of the dominant kernel (tcgen05 GEMM): CUDA events around every launch of one
+    # ---- roofline of the dominant kernel (wgmma GEMM): CUDA events around every launch of one
     # extra, untimed step on the launching stream; achieved = sum(2MNK) / sum(duration)
     rec = []
     orig = ops.gemm
@@ -364,18 +370,8 @@ def run_ymp(args, rank, local_rank, world):
     if args.config == "pretrain" and (T, L, Q) == (8, 128, 128):
         assert abs(gf_sample - GF_PER_SAMPLE) < 0.5, gf_sample       # SURVEY.md section 8(d), config 2
     step_tf = gf_sample * B / ms_step  # GFLOP/ms == TFLOP/s
-    traffic, traffic_note = None, None
-    tpath = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    if not os.path.exists(tpath):
-        tpath = os.path.join(ROOT, "profiles", "r01_gemm_traffic.json")
-    if os.path.exists(tpath) and args.config == "pretrain" and (B, T, L, Q) == (32, 8, 128, 128):
-        with open(tpath) as fh:
-            tj = json.load(fh)
-        traffic = tj["bytes_per_launch"]
-        traffic_note = (f"dram__bytes_read+write per GEMM launch, ncu capture committed in profiles/{os.path.basename(tpath)} "
-                        f"(= {tj['measured_over_algorithmic']:.2f} x the algorithmic operand bytes)")
-    roofline = dict(bound="tensor", kernel="gemm_bf16_tcgen05_2cta_kernel", achieved=tf, peak=pk["tf_sustained"], unit="TFLOP/s",
-                    frac=tf / pk["tf_sustained"], traffic=traffic, traffic_note=traffic_note,
+    roofline = dict(bound="tensor", kernel="gemm_bf16_wgmma_kernel", achieved=tf, peak=pk["tf_sustained"], unit="TFLOP/s",
+                    frac=tf / pk["tf_sustained"],
                     peak_source=pk["source"] + ", sustained figure",
                     launches_per_step=len(rec), gemm_ms_per_step=gemm_ms, gemm_share_of_step=gemm_ms / ms_step,
                     note="events around each GEMM launch of one extra untimed step; algorithmic 2MNK per launch")
@@ -398,7 +394,7 @@ def run_ymp(args, rank, local_rank, world):
                             lm_head_rows="B*L text rows: the B*Q visual-prefix rows have loss_mask 0 in the reference "
                                          "(distributed_gpt3.py:142-159) and get no final-LN / LM-head / CE work; loss and all "
                                          "gradients are unchanged, algorithmic FLOPs still count them",
-                            l2="per-step working set (~30 GB of activations) >> 126 MB L2; no explicit flush"),
+                            l2="per-step working set (~30 GB of activations) >> 50 MB L2; no explicit flush"),
                 clocks=clocks, gpu_launches=int(launches),
                 e2e=dict(value=e2e_val, unit="samples/s", h2d_bytes_per_step=int(h2d), d2h_bytes_per_step=4,
                          ms_per_step=ms_e2e / args.steps,
@@ -425,6 +421,29 @@ def run_ymp(args, rank, local_rank, world):
     print(json.dumps(line), flush=True)
     if world > 1:
         _teardown(eng, world)
+
+
+DUMP_SAMPLE = 1 << 20   # elements per sampled parameter array (4 MB in float32)
+
+
+def dump_outputs(out_dir, loss, eng):
+    """What the last timed step produced, as float32 / float64 .npy files: the loss it returned and the trainable
+    parameters it updated (bf16 working copy and fp32 master weights).  The parameters are sampled at fixed,
+    seeded positions (the same for every run with the same arguments), so two builds compare element for element."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss.item())], dtype=np.float64))
+    n = eng.master.numel()
+    idx = None
+    if n > DUMP_SAMPLE:
+        g = torch.Generator().manual_seed(20240)
+        idx = torch.randint(0, n, (DUMP_SAMPLE,), generator=g).sort().values.to(eng.master.device)
+    np.save(os.path.join(out_dir, "sample_index.npy"), (idx.cpu() if idx is not None else torch.arange(n)).double().numpy())
+    for name, t in (("params_bf16", eng.flat_param), ("params_master", eng.master)):
+        v = t if idx is None else t[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), v.float().cpu().numpy())
 
 
 def _teardown(eng, world):
@@ -469,6 +488,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--gemm-report", default=None, help="write per-shape GEMM timings of one step to this json file")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel eagerly (no CUDA graph replay)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's loss and a fixed sample of the updated parameters "
+                         "to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

@@ -1,5 +1,5 @@
 /*
- * ymp.h - C ABI of libymp_b200.so: the sm_100a kernels behind the mPLUG-Video (Youku-mPLUG)
+ * ymp.h - C ABI of libymp_b200.so: the sm_90a kernels behind the mPLUG-Video (Youku-mPLUG)
  * pre-training hot path.
  *
  * The reference (X-PLUG/Youku-mPLUG) has no native boundary of its own: every device op on the
@@ -64,7 +64,7 @@ typedef struct ymp_dropout_spec {
 #define YMP_DROP_SITE_BDA_MLP(layer) (4u * (layer) + 3u)    /* bias-dropout-add after the MLP (:1072-1078) */
 
 /* ------------------------------------------------------------------------------------------
- * GEMM  D[M,N] = epilogue( alpha * op(A)[M,K] . op(B)[N,K]^T )          tcgen05 + TMA + TMEM
+ * GEMM  D[M,N] = epilogue( alpha * op(A)[M,K] . op(B)[N,K]^T )          wgmma + TMA
  *
  * Replaces: F.linear in ViT Attention qkv/proj (models/vision_transformer.py:171-176,205),
  * temporal_fc (:250), Mlp fc1/fc2 (:103-110), AttentionPool in/out proj + MLP (:368-374),
@@ -113,7 +113,7 @@ typedef struct ymp_gemm_args {
   int32_t accumulate;   /* 1: D (fp32) += result using atomics */
   int32_t split_k;      /* >=1; >1 requires accumulate=1 and out_dtype=F32; 0 = library picks */
   float alpha;
-  int32_t tile_n;       /* 0 = auto, else 128 or 256 */
+  int32_t tile_n;       /* 0 = auto, else 128 or 256 (512 is accepted and means 256) */
   int32_t res_row_mod;  /* >0: residual row = m % res_row_mod (broadcast tables: position embeddings) */
   int32_t d_row_block;  /* >0: D row = (m / d_row_block) * d_row_stride + m % d_row_block           */
   int32_t d_row_stride; /*     (writes [B*Q] rows into a [B, S>=Q] buffer without a copy)           */
@@ -124,7 +124,7 @@ typedef struct ymp_gemm_args {
    * m = (b*N + n)*T + t (n = py*(W/P) + px: the encoder's patch-major token order), column k = (c, iy, ix) as in
    * conv_weight.flatten(1).  The TMA producer gathers each 128-row x 64-column operand tile straight from the video as
    * four 16-column sub-tiles (one pixel row of every patch: 5-D boxes {16 px, 1 row, T frames} = T rows x 32 bytes, i.e.
-   * SWIZZLE_32B atoms; one tcgen05.mma K-step per sub-tile); no patch matrix is written.  Needs P = 16, T % 8 == 0,
+   * SWIZZLE_32B atoms; one wgmma K-step per sub-tile); no patch matrix is written.  Needs P = 16, T % 8 == 0,
    * 128 % T == 0, M = B*N*T, K = C*P*P, a_mn_major = 0. */
   int32_t im2col_P, im2col_B, im2col_C, im2col_T, im2col_H, im2col_W;
 } ymp_gemm_args;
@@ -250,7 +250,7 @@ typedef struct ymp_attn_args {
   int64_t total_rows;  /* >0 (dense packed sequences only): rows beyond total_rows do not exist, so
                           the last sequence may be shorter than s_q */
   float scale;
-  ymp_dropout_spec drop;  /* dropout of the attention probabilities (tcgen05 kernels only): O = dropout(P) V, the
+  ymp_dropout_spec drop;  /* dropout of the attention probabilities (wgmma and mma.sync kernels): O = dropout(P) V, the
                              softmax statistics (lse) stay those of the undropped P */
   const int32_t* s_kv_dev; /* optional DEVICE scalar: only the first min(s_kv, *s_kv_dev) keys exist.  Lets a captured
                              CUDA graph of the single-token decoding step follow the growing KV cache (forward only,
@@ -271,11 +271,12 @@ typedef struct ymp_attn_bwd_args {
 } ymp_attn_bwd_args;
 int ymp_attn_bwd(const ymp_attn_bwd_args* a, void* stream);
 /* Diagnostic: which kernel family served the last ymp_attn_fwd / ymp_attn_bwd call of this thread (-1: none yet).
- * tcgen05 tiles serve head_dim 64 / 80 / 88 / 96 at any key range; warp-per-sequence kernels the packed
- * block-diagonal (temporal, T <= 16) case; the mma.sync kernels remain for head_dim 128 and for a few query
- * rows against a long cache (single-token decoding). */
+ * Warpgroup-MMA (wgmma) tiles serve head_dim 64 / 80 / 88 / 96 at any key range, with or without dropout; warp-per-
+ * sequence kernels the packed block-diagonal (temporal, T <= 16) case; the streaming kernel one query row per
+ * sequence; the mma.sync tiles head_dim 128, other block-diagonal masks, the device-side key count and a few query
+ * rows against a long cache. */
 #define YMP_ATTN_PATH_MMA_SYNC 0
-#define YMP_ATTN_PATH_TCGEN05 1
+#define YMP_ATTN_PATH_WGMMA 1
 #define YMP_ATTN_PATH_SMALL 2
 #define YMP_ATTN_PATH_DECODE 3  /* one query row per sequence: streaming kernel of the decoding step */
 int ymp_attn_last_path(void);

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE - generates tests/golden/*.pt from the UNMODIFIED reference.
 
-Run in the dev container (needs /root/reference):   python oracle/make_golden.py [--full]
+Run next to a checkout of the reference (YMP_REFERENCE=<path>):   python oracle/make_golden.py [--full]
 
 For each config it (1) builds weights with oracle.port.init_state_dict (seeded, reproducible
 anywhere), (2) loads them into the reference's DistributedGPT3_Pretrain (via oracle/ref_shims.py),
@@ -142,7 +142,7 @@ def run(name, vcfg, gcfg, Q, B, L, wseed, iseed, randomize, sample_logits=None, 
 def run_dropout(name, vcfg, gcfg, Q, B, L, wseed, iseed, p_hidden=0.1, p_attn=0.1, seed=20240924, offset=0):
     """Decoder dropout (the ★ row of the coverage table): the UNMODIFIED reference's DistributedGPT3_Pretrain in
     train() mode with hidden_dropout / attention_dropout live (as in real training: the frozen decoder stays in
-    train mode), its F.dropout masks drawn from the B200 kernels' Philox convention (ref_shims.philox_dropout).
+    train mode), its F.dropout masks drawn from the H100 kernels' Philox convention (ref_shims.philox_dropout).
     The oracle's restatement with the same masks must agree (pins port.gpt3_layer(drop=...)); the reference's
     outputs and gradients become the fixture the GPU kernels are checked against WITH dropout active."""
     sd = port.init_state_dict(vcfg, gcfg, Q, seed=wseed, randomize=True)

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE - numpy restatement of Philox4x32-10 (Salmon et al., SC'11; the Random123 library) and of
 the dropout-mask convention of youku-mplug_b200/csrc/philox.cuh, so that the CPU oracle can run the decoder WITH
-dropout and be compared against the B200 kernels element for element.
+dropout and be compared against the H100 kernels element for element.
 
 Pinned by the published known-answer vectors of Random123 (kat_vectors: philox4x32-10), checked in
 tests/test_oracle_golden.py.  Only tests / oracle code may import this module."""

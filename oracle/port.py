@@ -194,7 +194,7 @@ GPT_PRE = "text_decoder.dist_model.language_model."
 
 
 def _drop(t2d, drop, site, p):
-    """Dropout with the B200 kernels' Philox mask convention (oracle/philox.py) on a [rows, cols] view."""
+    """Dropout with the H100 kernels' Philox mask convention (oracle/philox.py) on a [rows, cols] view."""
     if drop is None or p <= 0.0:
         return t2d
     from oracle import philox
@@ -207,7 +207,7 @@ def gpt3_layer(x, sd, pre, heads, layer_number, eps, drop=None):
     reference uses [S,B,h]; the arithmetic per (b, head) is identical).  QKV rows are grouped per
     head as [q|k|v]; scores = q.k / (sqrt(hn)*layer) * layer; causal fill value -10000.
     drop = dict(seed, offset, p_hidden, p_attn): train-mode dropout of the attention probabilities (:772-780)
-    and the two bias-dropout-adds (:1051-1078), masks as the B200 kernels draw them (site = 4*layer + 1/2/3)."""
+    and the two bias-dropout-adds (:1051-1078), masks as the H100 kernels draw them (site = 4*layer + 1/2/3)."""
     B, S, H = x.shape
     li = layer_number - 1
     ph = drop["p_hidden"] if drop else 0.0

@@ -1,13 +1,13 @@
 """TEST INFRASTRUCTURE - makes the UNMODIFIED reference modules importable on CPU.
 
-The reference (/root/reference, X-PLUG/Youku-mPLUG @ 9d3dd3f) imports packages that are not in
+The reference ($YMP_REFERENCE, X-PLUG/Youku-mPLUG @ 9d3dd3f) imports packages that are not in
 this image.  This module installs minimal stand-ins into ``sys.modules`` so that
 ``models/{vision_transformer,modeling_distributed_gpt3,distributed_gpt3}.py`` import and run on
 CPU exactly as written.  It is used ONLY to (a) validate oracle/port.py and (b) generate the golden
-vectors under tests/golden/ (oracle/make_golden.py).  Nothing in the product imports it, and it
-cannot run on the GPU box (there is no /root/reference there).
+vectors under tests/golden/ (oracle/make_golden.py).  Nothing in the product or the tests imports it, and it
+needs a checkout of the reference.
 
-Un-vendored arithmetic restated here (source absent from /root/reference):
+Un-vendored arithmetic restated here (source absent from the reference checkout):
   * megatron_util==1.3.0 (README.md:60): tensor-parallel linears / embedding / vocab-parallel CE /
     FusedScaleMaskSoftmax / MixedFusedLayerNorm / bias_gelu_impl.  Stand-ins implement TP=1
     semantics following upstream Megatron-LM: linear = x @ W^T (+ b unless skip_bias_add, in which
@@ -31,7 +31,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-REFERENCE_ROOT = os.environ.get("YMP_REFERENCE", "/root/reference")
+REFERENCE_ROOT = os.environ.get("YMP_REFERENCE", "reference")
 
 
 def _module(name, **attrs):
@@ -235,7 +235,7 @@ def build_reference_pretrain(visual_cfg, gpt_cfg, num_learnable_token, seed=0, u
 
 class philox_dropout:
     """Context manager: while active, torch.nn.functional.dropout (hence nn.Dropout and the reference's
-    bias_dropout_add, models/modeling_distributed_gpt3.py:1056-1078) draws its masks from the B200 kernels' Philox
+    bias_dropout_add, models/modeling_distributed_gpt3.py:1056-1078) draws its masks from the H100 kernels' Philox
     convention (oracle/philox.py) instead of torch's generator, so the UNMODIFIED reference can be run in train()
     mode with exactly the masks the kernels will use.  Call sites of one decoder pass are identified by call order:
     embedding dropout ([s,b,h], :631) -> site 0, then per layer attention probabilities ([b,np,sq,sk], :732) ->

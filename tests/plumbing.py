@@ -87,68 +87,3 @@ schedular: {{
     with open(path, "w") as f:
         f.write(cfg)
     return dict(config=path, model_dir=md, output_dir=os.path.join(td, "out"), videos=vids)
-
-
-def make_downstream_workspace(td, task, num_videos=8, batch_size=2, max_length=8, num_frames=2):
-    """Workspace for the reference's downstream scripts (downstream/run_{cls,caption,retrieval,retrieval_itm}...py): the
-    tiny model directory of make_workspace plus train / val / test csv files in the format the task's dataset class reads
-    (dataset/video_downstream_datasets.py:34-41,118-125,335-347,413-423) and a task yaml with the reference's keys."""
-    ws = make_workspace(td, num_videos=num_videos, batch_size=batch_size, max_length=max_length)
-    rng = np.random.default_rng(1)
-    words = "a b c d e f g hello world video cat dog runs on the grass".split()
-    clips = [f"clip{i}.npy" for i in range(num_videos)]
-    if task == "cls":
-        classes = list(json.load(open(os.path.join(os.environ.get("YMP_REFERENCE", "/root/reference"), "classname.json"))))
-        header, rows = "video_id:FILE,title,label", [f"{c},{' '.join(rng.choice(words, 3))},{classes[i % len(classes)]}" for i, c in enumerate(clips)]
-        prefix, extra = "classification", "use_cls: true\nnum_frames: %d\nnum_classes: %d\n" % (num_frames, len(classes))
-    elif task == "caption":
-        header, rows = "video_id:FILE,golden_caption", [f"{c},\"['{' '.join(rng.choice(words, 3))}']\"" for c in clips]
-        prefix, extra = "captioning", "use_cls: true\nnum_frames: %d\nprompt: \"\"\n" % num_frames
-    else:
-        header, rows = "clip_name:FILE,caption", [f"{c},{' '.join(rng.choice(words, 3))}" for c in clips]
-        prefix = "retrieval"
-        extra = ("use_cls: true\n" if task == "retrieval_itm" else "") + "num_frames: %d\ntemp: 0.07\nembed_dim: 32\n" % num_frames
-    files = {}
-    for split in ("train", "val", "test"):
-        files[split] = os.path.join(td, f"{prefix}_{split}.csv")
-        with open(files[split], "w") as f:
-            f.write(header + "\n" + "\n".join(rows) + "\n")
-    cfg = f"""train_file: '{files['train']}'
-val_file: '{files['val']}'
-test_file: '{files['test']}'
-read_local_data: true
-video_root: "{ws['videos']}/"
-text_decoder: '{ws['model_dir']}/'
-text_cfg: {os.path.join(ws['model_dir'], 'config.json')}
-visual_cfg: '{os.path.join(td, 'vis.json')}'
-megatron_cfg: {{
-  "world_size": 1,
-  "model_parallel_size": 1,
-  "tensor_model_parallel_size": 1,
-}}
-batch_size: {batch_size}
-num_workers: 0
-max_length: {max_length}
-freeze_vit: false
-freeze_text_decoder: true
-num_learnable_token: 8
-{extra}optimizer: {{
-  lr: 2e-5,
-  opt: "AdamW",
-  weight_decay: 0.05,
-  clip_grad: 3.0,
-  opt_betas: [0.9, 0.999],
-  opt_eps: 1e-6
-}}
-schedular: {{
-  epochs: 1,
-  min_lr: 1e-6,
-  warmup_epochs: -1,
-  warmup_steps: 1,
-  lr_sched_type: "cosine"
-}}
-"""
-    path = os.path.join(td, f"{task}_tiny.yaml")
-    with open(path, "w") as f:
-        f.write(cfg)
-    return dict(ws, config=path)

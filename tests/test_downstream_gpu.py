@@ -1,4 +1,4 @@
-"""GPU: the downstream task models (SURVEY.md section 8a rows a20-a23) on the B200 kernels against the
+"""GPU: the downstream task models (SURVEY.md section 8a rows a20-a23) on the H100 kernels against the
 oracle composed from the same reference-pinned primitives (oracle/port.py)."""
 import os
 
@@ -116,7 +116,7 @@ def test_retrieval_cls_shapes_and_negatives(cuda):
 
 
 def test_downstream_models_match_reference_fixture(cuda):
-    """The four downstream task models on the B200 kernels against the UNMODIFIED reference's outputs
+    """The four downstream task models on the H100 kernels against the UNMODIFIED reference's outputs
     (tests/golden/tiny_downstream.pt: same seeded weights and inputs, reference run in fp32 on CPU)."""
     import os
     fx = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "tiny_downstream.pt"), weights_only=False)

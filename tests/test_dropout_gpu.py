@@ -98,7 +98,7 @@ def _attn_ref(q, k, v, scale, causal, keep, p):
 @pytest.mark.parametrize("hd,heads,S,causal", [(64, 4, 256, True), (64, 2, 100, True), (80, 2, 384, True), (96, 2, 197, False),
                                                (64, 2, 520, False)])
 def test_attention_dropout_fwd_bwd(cuda, hd, heads, S, causal):
-    """O = dropout(P) V forward and backward on the tcgen05 kernels (GPT3CoreAttention, :768-782), masks regenerated in
+    """O = dropout(P) V forward and backward on the wgmma kernels (GPT3CoreAttention, :768-782), masks regenerated in
     the backward from (seed, offset, site, row, key)."""
     from ymp import lib, ops
     torch.manual_seed(3)
@@ -113,7 +113,7 @@ def test_attention_dropout_fwd_bwd(cuda, hd, heads, S, causal):
     drop = ops.Drop(_rng(cuda), site, p)
     kw = dict(n_seq=n, n_heads=heads, head_dim=hd, s_q=S, s_kv=S, causal=causal, scale=hd ** -0.5, drop=drop)
     lse = ops.attn_fwd(tq, tk, tv, to, **kw)
-    assert lib.attn_last_path() == lib.ATTN_PATH_TCGEN05
+    assert lib.attn_last_path() == lib.ATTN_PATH_WGMMA
     keep = torch.from_numpy(philox.keep_mask(SEED, OFFSET, site, np.arange(n * heads * S), S, p)).to(cuda).view(n, heads, S, S).float()
     ref = _attn_ref(q, k, v, hd ** -0.5, causal, keep, p)
     assert _rel(out.view(n, S, heads, hd).permute(0, 2, 1, 3), ref) < 2e-2

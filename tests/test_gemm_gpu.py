@@ -1,4 +1,4 @@
-"""GPU parity: tcgen05 GEMM (ymp_gemm) vs an fp32 torch matmul of the same bf16 inputs."""
+"""GPU parity: wgmma GEMM (ymp_gemm) vs an fp32 torch matmul of the same bf16 inputs."""
 import pytest
 import torch
 
@@ -101,12 +101,12 @@ def test_gemm_f32_out_and_splitk(cuda):
     ops.gemm(a, b, a_t=True, b_t=True, out=acc2, accumulate=True, split_k=0)
     _close(acc2, ref, 1e-3)
     acc3 = torch.zeros(M, N, device=cuda, dtype=torch.float32)
-    ops.gemm(a, b, a_t=True, b_t=True, out=acc3, accumulate=True, split_k=4, tile_n=512)   # CTA-pair tiles
+    ops.gemm(a, b, a_t=True, b_t=True, out=acc3, accumulate=True, split_k=4, tile_n=512)   # the widest tile
     _close(acc3, ref, 1e-3)
 
 
 def test_gemm_large_persistent(cuda):
-    """More tiles than SMs: exercises the persistent loop, the smem ring wrap and both TMEM stages."""
+    """More tiles than SMs: exercises many CTAs per SM in sequence and the smem ring wrap."""
     from ymp import ops
     torch.manual_seed(4)
     M, N, K = 4096 + 64, 2048, 1024
@@ -115,9 +115,9 @@ def test_gemm_large_persistent(cuda):
     out = ops.gemm(a, b)
     ref, _ = _ref(a, b, False, False)
     _close(out, ref, 1e-2)
-    out_p = ops.gemm(a, b, tile_n=512)   # CTA pairs: persistent loop + 6-stage ring + both TMEM stages
+    out_p = ops.gemm(a, b, tile_n=512)   # the widest tile (256 columns)
     _close(out_p, ref, 1e-2)
-    big_m = torch.randn(20000, K, device=cuda).bfloat16()   # > 74 pairs: several tiles per pair
+    big_m = torch.randn(20000, K, device=cuda).bfloat16()   # more tiles than SMs: several waves of CTAs
     _close(ops.gemm(big_m, b, tile_n=512), big_m.float() @ b.float().t(), 1e-2)
     # strided views (ld > width) as produced by slicing packed QKV buffers
     big = torch.randn(M, 3 * K, device=cuda).bfloat16()

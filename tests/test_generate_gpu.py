@@ -1,4 +1,4 @@
-"""GPU: KV-cache decoding and generation (SURVEY.md 8f N2) on the B200 kernels against the reference's golden
+"""GPU: KV-cache decoding and generation (SURVEY.md 8f N2) on the H100 kernels against the reference's golden
 sequences (tests/golden/tiny_generate.pt) and the oracle's teacher-forced log-probabilities."""
 import os
 

@@ -1,4 +1,4 @@
-"""GPU parity of the whole hot path: the drop-in models (bf16, B200 kernels) against
+"""GPU parity of the whole hot path: the drop-in models (bf16, H100 kernels) against
 (a) the golden fixtures = outputs of the UNMODIFIED reference (fp32), and
 (b) the oracle (oracle/port.py, fp32 on CPU) fed the same bf16-rounded weights.
 Tolerance: north_star asks forward logits within 1e-2 rel of the reference; measured against the

@@ -94,7 +94,7 @@ def _attn_ref(q, k, v, scale, causal):
 @pytest.mark.parametrize("hd,heads,S,causal,layout", [
     (64, 4, 256, True, "gpt"), (64, 2, 100, True, "gpt"), (80, 2, 130, True, "gpt"),
     (96, 2, 197, False, "vit"), (96, 8, 64, False, "vit"), (64, 2, 300, False, "vit"),
-    # tcgen05 kernels at block boundaries: one / two key blocks, partial second query block, tiny sequences
+    # tensor-core tiles at block boundaries: one / two key blocks, partial second query block, tiny sequences
     (64, 2, 129, True, "gpt"), (96, 1, 33, True, "vit"), (96, 2, 128, False, "vit"), (96, 2, 256, False, "gpt"),
     (64, 3, 160, False, "gpt"), (64, 1, 8, True, "gpt"),
     # key ranges > 256 (KV loop + online softmax, dQ partial parked across > 2 key blocks) and head_dim 80 / 88
@@ -123,7 +123,7 @@ def test_attn_dense_fwd_bwd(cuda, hd, heads, S, causal, layout):
     to = ops.TView(out, 0, hd, m)
     kw = dict(n_seq=n, n_heads=heads, head_dim=hd, s_q=S, s_kv=S, causal=causal, scale=scale)
     lse = ops.attn_fwd(tq, tk, tv, to, **kw)
-    assert lib.attn_last_path() == lib.ATTN_PATH_TCGEN05    # no dense shape of the model falls back to mma.sync
+    assert lib.attn_last_path() == lib.ATTN_PATH_WGMMA    # no dense shape of the model falls back to mma.sync
     ref = _attn_ref(q, k, v, scale, causal)
     assert _rel(out.view(n, S, heads, hd).permute(0, 2, 1, 3), ref) < 2e-2
     dout = torch.randn(n * S, C, device=cuda).to(bf16)
@@ -132,7 +132,7 @@ def test_attn_dense_fwd_bwd(cuda, hd, heads, S, causal, layout):
     tdo = ops.TView(dout, 0, hd, m)
     tdq, tdk, tdv = (ops.TView(dqkv, o, hs, m) for o in offs)
     ops.attn_bwd(tq, tk, tv, to, lse, tdo, tdq, tdk, tdv, **kw)
-    assert lib.attn_last_path() == lib.ATTN_PATH_TCGEN05
+    assert lib.attn_last_path() == lib.ATTN_PATH_WGMMA
     if layout == "gpt":
         d5 = dqkv.float().view(n, S, heads, 3, hd)
         dq, dk, dv = (d5[:, :, :, i].permute(0, 2, 1, 3) for i in range(3))
@@ -177,7 +177,7 @@ def test_attn_dense_ragged_total_rows(cuda, hd, S, total, causal):
 @pytest.mark.parametrize("hd,sq,skv", [(64, 70, 200), (96, 256, 33), (96, 129, 256), (64, 128, 128),
                                        (96, 128, 1570), (64, 300, 520), (80, 130, 300), (96, 16, 1000)])
 def test_attn_cross_short_kv(cuda, hd, sq, skv):
-    """Non-causal cross attention with s_q != s_kv on the tcgen05 kernels: short key ranges and the long ones
+    """Non-causal cross attention with s_q != s_kv on the tensor-core kernels: short key ranges and the long ones
     of the abstractor (128 queries x 1570 keys, models/vision_transformer.py:368-374)."""
     from ymp import lib, ops
     torch.manual_seed(21)
@@ -190,7 +190,7 @@ def test_attn_cross_short_kv(cuda, hd, sq, skv):
     tq, tk, tv, to = ops.TView(qb, 0, hd, mq), ops.TView(kvb, 0, hd, mkv), ops.TView(kvb, C, hd, mkv), ops.TView(out, 0, hd, mq)
     kw = dict(n_seq=n, n_heads=heads, head_dim=hd, s_q=sq, s_kv=skv, causal=False, scale=hd ** -0.5)
     lse = ops.attn_fwd(tq, tk, tv, to, **kw)
-    assert lib.attn_last_path() == lib.ATTN_PATH_TCGEN05
+    assert lib.attn_last_path() == lib.ATTN_PATH_WGMMA
     q = qb.float().view(n, sq, heads, hd).permute(0, 2, 1, 3).contiguous().requires_grad_()
     kv = kvb.float().view(n, skv, 2, heads, hd)
     k, v = (kv[:, :, i].permute(0, 2, 1, 3).contiguous().requires_grad_() for i in range(2))

@@ -311,7 +311,7 @@ def _dp_worker(rank, world, port_no, q):
 
 def test_two_gpu_data_parallel_gradient_and_allgather(cuda):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -33,7 +33,7 @@ def initialize(args=None, model=None, optimizer=None, model_parameters=None, tra
                mpu=None, dist_init_required=None, collate_fn=None, config=None, config_params=None):
     from ymp.train import TrainEngine
     if not torch.cuda.is_available():
-        raise RuntimeError("deepspeed.initialize (ymp_b200 engine): needs a CUDA device - the B200 path has no CPU fallback")
+        raise RuntimeError("deepspeed.initialize (ymp_b200 engine): needs a CUDA device - the H100 path has no CPU fallback")
     cfg = config if config is not None else config_params
     if cfg is None:
         cfg = getattr(args, "deepspeed_config", None)
@@ -42,11 +42,11 @@ def initialize(args=None, model=None, optimizer=None, model_parameters=None, tra
             cfg = json.load(f)
     cfg = cfg or {}
     if cfg.get("fp16", {}).get("enabled", False):
-        raise NotImplementedError("the B200 engine trains in bf16 (pass --bf16): fp16 + dynamic loss scaling is not implemented")
+        raise NotImplementedError("the H100 engine trains in bf16 (pass --bf16): fp16 + dynamic loss scaling is not implemented")
     if dist_init_required and not dist.is_initialized():
         init_distributed()
     if mpu is not None and mpu.get_tensor_model_parallel_world_size() != 1:
-        raise ValueError("tensor model parallel size must be 1 on the B200 path (pure data parallel)")
+        raise ValueError("tensor model parallel size must be 1 on the H100 path (pure data parallel)")
     dev = torch.device("cuda", torch.cuda.current_device())
     model = model.to(dev)
     if cfg.get("bf16", {}).get("enabled", True):

@@ -1,12 +1,13 @@
 // Fused attention (softmax(scale * Q K^T + mask) V) forward and backward.
 //
-// This file holds the GENERIC kernels: warp-level mma.sync (m16n8k16 bf16, fp32 accumulate) flash-style
-// tiles for any sequence length and head_dim in {64, 80, 96, 128}; the score matrix never touches HBM.
-// ymp_attn_fwd / ymp_attn_bwd (bottom of the file) dispatch first to the specialised kernels -
-// attention_small.cu (block-diagonal sequences of <= 16 rows: TimeSformer temporal attention) and
-// attention_tc.cu (tcgen05, key range <= 256, head_dim 64 / 96: ViT spatial and GPT attention) - and fall
-// back to these for everything else (the abstractor's 1570-key cross attention, head_dim 80 / 128, long
-// decode contexts) or when YMP_ATTN_LEGACY=1.
+// Flash-style tiles for any sequence length; the score matrix never touches HBM.  Two kernel families share the
+// tiling, masking and softmax: warpgroup MMA (wgmma, head_dim 64 / 80 / 88 / 96: every dense, causal and cross shape
+// of the models) and warp-level mma.sync (m16n8k16; head_dim 128, packed block-diagonal masks, the device-side key
+// count, a few query rows against a long cache).  head_dim 88 is computed zero-padded to 96 in shared memory.
+// Optional dropout of the probabilities (Philox, philox.cuh): the forward drops P after the softmax normaliser, the
+// backward regenerates the same bits.  ymp_attn_fwd / ymp_attn_bwd (bottom of the file) dispatch first to
+// attention_small.cu (block-diagonal sequences of <= 16 rows: TimeSformer temporal attention) and to the
+// single-query decoding kernel, and run everything else here.
 //   forward   : CTA = 64 query rows x (seq, head); K/V tiles streamed with cp.async double buffering
 //   backward  : two kernels, no atomics, deterministic -
 //               dQ   kernel: CTA = 64 query rows, streams K/V   (also emits delta = rowsum(dO*O))
@@ -19,7 +20,9 @@
 #include <stdlib.h>
 
 #include "common.h"
+#include "philox.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace ymp {
 
@@ -116,7 +119,22 @@ struct AttnKParams {
   int lddo, hsdo, lddq, lddk, lddv, hsdq, hsdk, hsdv;
   SeqMap mdo, mdq, mdkv;
   const int* skv_dev;  // optional device scalar: number of keys that exist (KV-cache decoding under a CUDA graph)
+  DropSpec drop;       // dropout of the probabilities (has_drop): row = (seq*heads + head)*s_q + query, column = key
+  int has_drop;
 };
+
+// keep-or-drop of the two adjacent key columns col, col+1 (col even) of `row`: scale or zero in place
+__device__ __forceinline__ void drop2(const DropState& ds, uint32_t row, uint32_t col, float& a, float& b) {
+  const uint4 w = drop_words(ds, row, col >> 2);
+  const uint32_t w0 = (col & 2) ? w.z : w.x, w1 = (col & 2) ? w.w : w.y;
+  a = w0 >= ds.thresh ? a * ds.scale : 0.f;
+  b = w1 >= ds.thresh ? b * ds.scale : 0.f;
+}
+__device__ __forceinline__ float drop1(const DropState& ds, uint32_t row, uint32_t col, float a) {
+  const uint4 w = drop_words(ds, row, col >> 2);
+  const uint32_t c = col & 3, wc = c == 0 ? w.x : c == 1 ? w.y : c == 2 ? w.z : w.w;
+  return wc >= ds.thresh ? a * ds.scale : 0.f;
+}
 
 // effective lengths of sequence s (short last sequence when total_rows is set)
 __device__ __forceinline__ void eff_len(const AttnKParams& p, int s, int& sq, int& skv) {
@@ -154,8 +172,8 @@ __device__ __forceinline__ void apply_mask(const AttnKParams& p, float (&sc)[8][
   }
 }
 
-// Asynchronously load a [64 x D] bf16 tile (positions r0..r0+63 of the resolved sequence).
-template <int D>
+// Asynchronously load a [64 x D] bf16 tile (positions r0..r0+63 of the resolved sequence); columns DIO..D-1 are zero.
+template <int D, int DIO>
 __device__ __forceinline__ void load_tile_async(__nv_bfloat16* dst, const RMat& m, int r0, int n_valid) {
   constexpr int CH = D / 8, LDS = D + 8;
 #pragma unroll
@@ -164,13 +182,13 @@ __device__ __forceinline__ void load_tile_async(__nv_bfloat16* dst, const RMat& 
     if ((64 * CH) % 128 != 0 && idx >= 64 * CH) break;
     const int r = idx / CH, c = idx - r * CH;
     __nv_bfloat16* d = dst + r * LDS + c * 8;
-    if (r0 + r < n_valid) cp_async16(d, mrow(m, r0 + r) + c * 8);
+    if (r0 + r < n_valid && (DIO == D || c * 8 < DIO)) cp_async16(d, mrow(m, r0 + r) + c * 8);
     else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
   }
 }
 
 // ------------------------------------------------------------------------------ forward
-template <int D>
+template <int D, int DIO>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   constexpr int LDS = D + 8, KS = D / 16, TILE = 64 * LDS;
   extern __shared__ __align__(16) uint8_t smem_attn[];
@@ -197,9 +215,9 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   }
   const int ntiles = (kv_end - kv_begin + 63) / 64;
 
-  load_tile_async<D>(Qs, Mq, q0, sq);
-  load_tile_async<D>(KVs, Mk, kv_begin, skv);
-  load_tile_async<D>(KVs + TILE, Mv, kv_begin, skv);
+  load_tile_async<D, DIO>(Qs, Mq, q0, sq);
+  load_tile_async<D, DIO>(KVs, Mk, kv_begin, skv);
+  load_tile_async<D, DIO>(KVs + TILE, Mv, kv_begin, skv);
   cp_async_commit();
 
   uint32_t qf[KS][4];
@@ -208,6 +226,9 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   for (int i = 0; i < D / 8; ++i) { o_acc[i][0] = o_acc[i][1] = o_acc[i][2] = o_acc[i][3] = 0.f; }
   float m_i[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_i[2] = {0.f, 0.f};
   const bool warp_active = (q0 + warp * 16) < sq;
+  DropState ds;  // only read when has_drop
+  if (p.has_drop) ds = drop_state(p.drop);
+  const uint32_t drow0 = (uint32_t)(((long)s * p.n_heads + h) * p.s_q + q0 + warp * 16 + g);
 
   for (int t = 0; t < ntiles; ++t) {
     const int kv0 = kv_begin + t * 64;
@@ -215,8 +236,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
     __nv_bfloat16* Vs = Ks + TILE;
     if (t + 1 < ntiles) {
       __nv_bfloat16* Kn = KVs + ((t + 1) & 1) * 2 * TILE;
-      load_tile_async<D>(Kn, Mk, kv0 + 64, skv);
-      load_tile_async<D>(Kn + TILE, Mv, kv0 + 64, skv);
+      load_tile_async<D, DIO>(Kn, Mk, kv0 + 64, skv);
+      load_tile_async<D, DIO>(Kn + TILE, Mv, kv0 + 64, skv);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -288,6 +309,14 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
         o_acc[i][0] *= alpha[0]; o_acc[i][1] *= alpha[0];
         o_acc[i][2] *= alpha[1]; o_acc[i][3] *= alpha[1];
       }
+      if (p.has_drop) {  // O = dropout(P) V; the normaliser stays that of the undropped P (softmax, then dropout)
+#pragma unroll
+        for (int nb = 0; nb < 8; ++nb) {
+          const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
+          drop2(ds, drow0, col, sc[nb][0], sc[nb][1]);
+          drop2(ds, drow0 + 8, col, sc[nb][2], sc[nb][3]);
+        }
+      }
 #pragma unroll
       for (int kk2 = 0; kk2 < 4; ++kk2) {
         if (kk2 * 16 < nv && kk2 >= nb_lo) {
@@ -321,7 +350,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
     const float inv = l_i[r] > 0.f ? 1.f / l_i[r] : 0.f;
     __nv_bfloat16* orow = p.o + rrow(mo, qi) * p.ldo + h * p.hso;
 #pragma unroll
-    for (int nb = 0; nb < D / 8; ++nb)
+    for (int nb = 0; nb < DIO / 8; ++nb)
       *reinterpret_cast<uint32_t*>(orow + nb * 8 + t4 * 2) =
           pack_bf16(o_acc[nb][2 * r] * inv, o_acc[nb][2 * r + 1] * inv);
     if (p.lse && t4 == 0)
@@ -331,7 +360,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
 
 // ------------------------------------------------------------------------------ backward: dQ
 // Also writes delta[s,h,i] = sum_d dO[i,d] * O[i,d] for the dKdV kernel (which runs after this one).
-template <int D>
+template <int D, int DIO>
 __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
   constexpr int LDS = D + 8, KS = D / 16, TILE = 64 * LDS;
   extern __shared__ __align__(16) uint8_t smem_attn[];
@@ -356,22 +385,22 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
   }
   const int ntiles = (kv_end - kv_begin + 63) / 64;
 
-  load_tile_async<D>(Qs, Mq, q0, sq);
-  load_tile_async<D>(dOs, Mdo, q0, sq);
-  load_tile_async<D>(KVs, Mk, kv_begin, skv);
-  load_tile_async<D>(KVs + TILE, Mv, kv_begin, skv);
+  load_tile_async<D, DIO>(Qs, Mq, q0, sq);
+  load_tile_async<D, DIO>(dOs, Mdo, q0, sq);
+  load_tile_async<D, DIO>(KVs, Mk, kv_begin, skv);
+  load_tile_async<D, DIO>(KVs + TILE, Mv, kv_begin, skv);
   cp_async_commit();
   // delta / lse for this warp's 16 rows, straight from global (O is not needed anywhere else):
-  // lane -> (row = lane/2, half of the head dim = lane%2), all 16-byte loads independent
+  // lane -> (row = lane/2, every other 8-column chunk of the head dim = lane%2), all 16-byte loads independent
   {
     const int r = lane >> 1, hf = lane & 1;
     const int qi = q0 + warp * 16 + r;
     float acc = 0.f;
     if (qi < sq) {
-      const uint4* orow = reinterpret_cast<const uint4*>(p.o + rrow(mo, qi) * p.ldo + h * p.hso + hf * (D / 2));
-      const uint4* drow = reinterpret_cast<const uint4*>(p.dout + rrow(mdo, qi) * p.lddo + h * p.hsdo + hf * (D / 2));
+      const uint4* orow = reinterpret_cast<const uint4*>(p.o + rrow(mo, qi) * p.ldo + h * p.hso);
+      const uint4* drow = reinterpret_cast<const uint4*>(p.dout + rrow(mdo, qi) * p.lddo + h * p.hsdo);
 #pragma unroll
-      for (int c = 0; c < D / 16; ++c) {
+      for (int c = hf; c < DIO / 8; c += 2) {
         const uint4 a = __ldg(orow + c), b = __ldg(drow + c);
         acc += bf16_lo(a.x) * bf16_lo(b.x) + bf16_hi(a.x) * bf16_hi(b.x) + bf16_lo(a.y) * bf16_lo(b.y) +
                bf16_hi(a.y) * bf16_hi(b.y) + bf16_lo(a.z) * bf16_lo(b.z) + bf16_hi(a.z) * bf16_hi(b.z) +
@@ -393,6 +422,9 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
   for (int i = 0; i < D / 8; ++i) { dq_acc[i][0] = dq_acc[i][1] = dq_acc[i][2] = dq_acc[i][3] = 0.f; }
   const bool warp_active = (q0 + warp * 16) < sq;
   float lse_r[2], del_r[2];
+  DropState ds;  // only read when has_drop
+  if (p.has_drop) ds = drop_state(p.drop);
+  const uint32_t drow0 = (uint32_t)(((long)s * p.n_heads + h) * p.s_q + q0 + warp * 16 + g);
 
   for (int t = 0; t < ntiles; ++t) {
     const int kv0 = kv_begin + t * 64;
@@ -400,8 +432,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
     __nv_bfloat16* Vs = Ks + TILE;
     if (t + 1 < ntiles) {
       __nv_bfloat16* Kn = KVs + ((t + 1) & 1) * 2 * TILE;
-      load_tile_async<D>(Kn, Mk, kv0 + 64, skv);
-      load_tile_async<D>(Kn + TILE, Mv, kv0 + 64, skv);
+      load_tile_async<D, DIO>(Kn, Mk, kv0 + 64, skv);
+      load_tile_async<D, DIO>(Kn + TILE, Mv, kv0 + 64, skv);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -452,6 +484,14 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
       }
       if (tile_needs_mask(p, q0 + warp * 16, kv0, skv))
         apply_mask(p, sc, q0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);  // exp2(-inf) = 0
+      if (p.has_drop) {  // dP = dropout'(dO V^T): the same keep bits and scale as the forward
+#pragma unroll
+        for (int nb = 0; nb < 8; ++nb) {
+          const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
+          drop2(ds, drow0, col, dp[nb][0], dp[nb][1]);
+          drop2(ds, drow0 + 8, col, dp[nb][2], dp[nb][3]);
+        }
+      }
 #pragma unroll
       for (int nb = 0; nb < 8; ++nb) {
 #pragma unroll
@@ -487,14 +527,14 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
     if (qi >= sq) continue;
     __nv_bfloat16* dqrow = p.dq + rrow(mdq, qi) * p.lddq + h * p.hsdq;
 #pragma unroll
-    for (int nb = 0; nb < D / 8; ++nb)
+    for (int nb = 0; nb < DIO / 8; ++nb)
       *reinterpret_cast<uint32_t*>(dqrow + nb * 8 + t4 * 2) =
           pack_bf16(dq_acc[nb][2 * r] * p.scale, dq_acc[nb][2 * r + 1] * p.scale);
   }
 }
 
 // ------------------------------------------------------------------------------ backward: dK, dV
-template <int D>
+template <int D, int DIO>
 __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p) {
   constexpr int LDS = D + 8, KS = D / 16, TILE = 64 * LDS;
   extern __shared__ __align__(16) uint8_t smem_attn[];
@@ -522,8 +562,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
 
   auto load_stage = [&](int stage, int qi0) {
     __nv_bfloat16* Qn = QDs + stage * 2 * TILE;
-    load_tile_async<D>(Qn, Mq, qi0, sq);
-    load_tile_async<D>(Qn + TILE, Mdo, qi0, sq);
+    load_tile_async<D, DIO>(Qn, Mq, qi0, sq);
+    load_tile_async<D, DIO>(Qn + TILE, Mdo, qi0, sq);
     if (threadIdx.x < 64) {
       const int qi = qi0 + threadIdx.x;
       float* st = stat + stage * 128;
@@ -532,8 +572,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
     }
   };
 
-  load_tile_async<D>(Ks, Mk, kv0, skv);
-  load_tile_async<D>(Vs, Mv, kv0, skv);
+  load_tile_async<D, DIO>(Ks, Mk, kv0, skv);
+  load_tile_async<D, DIO>(Vs, Mv, kv0, skv);
   load_stage(0, q_begin);
   cp_async_commit();
 
@@ -544,6 +584,9 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
     dv_acc[i][0] = dv_acc[i][1] = dv_acc[i][2] = dv_acc[i][3] = 0.f;
   }
   const bool warp_active = (kv0 + warp * 16) < skv;
+  DropState ds;  // only read when has_drop
+  if (p.has_drop) ds = drop_state(p.drop);
+  const uint32_t dbase = (uint32_t)(((long)s * p.n_heads + h) * p.s_q);
 
   for (int t = 0; t < ntiles; ++t) {
     const int qi0 = q_begin + t * 64;
@@ -625,8 +668,16 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
         for (int e = 0; e < 4; ++e) {
           const int ql = nb * 8 + t4 * 2 + (e & 1);
           const float pv = exp2f(fmaf(st_[nb][e], p.scale_log2, -st[ql]));  // lse=+inf for absent queries -> 0
-          st_[nb][e] = pv;                              // P^T
-          dpt[nb][e] = pv * (dpt[nb][e] - st[64 + ql]);  // dS^T
+          float dz = dpt[nb][e];
+          if (p.has_drop) {  // Z = dropout(P): dV += Z^T dO, dP = dropout'(dZ)
+            const uint32_t qrow = dbase + (uint32_t)(qi0 + ql), key = (uint32_t)(kv0 + warp * 16 + g + (e >> 1) * 8);
+            const float keep = drop1(ds, qrow, key, 1.f);
+            dz *= keep;
+            st_[nb][e] = pv * keep;                    // Z^T
+          } else {
+            st_[nb][e] = pv;                           // P^T
+          }
+          dpt[nb][e] = pv * (dz - st[64 + ql]);        // dS^T
         }
       }
 #pragma unroll
@@ -666,9 +717,445 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
     __nv_bfloat16* dkrow = p.dk + row * p.lddk + h * p.hsdk;
     __nv_bfloat16* dvrow = p.dv + row * p.lddv + h * p.hsdv;
 #pragma unroll
-    for (int nb = 0; nb < D / 8; ++nb) {
+    for (int nb = 0; nb < DIO / 8; ++nb) {
       *reinterpret_cast<uint32_t*>(dkrow + nb * 8 + t4 * 2) =
           pack_bf16(dk_acc[nb][2 * r] * p.scale, dk_acc[nb][2 * r + 1] * p.scale);
+      *reinterpret_cast<uint32_t*>(dvrow + nb * 8 + t4 * 2) = pack_bf16(dv_acc[nb][2 * r], dv_acc[nb][2 * r + 1]);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------ wgmma kernels (head_dim 64 / 80 / 96)
+// The same tiling, masking, softmax and dropout as the mma.sync kernels above, but each CTA is ONE warpgroup whose
+// four warps issue warpgroup MMAs together: S / dP tiles are wgmma m64n64k16 with both operands in shared memory, and
+// the P.V / dS.K / P^T.dO / dS^T.Q products are wgmma m64nDk16 with the probabilities as the register A operand (the
+// m64 accumulator of a warp is exactly the A fragment of the next product) and the shared tile read MN-major.
+// Operand tiles are 64 rows x D bf16 in the SWIZZLE_128B K-major layout that TMA writes (64-column panels of
+// 64 rows x 128 bytes, 16-byte chunk c of row r at chunk c ^ (r & 7)), filled by cp.async through the seqmaps.
+// head_dim 88 is computed as 96 with zero-filled tail columns that are never stored.
+template <int D>
+struct WgTile {
+  static constexpr int BYTES = ((D + 63) / 64) * 8192;
+};
+template <int D, int DIO>
+__device__ __forceinline__ void wg_load_tile(uint8_t* dst, const RMat& m, int r0, int n_valid) {
+  constexpr int CH = D / 8;
+#pragma unroll
+  for (int it = 0; it < (64 * CH + 127) / 128; ++it) {
+    const int idx = threadIdx.x + it * 128;
+    if ((64 * CH) % 128 != 0 && idx >= 64 * CH) break;
+    const int r = idx / CH, c = idx - r * CH;
+    uint8_t* d = dst + (c >> 3) * 8192 + r * 128 + (((c & 7) ^ (r & 7)) << 4);
+    if (r0 + r < n_valid && (DIO == D || c * 8 < DIO)) cp_async16(d, mrow(m, r0 + r) + c * 8);
+    else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
+  }
+}
+// k-step ks (16 head-dim columns) of a tile whose rows are the M / N dimension
+__device__ __forceinline__ uint64_t wg_desc_k(uint32_t base, int ks) {
+  return make_smem_desc(base + (ks >> 2) * 8192 + (ks & 3) * 32, 16, 1024, 1);
+}
+// k-step ks (16 rows) of a tile whose rows are the K dimension and whose head-dim columns are N
+__device__ __forceinline__ uint64_t wg_desc_mn(uint32_t base, int ks) { return make_smem_desc(base + ks * 2048, 8192, 1024, 1); }
+
+template <int D>
+__device__ __forceinline__ void wg_rs(float (&d)[D / 2], const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (D == 64) wgmma_rs_m64n64_tb(d, a, db);
+  else if constexpr (D == 80) wgmma_rs_m64n80_tb(d, a, db);
+  else wgmma_rs_m64n96_tb(d, a, db);
+}
+// S[64 x 64] = A . B^T over the head dimension (both tiles K-major)
+template <int D>
+__device__ __forceinline__ void wg_scores(float (&s)[8][4], uint32_t a, uint32_t b) {
+  float (&f)[32] = *reinterpret_cast<float(*)[32]>(&s[0][0]);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) f[i] = 0.f;
+  wgmma_fence_acc(f);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < D / 16; ++kk) wgmma_ss_m64n64(f, wg_desc_k(a, kk), wg_desc_k(b, kk));
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_acc(f);
+}
+// acc[64 x D] += P[64 x 64] . T[64 x D]  (P as bf16 A fragments of its four 16-column k-steps)
+template <int D>
+__device__ __forceinline__ void wg_pv(float (&acc)[D / 8][4], const float (&pm)[8][4], uint32_t t) {
+  float (&f)[D / 2] = *reinterpret_cast<float(*)[D / 2]>(&acc[0][0]);
+  uint32_t pa[4][4];
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    pa[kk][0] = pack_bf16(pm[2 * kk][0], pm[2 * kk][1]);
+    pa[kk][1] = pack_bf16(pm[2 * kk][2], pm[2 * kk][3]);
+    pa[kk][2] = pack_bf16(pm[2 * kk + 1][0], pm[2 * kk + 1][1]);
+    pa[kk][3] = pack_bf16(pm[2 * kk + 1][2], pm[2 * kk + 1][3]);
+  }
+  wgmma_fence_acc(f);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) wg_rs<D>(f, pa[kk], wg_desc_mn(t, kk));
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_acc(f);
+}
+
+template <int D, int DIO>
+__global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
+  constexpr int TB = WgTile<D>::BYTES;
+  extern __shared__ uint8_t smem_wg[];
+  uint8_t* sm = smem_wg + ((1024u - (smem_u32(smem_wg) & 1023u)) & 1023u);
+  uint8_t* Qs = sm;
+  uint8_t* KVs = sm + TB;  // [stage][K|V]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = blockIdx.x * 64, h = blockIdx.y, s = blockIdx.z;
+  const int g = lane >> 2, t4 = lane & 3;
+  griddep_launch();   // (programmatic dependent launch; no-ops for an ordinary launch)
+  griddep_wait();
+  int sq, skv;
+  eff_len(p, s, sq, skv);
+  if (q0 >= sq) return;
+  const RSeq mkv = resolve(p.mkv, s), mo = resolve(p.mo, s);
+  const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq);
+  const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
+  int kv_end = skv;
+  if (p.mask == MASK_CAUSAL) kv_end = min(skv, q0 + 64);
+  const int ntiles = (kv_end + 63) / 64;
+
+  wg_load_tile<D, DIO>(Qs, Mq, q0, sq);
+  wg_load_tile<D, DIO>(KVs, Mk, 0, skv);
+  wg_load_tile<D, DIO>(KVs + TB, Mv, 0, skv);
+  cp_async_commit();
+
+  float o_acc[D / 8][4];
+#pragma unroll
+  for (int i = 0; i < D / 8; ++i) { o_acc[i][0] = o_acc[i][1] = o_acc[i][2] = o_acc[i][3] = 0.f; }
+  float m_i[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_i[2] = {0.f, 0.f};
+  DropState ds;  // only read when has_drop
+  if (p.has_drop) ds = drop_state(p.drop);
+  const uint32_t drow0 = (uint32_t)(((long)s * p.n_heads + h) * p.s_q + q0 + warp * 16 + g);
+
+  for (int t = 0; t < ntiles; ++t) {
+    const int kv0 = t * 64;
+    uint8_t* Ks = KVs + (t & 1) * 2 * TB;
+    uint8_t* Vs = Ks + TB;
+    if (t + 1 < ntiles) {
+      uint8_t* Kn = KVs + ((t + 1) & 1) * 2 * TB;
+      wg_load_tile<D, DIO>(Kn, Mk, kv0 + 64, skv);
+      wg_load_tile<D, DIO>(Kn + TB, Mv, kv0 + 64, skv);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    fence_proxy_async();  // cp.async / zero-fill writes -> visible to the wgmma (async proxy) reads
+    __syncthreads();
+    float sc[8][4];
+    wg_scores<D>(sc, smem_u32(Qs), smem_u32(Ks));
+    if (tile_needs_mask(p, q0 + warp * 16, kv0, skv)) apply_mask(p, sc, q0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);
+    float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+      mx[0] = fmaxf(mx[0], fmaxf(sc[nb][0], sc[nb][1]));
+      mx[1] = fmaxf(mx[1], fmaxf(sc[nb][2], sc[nb][3]));
+    }
+    float alpha[2], ms[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float mnew = fmaxf(m_i[r], mx[r]);
+      ms[r] = (mnew == -CUDART_INF_F) ? 0.f : mnew * p.scale_log2;
+      alpha[r] = exp2f(m_i[r] * p.scale_log2 - ms[r]);
+      m_i[r] = mnew;
+      l_i[r] *= alpha[r];
+    }
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float pv = exp2f(fmaf(sc[nb][e], p.scale_log2, -ms[e >> 1]));
+        sc[nb][e] = pv;
+        l_i[e >> 1] += pv;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < D / 8; ++i) {
+      o_acc[i][0] *= alpha[0]; o_acc[i][1] *= alpha[0];
+      o_acc[i][2] *= alpha[1]; o_acc[i][3] *= alpha[1];
+    }
+    if (p.has_drop) {  // O = dropout(P) V; the normaliser stays that of the undropped P (softmax, then dropout)
+#pragma unroll
+      for (int nb = 0; nb < 8; ++nb) {
+        const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
+        drop2(ds, drow0, col, sc[nb][0], sc[nb][1]);
+        drop2(ds, drow0 + 8, col, sc[nb][2], sc[nb][3]);
+      }
+    }
+    wg_pv<D>(o_acc, sc, smem_u32(Vs));
+    __syncthreads();  // every warpgroup MMA of this stage has retired before it is refilled
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_i[r] += __shfl_xor_sync(0xffffffffu, l_i[r], 1);
+    l_i[r] += __shfl_xor_sync(0xffffffffu, l_i[r], 2);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int qi = q0 + warp * 16 + g + r * 8;
+    if (qi >= sq) continue;
+    const float inv = l_i[r] > 0.f ? 1.f / l_i[r] : 0.f;
+    __nv_bfloat16* orow = p.o + rrow(mo, qi) * p.ldo + h * p.hso;
+#pragma unroll
+    for (int nb = 0; nb < DIO / 8; ++nb)
+      *reinterpret_cast<uint32_t*>(orow + nb * 8 + t4 * 2) = pack_bf16(o_acc[nb][2 * r] * inv, o_acc[nb][2 * r + 1] * inv);
+    if (p.lse && t4 == 0) p.lse[((size_t)s * p.n_heads + h) * p.s_q + qi] = m_i[r] * p.scale + logf(l_i[r]);
+  }
+}
+
+// dQ (and delta = rowsum(dO * O) for the dK / dV kernel, which runs after this one)
+template <int D, int DIO>
+__global__ void __launch_bounds__(128) attn_wg_bwd_dq_kernel(const AttnKParams p) {
+  constexpr int TB = WgTile<D>::BYTES;
+  extern __shared__ uint8_t smem_wg[];
+  uint8_t* sm = smem_wg + ((1024u - (smem_u32(smem_wg) & 1023u)) & 1023u);
+  uint8_t* Qs = sm;
+  uint8_t* dOs = sm + TB;
+  uint8_t* KVs = sm + 2 * TB;  // [stage][K|V]
+  float* stat = reinterpret_cast<float*>(sm + 6 * TB);  // lse(log2)[64], delta[64]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = blockIdx.x * 64, h = blockIdx.y, s = blockIdx.z;
+  const int g = lane >> 2, t4 = lane & 3;
+  int sq, skv;
+  eff_len(p, s, sq, skv);
+  if (q0 >= sq) return;
+  const RSeq mkv = resolve(p.mkv, s), mo = resolve(p.mo, s), mdo = resolve(p.mdo, s), mdq = resolve(p.mdq, s);
+  const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq), Mdo = rmat(p.dout, mdo, p.lddo, h * p.hsdo);
+  const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
+  int kv_end = skv;
+  if (p.mask == MASK_CAUSAL) kv_end = min(skv, q0 + 64);
+  const int ntiles = (kv_end + 63) / 64;
+
+  wg_load_tile<D, DIO>(Qs, Mq, q0, sq);
+  wg_load_tile<D, DIO>(dOs, Mdo, q0, sq);
+  wg_load_tile<D, DIO>(KVs, Mk, 0, skv);
+  wg_load_tile<D, DIO>(KVs + TB, Mv, 0, skv);
+  cp_async_commit();
+  {
+    const int r = lane >> 1, hf = lane & 1;
+    const int qi = q0 + warp * 16 + r;
+    float acc = 0.f;
+    if (qi < sq) {
+      const uint4* orow = reinterpret_cast<const uint4*>(p.o + rrow(mo, qi) * p.ldo + h * p.hso);
+      const uint4* drow = reinterpret_cast<const uint4*>(p.dout + rrow(mdo, qi) * p.lddo + h * p.hsdo);
+#pragma unroll
+      for (int c = hf; c < DIO / 8; c += 2) {
+        const uint4 a = __ldg(orow + c), b = __ldg(drow + c);
+        acc += bf16_lo(a.x) * bf16_lo(b.x) + bf16_hi(a.x) * bf16_hi(b.x) + bf16_lo(a.y) * bf16_lo(b.y) +
+               bf16_hi(a.y) * bf16_hi(b.y) + bf16_lo(a.z) * bf16_lo(b.z) + bf16_hi(a.z) * bf16_hi(b.z) +
+               bf16_lo(a.w) * bf16_lo(b.w) + bf16_hi(a.w) * bf16_hi(b.w);
+      }
+    }
+    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+    if (hf == 0) {
+      const size_t li = ((size_t)s * p.n_heads + h) * p.s_q + qi;
+      stat[64 + warp * 16 + r] = acc;
+      stat[warp * 16 + r] = (qi < sq) ? p.lse[li] * 1.4426950408889634f : CUDART_INF_F;
+      if (qi < sq) p.delta[li] = acc;
+    }
+  }
+  float dq_acc[D / 8][4];
+#pragma unroll
+  for (int i = 0; i < D / 8; ++i) { dq_acc[i][0] = dq_acc[i][1] = dq_acc[i][2] = dq_acc[i][3] = 0.f; }
+  float lse_r[2], del_r[2];
+  DropState ds;  // only read when has_drop
+  if (p.has_drop) ds = drop_state(p.drop);
+  const uint32_t drow0 = (uint32_t)(((long)s * p.n_heads + h) * p.s_q + q0 + warp * 16 + g);
+
+  for (int t = 0; t < ntiles; ++t) {
+    const int kv0 = t * 64;
+    uint8_t* Ks = KVs + (t & 1) * 2 * TB;
+    uint8_t* Vs = Ks + TB;
+    if (t + 1 < ntiles) {
+      uint8_t* Kn = KVs + ((t + 1) & 1) * 2 * TB;
+      wg_load_tile<D, DIO>(Kn, Mk, kv0 + 64, skv);
+      wg_load_tile<D, DIO>(Kn + TB, Mv, kv0 + 64, skv);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    fence_proxy_async();
+    __syncthreads();
+    if (t == 0) {
+      lse_r[0] = stat[warp * 16 + g]; lse_r[1] = stat[warp * 16 + g + 8];
+      del_r[0] = stat[64 + warp * 16 + g]; del_r[1] = stat[64 + warp * 16 + g + 8];
+    }
+    float sc[8][4], dp[8][4];
+    wg_scores<D>(sc, smem_u32(Qs), smem_u32(Ks));
+    wg_scores<D>(dp, smem_u32(dOs), smem_u32(Vs));
+    if (tile_needs_mask(p, q0 + warp * 16, kv0, skv)) apply_mask(p, sc, q0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);
+    if (p.has_drop) {  // dP = dropout'(dO V^T): the same keep bits and scale as the forward
+#pragma unroll
+      for (int nb = 0; nb < 8; ++nb) {
+        const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
+        drop2(ds, drow0, col, dp[nb][0], dp[nb][1]);
+        drop2(ds, drow0 + 8, col, dp[nb][2], dp[nb][3]);
+      }
+    }
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float pv = exp2f(fmaf(sc[nb][e], p.scale_log2, -lse_r[e >> 1]));
+        sc[nb][e] = pv * (dp[nb][e] - del_r[e >> 1]);  // dS
+      }
+    }
+    wg_pv<D>(dq_acc, sc, smem_u32(Ks));
+    __syncthreads();
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int qi = q0 + warp * 16 + g + r * 8;
+    if (qi >= sq) continue;
+    __nv_bfloat16* dqrow = p.dq + rrow(mdq, qi) * p.lddq + h * p.hsdq;
+#pragma unroll
+    for (int nb = 0; nb < DIO / 8; ++nb)
+      *reinterpret_cast<uint32_t*>(dqrow + nb * 8 + t4 * 2) = pack_bf16(dq_acc[nb][2 * r] * p.scale, dq_acc[nb][2 * r + 1] * p.scale);
+  }
+}
+
+// dK, dV: CTA = 64 key rows, streams Q / dO tiles; everything in the transposed frame (rows = keys, columns = queries)
+template <int D, int DIO>
+__global__ void __launch_bounds__(128) attn_wg_bwd_dkdv_kernel(const AttnKParams p) {
+  constexpr int TB = WgTile<D>::BYTES;
+  extern __shared__ uint8_t smem_wg[];
+  uint8_t* sm = smem_wg + ((1024u - (smem_u32(smem_wg) & 1023u)) & 1023u);
+  uint8_t* Ks = sm;
+  uint8_t* Vs = sm + TB;
+  uint8_t* QDs = sm + 2 * TB;  // [stage][Q|dO]
+  float* stat = reinterpret_cast<float*>(sm + 6 * TB);  // [stage][lse(log2) 64 | delta 64]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int kv0 = blockIdx.x * 64, h = blockIdx.y, s = blockIdx.z;
+  const int g = lane >> 2, t4 = lane & 3;
+  int sq, skv;
+  eff_len(p, s, sq, skv);
+  if (kv0 >= skv) return;
+  const RSeq mkv = resolve(p.mkv, s), mdkv = resolve(p.mdkv, s);
+  const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq), Mdo = rmat(p.dout, resolve(p.mdo, s), p.lddo, h * p.hsdo);
+  const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
+  const int q_begin = (p.mask == MASK_CAUSAL) ? kv0 : 0;  // 64-aligned
+  const int ntiles = (sq - q_begin + 63) / 64;
+  const size_t stat_base = ((size_t)s * p.n_heads + h) * p.s_q;
+
+  auto load_stage = [&](int stage, int qi0) {
+    uint8_t* Qn = QDs + stage * 2 * TB;
+    wg_load_tile<D, DIO>(Qn, Mq, qi0, sq);
+    wg_load_tile<D, DIO>(Qn + TB, Mdo, qi0, sq);
+    if (threadIdx.x < 64) {
+      const int qi = qi0 + threadIdx.x;
+      float* st = stat + stage * 128;
+      st[threadIdx.x] = (qi < sq) ? p.lse[stat_base + qi] * 1.4426950408889634f : CUDART_INF_F;
+      st[64 + threadIdx.x] = (qi < sq) ? p.delta[stat_base + qi] : 0.f;
+    }
+  };
+
+  wg_load_tile<D, DIO>(Ks, Mk, kv0, skv);
+  wg_load_tile<D, DIO>(Vs, Mv, kv0, skv);
+  load_stage(0, q_begin);
+  cp_async_commit();
+
+  float dk_acc[D / 8][4], dv_acc[D / 8][4];
+#pragma unroll
+  for (int i = 0; i < D / 8; ++i) {
+    dk_acc[i][0] = dk_acc[i][1] = dk_acc[i][2] = dk_acc[i][3] = 0.f;
+    dv_acc[i][0] = dv_acc[i][1] = dv_acc[i][2] = dv_acc[i][3] = 0.f;
+  }
+  DropState ds;  // only read when has_drop
+  if (p.has_drop) ds = drop_state(p.drop);
+  const uint32_t dbase = (uint32_t)stat_base;
+  const int k0 = kv0 + warp * 16 + g, k1 = k0 + 8;  // this thread's two key rows (elements 0, 1 and 2, 3)
+
+  for (int t = 0; t < ntiles; ++t) {
+    const int qi0 = q_begin + t * 64;
+    uint8_t* Qs = QDs + (t & 1) * 2 * TB;
+    uint8_t* dOs = Qs + TB;
+    const float* st = stat + (t & 1) * 128;
+    if (t + 1 < ntiles) {
+      load_stage((t + 1) & 1, qi0 + 64);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    fence_proxy_async();
+    __syncthreads();
+    float st_[8][4], dpt[8][4];
+    wg_scores<D>(st_, smem_u32(Ks), smem_u32(Qs));   // S^T = K Q^T
+    wg_scores<D>(dpt, smem_u32(Vs), smem_u32(dOs));  // dZ^T = V dO^T
+    {
+      const int k_lo = kv0 + warp * 16;
+      const bool need = (k_lo + 16 > skv) || (p.mask == MASK_CAUSAL && k_lo + 15 > qi0);
+      if (need) {
+#pragma unroll
+        for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int qc = qi0 + nb * 8 + t4 * 2 + e;
+            bool m0 = k0 >= skv, m1 = k1 >= skv;
+            if (p.mask == MASK_CAUSAL) { m0 |= k0 > qc; m1 |= k1 > qc; }
+            if (m0) st_[nb][e] = -CUDART_INF_F;
+            if (m1) st_[nb][2 + e] = -CUDART_INF_F;
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+      // dropout keep bits of the four (query, key) pairs this thread holds, bit e for element e: queries q, q + 1 and keys
+      // k0, k1 = k0 + 8.  The four lanes g = 4a .. 4a+3 (same t4) need the same four Philox calls (rows q / q + 1, key
+      // groups of k0 / k1), each a different word of them: lane j = g & 3 makes call j and the words are exchanged.
+      uint32_t keep = 0xFu;
+      if (p.has_drop) {
+        const int j = g & 3;
+        const uint32_t qr = dbase + (uint32_t)(qi0 + nb * 8 + t4 * 2 + (j & 1));
+        const uint4 w = drop_words(ds, qr, (uint32_t)(kv0 + warp * 16 + (g & ~3) + (j >> 1) * 8) >> 2);
+        keep = 0;
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int comp = (j + r) & 3, c = (j - r) & 3;  // send word comp, receive call c's word j
+          const uint32_t v = comp == 0 ? w.x : comp == 1 ? w.y : comp == 2 ? w.z : w.w;
+          const uint32_t got = __shfl_sync(0xffffffffu, v, (lane & ~0xC) | (c << 2));
+          keep |= (got >= ds.thresh ? 1u : 0u) << c;
+        }
+      }
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int ql = nb * 8 + t4 * 2 + (e & 1);
+        const float pv = exp2f(fmaf(st_[nb][e], p.scale_log2, -st[ql]));  // lse=+inf for absent queries -> 0
+        float dz = dpt[nb][e];
+        if (p.has_drop) {  // Z = dropout(P): dV += Z^T dO, dP = dropout'(dZ)
+          const float kf = (keep >> e) & 1u ? ds.scale : 0.f;
+          dz *= kf;
+          st_[nb][e] = pv * kf;  // Z^T
+        } else {
+          st_[nb][e] = pv;       // P^T
+        }
+        dpt[nb][e] = pv * (dz - st[64 + ql]);  // dS^T
+      }
+    }
+    wg_pv<D>(dv_acc, st_, smem_u32(dOs));
+    wg_pv<D>(dk_acc, dpt, smem_u32(Qs));
+    __syncthreads();
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int kvr = kv0 + warp * 16 + g + r * 8;
+    if (kvr >= skv) continue;
+    const long row = rrow(mdkv, kvr);
+    __nv_bfloat16* dkrow = p.dk + row * p.lddk + h * p.hsdk;
+    __nv_bfloat16* dvrow = p.dv + row * p.lddv + h * p.hsdv;
+#pragma unroll
+    for (int nb = 0; nb < DIO / 8; ++nb) {
+      *reinterpret_cast<uint32_t*>(dkrow + nb * 8 + t4 * 2) = pack_bf16(dk_acc[nb][2 * r] * p.scale, dk_acc[nb][2 * r + 1] * p.scale);
       *reinterpret_cast<uint32_t*>(dvrow + nb * 8 + t4 * 2) = pack_bf16(dv_acc[nb][2 * r], dv_acc[nb][2 * r + 1]);
     }
   }
@@ -789,6 +1276,30 @@ static int launch_decode(const AttnKParams& p, cudaStream_t st) {
   return YMP_OK;
 }
 
+template <int D, int DIO = D>
+static int launch_wg_fwd(const AttnKParams& p, cudaStream_t st) {
+  const int smem = 5 * WgTile<D>::BYTES + 1024;
+  static DeviceOnce once;
+  if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(attn_wg_fwd_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
+  launch_k(attn_wg_fwd_kernel<D, DIO>, dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), dim3(128), smem, st, p);
+  YMP_LAUNCH_CHECK();
+  return YMP_OK;
+}
+template <int D, int DIO = D>
+static int launch_wg_bwd(const AttnKParams& p, cudaStream_t st) {
+  const int smem = 6 * WgTile<D>::BYTES + 1024 + 1024;
+  static DeviceOnce once;
+  if (once.first()) {
+    YMP_CUDA(cudaFuncSetAttribute(attn_wg_bwd_dq_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    YMP_CUDA(cudaFuncSetAttribute(attn_wg_bwd_dkdv_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  }
+  attn_wg_bwd_dq_kernel<D, DIO><<<dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
+  YMP_LAUNCH_CHECK();
+  attn_wg_bwd_dkdv_kernel<D, DIO><<<dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
+  YMP_LAUNCH_CHECK();
+  return YMP_OK;
+}
+
 static int fill_params(const ymp_attn_args* a, AttnKParams& p, const char* who) {
   YMP_CHECK_ARG(a && a->q && a->k && a->v, "%s: null q/k/v", who);
   YMP_CHECK_ARG(a->head_dim == 64 || a->head_dim == 80 || a->head_dim == 88 || a->head_dim == 96 || a->head_dim == 128,
@@ -811,30 +1322,32 @@ static int fill_params(const ymp_attn_args* a, AttnKParams& p, const char* who) 
   p.mask = a->mask; p.mask_block = a->mask_block > 0 ? a->mask_block : 1; p.total_rows = a->total_rows;
   p.scale = a->scale; p.scale_log2 = a->scale * 1.4426950408889634f;
   p.skv_dev = a->s_kv_dev;
+  p.has_drop = (a->drop.rng && a->drop.p > 0.f) ? 1 : 0;
+  p.drop.rng = (const uint64_t*)a->drop.rng; p.drop.site = a->drop.site; p.drop.p = a->drop.p;
   return YMP_OK;
 }
 
-template <int D>
+template <int D, int DIO = D>
 static int launch_fwd(const AttnKParams& p, cudaStream_t st) {
   const int smem = 5 * 64 * (D + 8) * 2;
   static DeviceOnce once;
-  if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
+  if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
   dim3 grid((p.s_q + 63) / 64, p.n_heads, p.n_seq);
-  launch_k(attn_fwd_kernel<D>, grid, dim3(128), smem, st, p);
+  launch_k(attn_fwd_kernel<D, DIO>, grid, dim3(128), smem, st, p);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }
-template <int D>
+template <int D, int DIO = D>
 static int launch_bwd(const AttnKParams& p, cudaStream_t st) {
   const int smem = 6 * 64 * (D + 8) * 2 + 1024;
   static DeviceOnce once;
   if (once.first()) {
-    YMP_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    YMP_CUDA(cudaFuncSetAttribute(attn_bwd_dkdv_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    YMP_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    YMP_CUDA(cudaFuncSetAttribute(attn_bwd_dkdv_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   }
-  attn_bwd_dq_kernel<D><<<dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
+  attn_bwd_dq_kernel<D, DIO><<<dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
   YMP_LAUNCH_CHECK();
-  attn_bwd_dkdv_kernel<D><<<dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
+  attn_bwd_dkdv_kernel<D, DIO><<<dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }
@@ -842,8 +1355,6 @@ static int launch_bwd(const AttnKParams& p, cudaStream_t st) {
 }  // namespace ymp
 
 namespace ymp {
-int attn_tc_fwd_try(const ymp_attn_args* a, cudaStream_t st);
-int attn_tc_bwd_try(const ymp_attn_bwd_args* b, cudaStream_t st);
 int attn_small_fwd_try(const ymp_attn_args* a, cudaStream_t st);
 int attn_small_bwd_try(const ymp_attn_bwd_args* b, cudaStream_t st);
 }
@@ -858,11 +1369,9 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   if (rc) return rc;
   YMP_CHECK_ARG(a->o && aligned16(a->o), "ymp_attn_fwd: bad o");
   cudaStream_t st = (cudaStream_t)stream;
-  // short key ranges run on the tcgen05 kernel (attention_tc.cu); YMP_ATTN_LEGACY=1 forces mma.sync
-  static const bool legacy = [] { const char* e = getenv("YMP_ATTN_LEGACY"); return e && e[0] == '1'; }();
-  const bool dropped = a->drop.rng && a->drop.p > 0.f;
+  const bool dropped = p.has_drop;
   YMP_CHECK_ARG(!dropped || a->drop.p < 1.f, "ymp_attn_fwd: dropout p must be < 1");
-  if (a->s_q == 1 && a->mask == YMP_MASK_NONE && a->total_rows == 0 && !dropped && a->head_dim != 88 && a->head_dim != 128 && !legacy) {
+  if (a->s_q == 1 && a->mask == YMP_MASK_NONE && a->total_rows == 0 && !dropped && a->head_dim != 88 && a->head_dim != 128) {
     g_attn_path = YMP_ATTN_PATH_DECODE;   // one query row per sequence: the streaming kernel (also follows s_kv_dev)
     switch (a->head_dim) {
       case 64: return launch_decode<64>(p, st);
@@ -873,20 +1382,26 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   const bool dev_len = a->s_kv_dev != nullptr;  // key count read on the device: the mma.sync kernels bound their KV loop by it
   YMP_CHECK_ARG(!dev_len || (!dropped && a->mask == YMP_MASK_NONE && a->total_rows == 0 && a->head_dim != 88),
                 "ymp_attn_fwd: s_kv_dev needs mask none, no dropout, no total_rows, head_dim in {64,80,96,128}");
-  if ((!legacy || dropped) && !dev_len) {
-    if (!dropped) {
-      rc = attn_small_fwd_try(a, st);  // short dense block-diagonal sequences (attention_small.cu)
-      if (rc != YMP_ENOSUP) { g_attn_path = YMP_ATTN_PATH_SMALL; return rc; }
-    }
-    rc = attn_tc_fwd_try(a, st);
-    if (rc != YMP_ENOSUP) { g_attn_path = YMP_ATTN_PATH_TCGEN05; return rc; }
+  if (!dropped && !dev_len) {
+    rc = attn_small_fwd_try(a, st);  // short dense block-diagonal sequences (attention_small.cu)
+    if (rc != YMP_ENOSUP) { g_attn_path = YMP_ATTN_PATH_SMALL; return rc; }
   }
-  if (dropped) return set_error(YMP_ENOSUP, "ymp_attn_fwd: dropout of the probabilities is implemented by the tcgen05 kernels only");
+  // warpgroup-MMA tiles for head_dim <= 96; the mma.sync tiles for head_dim 128, the packed block-diagonal mask (they
+  // skip the masked chunks warp by warp), the device-side key count and a few query rows against a long cache
+  if (a->head_dim != 128 && a->mask != YMP_MASK_BLOCK && !dev_len && !(a->s_q < 16 && a->s_kv > 256)) {
+    g_attn_path = YMP_ATTN_PATH_WGMMA;
+    switch (a->head_dim) {
+      case 64: return launch_wg_fwd<64>(p, st);
+      case 80: return launch_wg_fwd<80>(p, st);
+      case 88: return launch_wg_fwd<96, 88>(p, st);
+      default: return launch_wg_fwd<96>(p, st);
+    }
+  }
   g_attn_path = YMP_ATTN_PATH_MMA_SYNC;
-  if (a->head_dim == 88) return set_error(YMP_ENOSUP, "ymp_attn_fwd: head_dim 88 is served by the tcgen05 kernels only (dense or cross attention, s_q >= 16)");
   switch (a->head_dim) {
     case 64: return launch_fwd<64>(p, st);
     case 80: return launch_fwd<80>(p, st);
+    case 88: return launch_fwd<96, 88>(p, st);
     case 96: return launch_fwd<96>(p, st);
     default: return launch_fwd<128>(p, st);
   }
@@ -902,6 +1417,7 @@ extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {
   YMP_CHECK_ARG(a->o && a->lse && b->dout && b->dq && b->dk && b->dv && b->delta_ws, "ymp_attn_bwd: null o/lse/dout/dq/dk/dv/delta_ws");
   YMP_CHECK_ARG(b->lddo % 8 == 0 && b->lddq % 8 == 0 && b->lddk % 8 == 0 && b->lddv % 8 == 0, "ymp_attn_bwd: grad row strides must be multiples of 8");
   YMP_CHECK_ARG(!a->s_kv_dev, "ymp_attn_bwd: s_kv_dev is forward only");
+  YMP_CHECK_ARG(!p.has_drop || a->drop.p < 1.f, "ymp_attn_bwd: dropout p must be < 1");
   p.dout = (const __nv_bfloat16*)b->dout; p.dq = (__nv_bfloat16*)b->dq; p.dk = (__nv_bfloat16*)b->dk; p.dv = (__nv_bfloat16*)b->dv;
   p.delta = b->delta_ws;
   p.lddo = b->lddo; p.hsdo = b->do_head_stride;
@@ -909,22 +1425,24 @@ extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {
   p.hsdq = b->dq_head_stride; p.hsdk = b->dk_head_stride; p.hsdv = b->dv_head_stride;
   p.mdo = to_map(b->map_do); p.mdq = to_map(b->map_dq); p.mdkv = to_map(b->map_dkv);
   cudaStream_t st = (cudaStream_t)stream;
-  static const bool legacy = [] { const char* e = getenv("YMP_ATTN_LEGACY"); return e && e[0] == '1'; }();
-  const bool dropped = a->drop.rng && a->drop.p > 0.f;
-  if (!legacy || dropped) {
-    if (!dropped) {
-      rc = attn_small_bwd_try(b, st);
-      if (rc != YMP_ENOSUP) { g_attn_path = YMP_ATTN_PATH_SMALL; return rc; }
-    }
-    rc = attn_tc_bwd_try(b, st);
-    if (rc != YMP_ENOSUP) { g_attn_path = YMP_ATTN_PATH_TCGEN05; return rc; }
+  if (!p.has_drop) {
+    rc = attn_small_bwd_try(b, st);
+    if (rc != YMP_ENOSUP) { g_attn_path = YMP_ATTN_PATH_SMALL; return rc; }
   }
-  if (dropped) return set_error(YMP_ENOSUP, "ymp_attn_bwd: dropout of the probabilities is implemented by the tcgen05 kernels only");
+  if (a->head_dim != 128 && a->mask != YMP_MASK_BLOCK) {
+    g_attn_path = YMP_ATTN_PATH_WGMMA;
+    switch (a->head_dim) {
+      case 64: return launch_wg_bwd<64>(p, st);
+      case 80: return launch_wg_bwd<80>(p, st);
+      case 88: return launch_wg_bwd<96, 88>(p, st);
+      default: return launch_wg_bwd<96>(p, st);
+    }
+  }
   g_attn_path = YMP_ATTN_PATH_MMA_SYNC;
-  if (a->head_dim == 88) return set_error(YMP_ENOSUP, "ymp_attn_bwd: head_dim 88 is served by the tcgen05 kernels only");
   switch (a->head_dim) {
     case 64: return launch_bwd<64>(p, st);
     case 80: return launch_bwd<80>(p, st);
+    case 88: return launch_bwd<96, 88>(p, st);
     case 96: return launch_bwd<96>(p, st);
     default: return launch_bwd<128>(p, st);
   }

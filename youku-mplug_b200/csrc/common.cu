@@ -19,11 +19,11 @@ int set_error(int code, const char* fmt, ...) {
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached[dev] = n;
   }
   return cached[dev];

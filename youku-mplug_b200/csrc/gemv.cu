@@ -1,7 +1,7 @@
 // Skinny GEMM for single-token decoding (SURVEY.md 8f N2): y[M, N] = epilogue(x[M, K] . w[N, K]^T) with M <= 8 rows
 // (beam width / decode batch).  Replaces the GPT-3 layer's linears at the KV-cache step of
 // models/modeling_distributed_gpt3.py:868-938,580-595,1348-1350.  With a handful of rows the work is one pass over
-// the weight matrix: HBM-bound.  A 128-row tcgen05 tile would occupy N/128 CTAs (16 for N = 2048) and stream the
+// the weight matrix: HBM-bound.  A 128-row tensor-core tile would occupy N/128 CTAs (16 for N = 2048) and stream the
 // weights at a fraction of the memory bandwidth; a CUDA-core dot product needs ~2.5 issue slots per weight byte-pair
 // (bf16 -> fp32 converts + FMAs for every row) and is issue-bound at a quarter of the bandwidth.  So:
 //   * a warp owns 8 output columns and one K slice and feeds mma.sync.m16n8k16 (bf16, fp32 accumulate) STRAIGHT FROM
@@ -244,7 +244,7 @@ extern "C" int ymp_gemm_skinny(const ymp_gemm_skinny_args* a, void* stream) {
   // K slices per CTA (the warps of a CTA that share one 8-column tile): as many as leave >= 4 k-blocks of 32 per slice
   int ks = 1;
   static const int force = [] { const char* e = getenv("YMP_SKINNY_KSPLIT"); return e ? atoi(e) : 0; }();
-  const int ks_max = a->N <= 4096 ? 8 : 4;   // measured (tools/skinny_probe.py): wide outputs prefer fatter CTAs
+  const int ks_max = a->N <= 4096 ? 8 : 4;   // wide outputs get fewer K slices per CTA (more column tiles)
   while (ks < ks_max && a->K / (2 * ks) >= 128) ks *= 2;
   if (force == 1 || force == 2 || force == 4 || force == 8) ks = force;
   p.ksplit = ks;

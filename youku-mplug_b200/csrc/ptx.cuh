@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA/TMEM).
-// Everything here is architecture-specific on purpose: this library targets B200 only.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors and fences.
+// Everything here is architecture-specific on purpose: this library targets H100 only.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -82,154 +82,27 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const void* desc, ui
         "r"(c3), "r"(c4)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_5d_cta2(void* smem_dst, const void* desc, uint64_t* bar, int32_t c0, int32_t c1,
-                                                 int32_t c2, int32_t c3, int32_t c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1),
-        "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the accumulator registers ordered against the asynchronous wgmma that reads / writes them
+template <int N>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 x bf16 -> fp32
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <- lane base+i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor (sm_100 "version 1"), SWIZZLE_128B.
-//   start address [0,14) >>4 | LBO [16,30) >>4 | SBO [32,46) >>4 | version=1 [46,48) | layout [61,64)=2
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
+// Shared-memory matrix descriptor of wgmma (sm_90):
+//   start address [0,14) >>4 | LBO [16,30) >>4 | SBO [32,46) >>4 | layout [62,64): 1 = SWIZZLE_128B, 3 = SWIZZLE_32B
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)layout << 62;
   return d;
-}
-
-// Instruction descriptor for kind::f16, bf16 inputs, fp32 accumulate.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major,
-                                                       int b_mn_major) {
-  return (1u << 4)                       // c_format = F32
-         | (1u << 7)                     // a_format = BF16
-         | (1u << 10)                    // b_format = BF16
-         | ((uint32_t)a_mn_major << 15)  // a_major
-         | ((uint32_t)b_mn_major << 16)  // b_major
-         | ((uint32_t)(N >> 3) << 17)    // n_dim
-         | ((uint32_t)(M >> 4) << 24);   // m_dim
-}
-
-// ---------------------------------------------------------------- 2-CTA (cta_group::2) variants
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load issued by either CTA of a pair; the bytes are accounted on the LEADER CTA's mbarrier
-// (peer bit of the shared::cluster address cleared), where the single MMA issuer waits.
-__device__ __forceinline__ void tma_load_2d_cta2(void* smem_dst, const void* desc, uint64_t* bar, int32_t c0,
-                                                 int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar) & 0xFEFFFFFFu),
-        "r"(c0), "r"(c1)
-      : "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc_cta2(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc_cta2(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-// D[tmem of both CTAs, 256 x N] (+)= A (128 rows per CTA) * B (N/2 rows per CTA); issued by the leader
-__device__ __forceinline__ void umma_bf16_cta2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of the pair's MMAs -> arrive on the mbarrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_cta2(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-// arrive on the mbarrier at this offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  uint32_t raddr;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(bar)), "r"(rank));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
 }
 
 // ---------------------------------------------------------------- small math helpers
@@ -292,27 +165,12 @@ __device__ __forceinline__ float gelu_erf(float x) {
   float e;
   return x * norm_cdf_pdf(x, e);
 }
-// ---- packed fp32 pairs (Blackwell FFMA2 / FMUL2 / FADD2: one issue slot for two IEEE operations, bit-identical to the
-// scalar instructions).  The GEMM epilogues are issue-slot / dependency-latency bound on the activation polynomials.
+// ---- fp32 pairs: two scalar IEEE operations each.  The GEMM epilogues are issue-slot / dependency-latency bound on the
+// activation polynomials; the x8 helpers below interleave four independent chains.
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra, rb, rc, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  unsigned long long ra, rb, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
-}
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 splat2(float c) { return make_float2(c, c); }
 
 // Phi and the normal pdf of EIGHT values in lockstep (four packed pairs): the same arithmetic as norm_cdf_pdf, element

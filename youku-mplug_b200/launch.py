@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Run one of the reference's scripts UNMODIFIED on the B200 `models` package.
+"""Run one of the reference's scripts UNMODIFIED on the H100 `models` package.
 
     python youku-mplug_b200/launch.py /path/to/Youku-mPLUG/run_pretrain_distributed_gpt3.py \
         --config configs/pretrain/gpt3_1.3B/pretrain_gpt3_freezeGPT_youku_v0.yaml --output_dir out \
@@ -7,7 +7,7 @@
     python -m torch.distributed.run --nproc-per-node 8 youku-mplug_b200/launch.py <script> <args ...>
 
 What it does before handing control to the script (runpy, `__main__`):
-  1. puts this directory first on sys.path and imports the B200 `models` package, then appends the reference's own
+  1. puts this directory first on sys.path and imports the H100 `models` package, then appends the reference's own
      `models/` directory to `models.__path__`: `models.distributed_gpt3`, `models.modeling_distributed_gpt3`,
      `models.vision_transformer`, `models.distributed_utils`, `models.model_pretrain_gpt` resolve HERE, every other
      submodule the scripts' imports pull in (`models.tokenization_bert` via `dataset/grounding_dataset.py:28`,
@@ -17,7 +17,7 @@ What it does before handing control to the script (runpy, `__main__`):
      `scheduler`;
   3. appends `compat/` (stand-ins for deepspeed / megatron_util / ruamel.yaml / timm / addict / sh / tensorboardX /
      decord, see compat/README.md) to the END of sys.path so that really installed packages win - except
-     `deepspeed`, whose `initialize()` must return the B200 engine (set YMP_KEEP_DEEPSPEED=1 to keep a real one);
+     `deepspeed`, whose `initialize()` must return the H100 engine (set YMP_KEEP_DEEPSPEED=1 to keep a real one);
   4. restores three private helpers transformers 5.x removed and the reference's BERT tokenizer imports
      (models/tokenization_bert.py:23);
   5. optional `--ymp-pre FILE`: a Python file executed first (site-specific hooks, e.g. registering a dataset).
@@ -77,7 +77,7 @@ def prepare(script, need_reference=True):
     for name, fn in (("_is_whitespace", _is_whitespace), ("_is_control", _is_control), ("_is_punctuation", _is_punctuation)):
         if not hasattr(tu, name):
             setattr(tu, name, fn)
-    import models  # the B200 package (HERE is first on sys.path)
+    import models  # the H100 package (HERE is first on sys.path)
     assert os.path.dirname(os.path.abspath(models.__file__)) == os.path.join(HERE, "models"), models.__file__
     if ref:
         ref_models = os.path.join(ref, "models")

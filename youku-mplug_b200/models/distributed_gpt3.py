@@ -1,4 +1,4 @@
-"""mPLUG-Video task models on the B200 kernels - drop-in for the reference `models/distributed_gpt3.py`.
+"""mPLUG-Video task models on the H100 kernels - drop-in for the reference `models/distributed_gpt3.py`.
 
 DistributedGPT3_Pretrain (:31-226) is the hot path: TimeSformer -> AttentionPool abstractor ->
 visual_fc -> frozen GPT-3 causal decoder over [visual prefix | text] -> masked token CE.  Same
@@ -22,7 +22,7 @@ from .vision_transformer import AttentionPool, LayerNormWithForceFP32, TimeSform
 
 
 class _Linear(nn.Linear):
-    """nn.Linear whose forward runs on the tcgen05 GEMM (same parameters / state_dict keys)."""
+    """nn.Linear whose forward runs on the wgmma GEMM (same parameters / state_dict keys)."""
 
     def forward(self, x):
         return YF.LinearFn.apply(x, self.weight, self.bias)
@@ -186,7 +186,7 @@ class DistributedGPT3_Pretrain(_PrefixModelBase):
         vision_feats_all = all_gather_cat(vision_feats) if dist_on else vision_feats   # [B*W, Q, E]
         text_feat_all = all_gather_cat(text_feat) if dist_on else text_feat            # [B*W, E]
         # sim_q2t[b, j, q] = <vision_feats[b,q], text_all[j]> ; max over queries (:186-202).  Both contractions
-        # run on the tcgen05 GEMM (bf16 operands like the reference's bf16 module, fp32 accumulation / output).
+        # run on the wgmma GEMM (bf16 operands like the reference's bf16 module, fp32 accumulation / output).
         Bv, Qv, E = vision_feats.shape
         J = text_feat_all.shape[0]
         sim_i2t = YF.matmul_nt(vision_feats.reshape(Bv * Qv, E), text_feat_all).view(Bv, Qv, J).max(1)[0] / self.temp
@@ -208,7 +208,7 @@ class DistributedGPT3_Pretrain_Image(_PrefixModelBase):
         super().__init__()
         from . import eva_vit
         if not config.get('use_eva_g', False):
-            raise NotImplementedError("DistributedGPT3_Pretrain_Image on the B200 path implements the EVA-g encoder (use_eva_g: true)")
+            raise NotImplementedError("DistributedGPT3_Pretrain_Image on the H100 path implements the EVA-g encoder (use_eva_g: true)")
         self.tokenizer = tokenizer
         with open(config['visual_cfg'], 'r') as f:
             visual_cfg = json.load(f)

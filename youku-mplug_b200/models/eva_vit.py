@@ -1,4 +1,4 @@
-"""EVA image encoder on the B200 kernels - mirrors the classes of the reference `models/eva_vit.py` that
+"""EVA image encoder on the H100 kernels - mirrors the classes of the reference `models/eva_vit.py` that
 `DistributedGPT3_Pretrain_Image` uses (SURVEY.md 8f N3): VisionTransformer (:245-350), create_eva_vit_g (:413-436:
 224 px, 14 x 14 patches, 1408 wide, 40 blocks, 16 heads of 88, mlp 4.3637), interpolate_pos_embed (:372-392).
 Parameter names follow the reference (`blocks.{i}.attn.{q_bias,v_bias,qkv.weight,proj.*}`, `patch_embed.proj.*`, ...),
@@ -21,11 +21,11 @@ class VisionTransformer(nn.Module):
                  use_shared_rel_pos_bias=False, use_mean_pooling=True, init_scale=0.001, use_checkpoint=False):
         super().__init__()
         if use_rel_pos_bias or use_shared_rel_pos_bias or not use_abs_pos_emb or (init_values is not None and init_values > 0):
-            raise NotImplementedError("EVA encoder on the B200 path: absolute position embeddings, no layer scale")
+            raise NotImplementedError("EVA encoder on the H100 path: absolute position embeddings, no layer scale")
         if not qkv_bias or use_mean_pooling or in_chans != 3 or drop_rate or attn_drop_rate:
-            raise NotImplementedError("EVA encoder on the B200 path: qkv_bias=True, use_mean_pooling=False, no dropout")
+            raise NotImplementedError("EVA encoder on the H100 path: qkv_bias=True, use_mean_pooling=False, no dropout")
         if drop_path_rate:
-            raise NotImplementedError("stochastic depth (drop_path > 0) is not implemented on the B200 path")
+            raise NotImplementedError("stochastic depth (drop_path > 0) is not implemented on the H100 path")
         self.image_size, self.num_features, self.embed_dim = img_size, embed_dim, embed_dim
         eps = 1e-5
         if norm_layer is not None:

@@ -1,4 +1,4 @@
-"""GPT-3 (1.3B / 2.7B Megatron-style) decoder of mPLUG-Video on the B200 kernels.
+"""GPT-3 (1.3B / 2.7B Megatron-style) decoder of mPLUG-Video on the H100 kernels.
 
 Mirrors the reference module `models/modeling_distributed_gpt3.py`: GPT3Config (:459-547),
 BatchEncoding (:139-178), DistributedGPT3Tokenizer (:180-319), DistributedGPT3 (:1522-1618).
@@ -71,7 +71,7 @@ class GPT3Config:
         for k, v in kwargs.items():
             setattr(self, k, v)
         if apply_residual_connection_post_layernorm or sequence_parallel or fp32_residual_connection:
-            raise NotImplementedError("unsupported GPT3Config option for the B200 path")
+            raise NotImplementedError("unsupported GPT3Config option for the H100 path")
 
     @classmethod
     def from_json_file(cls, path):
@@ -258,7 +258,7 @@ def _check_tp1(megatron_cfg):
     for k in ('tensor_model_parallel_size', 'model_parallel_size'):
         v = megatron_cfg.get(k, 1)
         if v not in (None, 1):
-            raise ValueError(f"megatron_cfg.{k}={v}: the B200 path is pure data parallel; set it to 1 "
+            raise ValueError(f"megatron_cfg.{k}={v}: the H100 path is pure data parallel; set it to 1 "
                              "(as the reference's own scripts/*.sh:13-14 and retrieval yaml do)")
 
 
@@ -529,7 +529,7 @@ class DistributedGPT3(nn.Module):
         if tokens is None and input_embeds is None:
             raise ValueError("You have to specify either decoder_input_ids or decoder_inputs_embeds")
         if position_ids is not None:
-            raise NotImplementedError("custom position_ids are not supported on the B200 path")
+            raise NotImplementedError("custom position_ids are not supported on the H100 path")
         if tokens is not None:
             input_embeds = self.dist_model.language_model.embedding.word_embeddings(tokens)
         if query_embeds is not None:

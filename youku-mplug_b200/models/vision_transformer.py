@@ -1,4 +1,4 @@
-"""TimeSformer video encoder + AttentionPool visual abstractor on the B200 kernels.
+"""TimeSformer video encoder + AttentionPool visual abstractor on the H100 kernels.
 
 Mirrors the reference module `models/vision_transformer.py` for the classes the GPT-3 path uses:
 TimeSformer (:440-592), AttentionPool (:341-374), LayerNormWithForceFP32 (:43-75),
@@ -59,9 +59,9 @@ class TimeSformer(nn.Module):
         if use_rel_pos_bias or use_shared_rel_pos_bias or not use_abs_pos_emb:
             raise NotImplementedError("only absolute position embeddings are supported (all shipped configs)")
         if not qkv_bias or postnorm or stop_grad_conv1 or in_chans != 3:
-            raise NotImplementedError("unsupported TimeSformer option for the B200 path")
+            raise NotImplementedError("unsupported TimeSformer option for the H100 path")
         if init_values:  # layer scale (gamma_1 / gamma_2): no shipped config sets it
-            raise NotImplementedError("layer_scale_init_value > 0 is not supported on the B200 path")
+            raise NotImplementedError("layer_scale_init_value > 0 is not supported on the H100 path")
         # drop_path_rate is accepted and has no effect, exactly like the reference: Block.forward
         # (models/vision_transformer.py:243-275) never applies self.drop_path.
         self.num_features = self.embed_dim = embed_dim
@@ -111,7 +111,7 @@ class AttentionPool(nn.Module):
                  attn_head_dim=None, postnorm=False, kdim=None):
         super().__init__()
         if kdim not in (None, dim) or not qkv_bias or (init_values is not None and init_values > 0) or postnorm:
-            raise NotImplementedError("unsupported AttentionPool option for the B200 path")
+            raise NotImplementedError("unsupported AttentionPool option for the H100 path")
         self.dim, self.num_heads = dim, num_heads
         hid = int(dim * mlp_ratio)
         for nm in ("norm1", "normk", "norm2"):
@@ -138,7 +138,7 @@ class AttentionPool(nn.Module):
         every sample holds the same query block (checked), anything else raises."""
         if queries_param is None:
             if x.shape[0] > 1 and not bool((x == x[:1]).all()):
-                raise NotImplementedError("AttentionPool on the B200 path needs one query block shared by all samples "
+                raise NotImplementedError("AttentionPool on the H100 path needs one query block shared by all samples "
                                           "(learnable_queries.repeat(B,1,1), models/distributed_gpt3.py:134)")
             queries_param = x[:1]
         keys, params = named_param_list(self, "attn_pool.")

@@ -691,8 +691,8 @@ class TokenStep:
     def body(self):
         """Enqueue the step on the current stream (eagerly or under capture): reads emb_in, returns (hid, logits).
         YMP_DECODE_PDL=1 chains the kernels by programmatic dependent launch (each may start - and the GEMMs already
-        stream their first weights - while the previous one drains).  Off by default: measured SLOWER inside the
-        captured graph on B200 (1.63 vs 1.47 ms per token at 1.3B / beam 5, profiles/r02l_pdl.log)."""
+        stream their first weights - while the previous one drains).  Off by default: inside the captured graph it
+        has not been shown to help."""
         import os
         prev = L.set_pdl(os.environ.get("YMP_DECODE_PDL", "0") == "1")
         try:
@@ -710,9 +710,8 @@ class TokenStep:
 
         import os
         # YMP_DECODE_FUSED_LN=1: every LayerNorm but the first is computed by the last CTA of the GEMM that completes its
-        # input (one kernel boundary less per sub-layer).  Off by default: measured neutral on B200 (captured step 1.466
-        # vs 1.438 ms, profiles/r02p_decode_ab.log) - the ticket + three L2 round trips of the tail cost what the
-        # stand-alone kernel and its launch gap cost.
+        # input (one kernel boundary less per sub-layer).  Off by default: the ticket + three L2 round trips of the tail
+        # cost about what the stand-alone kernel and its launch gap cost.
         fused_ln = os.environ.get("YMP_DECODE_FUSED_LN", "0") == "1"
 
         def ln_of(prefix):

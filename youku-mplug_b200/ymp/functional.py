@@ -32,7 +32,7 @@ def as_bf16(p):
 
 def _require_cuda(t, what):
     if not t.is_cuda:
-        raise RuntimeError(f"{what}: the B200 kernels need CUDA tensors (got {t.device}); there is no CPU fallback")
+        raise RuntimeError(f"{what}: the H100 kernels need CUDA tensors (got {t.device}); there is no CPU fallback")
 
 
 _SINK = None
@@ -294,7 +294,7 @@ def _padded_cols(t, dtype=bf16):
 
 
 class LinearFn(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 GEMM (visual_fc, projection heads, cls_head layers).  Any out_features:
+    """y = x W^T + b on the wgmma GEMM (visual_fc, projection heads, cls_head layers).  Any out_features:
     outputs narrower than / not a multiple of 8 columns (the 2 / 5 / 45-way classifier heads) are written
     into a row-padded buffer and returned as a view."""
 
@@ -345,7 +345,7 @@ class LinearFn(torch.autograd.Function):
 
 
 class MatmulNTFn(torch.autograd.Function):
-    """s = x @ y^T in fp32 from bf16 operands on the tcgen05 GEMM, with both gradients: the similarity
+    """s = x @ y^T in fp32 from bf16 operands on the wgmma GEMM, with both gradients: the similarity
     contractions of the contrastive branches (models/distributed_gpt3.py:186-202, :957-958)."""
 
     @staticmethod

@@ -154,7 +154,7 @@ lib.ymp_launch_count.restype = C.c_uint64
 lib.ymp_attn_last_path.restype = C.c_int
 lib.ymp_set_pdl.restype = C.c_int
 lib.ymp_set_pdl.argtypes = [C.c_int]
-ATTN_PATH_MMA_SYNC, ATTN_PATH_TCGEN05, ATTN_PATH_SMALL, ATTN_PATH_DECODE = 0, 1, 2, 3
+ATTN_PATH_MMA_SYNC, ATTN_PATH_WGMMA, ATTN_PATH_SMALL, ATTN_PATH_DECODE = 0, 1, 2, 3
 
 
 def _declare(name, argstruct):

@@ -1,6 +1,6 @@
 """Data-parallel training engine for the drop-in models: the part of `deepspeed.initialize(...)`
 the reference scripts rely on (run_pretrain_distributed_gpt3.py:257-267,134-138; utils.py:483-562),
-rebuilt for one-process-per-GPU B200 training.
+rebuilt for one-process-per-GPU H100 training.
 
   engine = TrainEngine(model, optimizer_params, lr=..., betas=..., eps=..., clip_grad=...)
   loss, _ = engine(video, text); engine.backward(loss); engine.step()
