@@ -1,7 +1,7 @@
 // Warp-specialised bf16 GEMM for sm_90a (one 128 x BN output tile per CTA, BN = 128 or 256).
 //   warpgroup 0   : TMA producer   (cp.async.bulk.tensor 2D / 5D, SWIZZLE_128B, NSTAGE-deep mbarrier ring)
 //   warpgroups 1-2: consumers      (wgmma.mma_async m64 x BN x 16 each, fp32 accumulators in registers), then the
-//                   epilogue: accumulators staged through shared memory -> one thread per row and 32 columns ->
+//                   epilogue: accumulators staged through shared memory -> each warp along one row, two 4-column quads a thread ->
 //                   bias / GELU / GELU' / dropout / residual -> bf16 | fp32 | atomic fp32
 // Operands may be K-major or MN-major (the transpose bits of wgmma), so the same kernel serves forward (x.W^T),
 // dgrad (dy.W) and wgrad (dy^T.x, split-K with fp32 atomics).
@@ -51,165 +51,141 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + 256 + 1024;
 };
 
-// 16 consecutive bf16 (32 bytes: one sector) <-> 16 floats, as two 128-bit accesses (the widest of sm_90)
-__device__ __forceinline__ void load16(const __nv_bfloat16* p, float (&f)[16]) {
-  const uint4 a = __ldg(reinterpret_cast<const uint4*>(p)), b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
-  const uint32_t r[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-#pragma unroll
-  for (int i = 0; i < 8; ++i) { f[2 * i] = bf16_lo(r[i]); f[2 * i + 1] = bf16_hi(r[i]); }
-}
-__device__ __forceinline__ void store16(__nv_bfloat16* p, const float* f) {
-  uint32_t r[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) r[i] = pack_bf16(f[2 * i], f[2 * i + 1]);
-  reinterpret_cast<uint4*>(p)[0] = make_uint4(r[0], r[1], r[2], r[3]);
-  reinterpret_cast<uint4*>(p)[1] = make_uint4(r[4], r[5], r[6], r[7]);
+// Epilogue thread layout: the threads of a warp cover consecutive columns of one output row (two rows for BN = 128), so
+// every global access of the epilogue is coalesced along the row and every staging read is a contiguous run of shared
+// memory.  A thread owns two 4-column quads of the tile, columns 4j .. 4j+3 and BN/2 + 4j .. +3, in every RPP-th row;
+// its bias is loaded once.
+template <int BN>
+struct EpiCfg {
+  static constexpr int TPR = BN / 8;        // threads per row
+  static constexpr int RPP = 256 / TPR;     // rows per pass of the 256 epilogue threads
+  static constexpr int GROUP = 4;           // rows whose global operands are fetched together
+  static_assert(BM % (RPP * GROUP) == 0, "row groups tile BM");
+};
+
+// bf16 quad (8 bytes) <-> 4 floats
+__device__ __forceinline__ uint2 ld_bf16x4(const __nv_bfloat16* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
+__device__ __forceinline__ void st_bf16x4(__nv_bfloat16* p, const float* f) {
+  *reinterpret_cast<uint2*>(p) = make_uint2(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]));
 }
 
-// Global operands of one epilogue chunk (32 columns of one row), fetched before the staged accumulators are
-// read back so that their latency overlaps the shared-memory reads.
-struct EpiPrefetch {
-  uint32_t bias[16];  // 32 bf16
-  uint32_t aux[16];   // 32 bf16 (aux_in)
-  uint32_t res[32];   // 32 fp32 or 32 bf16 (first 16 words)
+// Global operands of one row of a thread's two quads, fetched for a group of rows before any of them is stored.
+struct EpiIn {
+  uint32_t res[8];  // 8 fp32, or 8 bf16 in the first 4 words
+  uint32_t aux[4];  // 8 bf16 (aux_in)
 };
-__device__ __forceinline__ void load32_raw(const __nv_bfloat16* p, uint32_t* r) {
+__device__ __forceinline__ void epilogue_fetch(const GemmKParams& p, int row, const int (&col)[2], bool full, EpiIn& in) {
+  if (row >= p.M || !full) return;
+  if (p.aux_in) {
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const uint4 a = __ldg(reinterpret_cast<const uint4*>(p) + j);
-    r[4 * j] = a.x; r[4 * j + 1] = a.y; r[4 * j + 2] = a.z; r[4 * j + 3] = a.w;
+    for (int q = 0; q < 2; ++q) {
+      const uint2 a = ld_bf16x4(p.aux_in + (size_t)row * p.ldd + col[q]);
+      in.aux[2 * q] = a.x; in.aux[2 * q + 1] = a.y;
+    }
   }
-}
-__device__ __forceinline__ void epilogue_prefetch(const GemmKParams& p, int row, int col0, EpiPrefetch& pf) {
-  if (row >= p.M || col0 + 32 > p.N) return;
-  if (p.bias) load32_raw(p.bias + col0, pf.bias);
-  if (p.aux_in) load32_raw(p.aux_in + (size_t)row * p.ldd + col0, pf.aux);
   if (p.residual) {
     const int rrow = p.res_row_mod ? row % p.res_row_mod : row;
-    if (p.res_f32) {
-      const float* rf = reinterpret_cast<const float*>(p.residual) + (size_t)rrow * p.ldr + col0;
-      const float4* rp = reinterpret_cast<const float4*>(rf);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 a = __ldg(rp + j);
-        pf.res[4 * j] = __float_as_uint(a.x); pf.res[4 * j + 1] = __float_as_uint(a.y);
-        pf.res[4 * j + 2] = __float_as_uint(a.z); pf.res[4 * j + 3] = __float_as_uint(a.w);
+    for (int q = 0; q < 2; ++q) {
+      if (p.res_f32) {
+        const float4 a = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.residual) + (size_t)rrow * p.ldr + col[q]));
+        in.res[4 * q] = __float_as_uint(a.x); in.res[4 * q + 1] = __float_as_uint(a.y);
+        in.res[4 * q + 2] = __float_as_uint(a.z); in.res[4 * q + 3] = __float_as_uint(a.w);
+      } else {
+        const uint2 a = ld_bf16x4(reinterpret_cast<const __nv_bfloat16*>(p.residual) + (size_t)rrow * p.ldr + col[q]);
+        in.res[2 * q] = a.x; in.res[2 * q + 1] = a.y;
       }
-    } else {
-      load32_raw(reinterpret_cast<const __nv_bfloat16*>(p.residual) + (size_t)rrow * p.ldr + col0, pf.res);
     }
   }
 }
 
-// Epilogue for one thread: 32 consecutive columns of one output row.
+// Epilogue of one row of a thread's two quads: v[4q + e] is column col[q] + e.  `full`: both quads lie inside N.
 template <bool DROP>
-__device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, const uint32_t (&r)[32],
-                                               int row, int col0, const EpiPrefetch& pf, const DropState& ds) {
-  if (row >= p.M || col0 >= p.N) return;
-  const bool full = (col0 + 32 <= p.N);
+__device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8], int row, const int (&col)[2], bool full,
+                                             const uint32_t (&bias)[4], const EpiIn& in, const DropState& ds) {
+  if (row >= p.M) return;
   const int drow = p.d_row_block ? (row / p.d_row_block) * p.d_row_stride + row % p.d_row_block : row;
   const int rrow = p.res_row_mod ? row % p.res_row_mod : row;
-  float v[32];
-  if (p.alpha == 1.0f) {
+  if (p.alpha != 1.0f) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-  } else {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]) * p.alpha;
+    for (int i = 0; i < 8; ++i) v[i] = v[i] * p.alpha;
   }
 
   if (full) {
     if (p.bias) {
 #pragma unroll
-      for (int i = 0; i < 16; ++i) { v[2 * i] += bf16_lo(pf.bias[i]); v[2 * i + 1] += bf16_hi(pf.bias[i]); }
+      for (int i = 0; i < 4; ++i) { v[2 * i] += bf16_lo(bias[i]); v[2 * i + 1] += bf16_hi(bias[i]); }
     }
-    const size_t off = (size_t)row * p.ldd + col0;          // aux tensors: plain rows
-    const size_t doff = (size_t)drow * p.ldd + col0;        // D: optionally re-blocked rows
+    const size_t off[2] = {(size_t)row * p.ldd + col[0], (size_t)row * p.ldd + col[1]};      // aux tensors: plain rows
+    const size_t doff[2] = {(size_t)drow * p.ldd + col[0], (size_t)drow * p.ldd + col[1]};   // D: optionally re-blocked
     // aux_out: with an activation it receives act'(v) (what the backward epilogue multiplies by),
     // without one the value itself.  aux_in: a plain multiplier.  Switches are warp-uniform.
     if (p.aux_in) {
 #pragma unroll
-      for (int i = 0; i < 16; ++i) { v[2 * i] *= bf16_lo(pf.aux[i]); v[2 * i + 1] *= bf16_hi(pf.aux[i]); }
+      for (int i = 0; i < 4; ++i) { v[2 * i] *= bf16_lo(in.aux[i]); v[2 * i + 1] *= bf16_hi(in.aux[i]); }
     } else if (p.act == YMP_ACT_GELU_ERF) {
       if (p.aux_out) {
-        float d[32];
+        float x[8], d[8];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float x8[8], v8[8], d8[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) x8[e] = v[8 * j + e];
-          gelu_erf_both_x8(x8, v8, d8);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) { v[8 * j + e] = v8[e]; d[8 * j + e] = d8[e]; }
-        }
-        store16(p.aux_out + off, d);
-        store16(p.aux_out + off + 16, d + 16);
+        for (int i = 0; i < 8; ++i) x[i] = v[i];
+        gelu_erf_both_x8(x, v, d);
+        st_bf16x4(p.aux_out + off[0], d);
+        st_bf16x4(p.aux_out + off[1], d + 4);
       } else {
+        float x[8];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float x8[8], v8[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) x8[e] = v[8 * j + e];
-          gelu_erf_x8(x8, v8);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) v[8 * j + e] = v8[e];
-        }
+        for (int i = 0; i < 8; ++i) x[i] = v[i];
+        gelu_erf_x8(x, v);
       }
     } else if (p.act == YMP_ACT_GELU_TANH) {
       if (p.aux_out) {
-        float d[32];
+        float d[8];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = gelu_tanh_both(v[i], d[i]);
-        store16(p.aux_out + off, d);
-        store16(p.aux_out + off + 16, d + 16);
+        for (int i = 0; i < 8; ++i) v[i] = gelu_tanh_both(v[i], d[i]);
+        st_bf16x4(p.aux_out + off[0], d);
+        st_bf16x4(p.aux_out + off[1], d + 4);
       } else {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = gelu_tanh(v[i]);
+        for (int i = 0; i < 8; ++i) v[i] = gelu_tanh(v[i]);
       }
     } else if (p.aux_out) {
-      store16(p.aux_out + off, v);
-      store16(p.aux_out + off + 16, v + 16);
+      st_bf16x4(p.aux_out + off[0], v);
+      st_bf16x4(p.aux_out + off[1], v + 4);
     }
     if constexpr (DROP) {  // bias-dropout-add: residual + dropout(x + bias)
 #pragma unroll
-      for (int j = 0; j < 8; ++j) drop4(ds, (uint32_t)row, (uint32_t)(col0 + 4 * j), v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+      for (int q = 0; q < 2; ++q) drop4(ds, (uint32_t)row, (uint32_t)col[q], v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
     }
     if (p.residual) {
       if (p.res_f32) {  // fp32 residual stream
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] += __uint_as_float(pf.res[i]);
+        for (int i = 0; i < 8; ++i) v[i] += __uint_as_float(in.res[i]);
       } else {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) { v[2 * i] += bf16_lo(pf.res[i]); v[2 * i + 1] += bf16_hi(pf.res[i]); }
+        for (int i = 0; i < 4; ++i) { v[2 * i] += bf16_lo(in.res[i]); v[2 * i + 1] += bf16_hi(in.res[i]); }
       }
     }
-    if (!p.out_f32) {
-      __nv_bfloat16* dp = reinterpret_cast<__nv_bfloat16*>(p.D) + doff;
-      store16(dp, v);
-      store16(dp + 16, v + 16);
-    } else if (!p.accumulate) {
-      float* d = reinterpret_cast<float*>(p.D) + doff;
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-        reinterpret_cast<float4*>(d)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-    } else {
-      float* d = reinterpret_cast<float*>(p.D) + doff;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d + 4 * j),
-                     "f"(v[4 * j]), "f"(v[4 * j + 1]), "f"(v[4 * j + 2]), "f"(v[4 * j + 3])
+    for (int q = 0; q < 2; ++q) {
+      if (!p.out_f32) {
+        st_bf16x4(reinterpret_cast<__nv_bfloat16*>(p.D) + doff[q], v + 4 * q);
+      } else if (!p.accumulate) {
+        *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.D) + doff[q]) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+      } else {
+        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(reinterpret_cast<float*>(p.D) + doff[q]),
+                     "f"(v[4 * q]), "f"(v[4 * q + 1]), "f"(v[4 * q + 2]), "f"(v[4 * q + 3])
                      : "memory");
       }
     }
   } else {
     // ragged N tail: scalar, bounds-checked
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int col = col0 + i;
-      if (col < p.N) {
+    for (int i = 0; i < 8; ++i) {
+      const int c = col[i >> 2] + (i & 3);
+      if (c < p.N) {
         float x = v[i];
-        if (p.bias) x += __bfloat162float(p.bias[col]);
-        const size_t off = (size_t)row * p.ldd + col, doff = (size_t)drow * p.ldd + col;
+        if (p.bias) x += __bfloat162float(p.bias[c]);
+        const size_t off = (size_t)row * p.ldd + c, doff = (size_t)drow * p.ldd + c;
         if (p.aux_in) {
           x *= __bfloat162float(p.aux_in[off]);
         } else if (p.act == YMP_ACT_GELU_ERF) {
@@ -222,13 +198,13 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, const uint3
           p.aux_out[off] = __float2bfloat16(x);
         }
         if constexpr (DROP) {
-          const uint4 w = drop_words(ds, (uint32_t)row, (uint32_t)col >> 2);
-          const uint32_t wc = (col & 3) == 0 ? w.x : (col & 3) == 1 ? w.y : (col & 3) == 2 ? w.z : w.w;
+          const uint4 w = drop_words(ds, (uint32_t)row, (uint32_t)c >> 2);
+          const uint32_t wc = (c & 3) == 0 ? w.x : (c & 3) == 1 ? w.y : (c & 3) == 2 ? w.z : w.w;
           x = wc >= ds.thresh ? x * ds.scale : 0.f;
         }
         if (p.residual)
-          x += p.res_f32 ? reinterpret_cast<const float*>(p.residual)[(size_t)rrow * p.ldr + col]
-                         : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[(size_t)rrow * p.ldr + col]);
+          x += p.res_f32 ? reinterpret_cast<const float*>(p.residual)[(size_t)rrow * p.ldr + c]
+                         : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[(size_t)rrow * p.ldr + c]);
         if (!p.out_f32) reinterpret_cast<__nv_bfloat16*>(p.D)[doff] = __float2bfloat16(x);
         else if (!p.accumulate) reinterpret_cast<float*>(p.D)[doff] = x;
         else atomicAdd(reinterpret_cast<float*>(p.D) + doff, x);
@@ -387,22 +363,32 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
   named_sync(1, 256);
   DropState ds;  // only read when has_drop
   if (p.has_drop) ds = drop_state(p.drop);
-  const int et = threadIdx.x - 128, lr = et & (BM - 1), row = m_blk * BM + lr;
-#pragma unroll 1
-  for (int c = et >> 7; c < BN / 32; c += 2) {
-    const int col0 = n_blk * BN + c * 32;
-    EpiPrefetch pf;
-    epilogue_prefetch(p, row, col0, pf);
-    uint32_t r[32];
-    const float4* sp = reinterpret_cast<const float4*>(stg + lr * Cfg::STG_LD + c * 32);
+  using Epi = EpiCfg<BN>;
+  const int et = threadIdx.x - 128, tj = et % Epi::TPR, tr = et / Epi::TPR;
+  const int col[2] = {n_blk * BN + 4 * tj, n_blk * BN + BN / 2 + 4 * tj};
+  const bool full = col[1] + 4 <= p.N;
+  uint32_t bias[4];
+  if (p.bias && full) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 v = sp[j];
-      r[4 * j] = __float_as_uint(v.x); r[4 * j + 1] = __float_as_uint(v.y);
-      r[4 * j + 2] = __float_as_uint(v.z); r[4 * j + 3] = __float_as_uint(v.w);
+    for (int q = 0; q < 2; ++q) {
+      const uint2 b = ld_bf16x4(p.bias + col[q]);
+      bias[2 * q] = b.x; bias[2 * q + 1] = b.y;
     }
-    if (p.has_drop) epilogue_chunk<true>(p, r, row, col0, pf, ds);
-    else epilogue_chunk<false>(p, r, row, col0, pf, ds);
+  }
+#pragma unroll 1
+  for (int lr0 = tr; lr0 < BM; lr0 += Epi::RPP * Epi::GROUP) {
+    EpiIn in[Epi::GROUP];
+#pragma unroll
+    for (int u = 0; u < Epi::GROUP; ++u) epilogue_fetch(p, m_blk * BM + lr0 + u * Epi::RPP, col, full, in[u]);
+#pragma unroll
+    for (int u = 0; u < Epi::GROUP; ++u) {
+      const int lr = lr0 + u * Epi::RPP;
+      const float4 a = *reinterpret_cast<const float4*>(stg + lr * Cfg::STG_LD + 4 * tj);
+      const float4 b = *reinterpret_cast<const float4*>(stg + lr * Cfg::STG_LD + BN / 2 + 4 * tj);
+      float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+      if (p.has_drop) epilogue_row<true>(p, v, m_blk * BM + lr, col, full, bias, in[u], ds);
+      else epilogue_row<false>(p, v, m_blk * BM + lr, col, full, bias, in[u], ds);
+    }
   }
 }
 
