@@ -20,6 +20,7 @@ class VisionTransformer(nn.Module):
                  norm_layer=nn.LayerNorm, init_values=None, use_abs_pos_emb=True, use_rel_pos_bias=False,
                  use_shared_rel_pos_bias=False, use_mean_pooling=True, init_scale=0.001, use_checkpoint=False):
         super().__init__()
+        # use_checkpoint is accepted and ignored: activations of every block are kept for the backward
         if use_rel_pos_bias or use_shared_rel_pos_bias or not use_abs_pos_emb or (init_values is not None and init_values > 0):
             raise NotImplementedError("EVA encoder on the H100 path: absolute position embeddings, no layer scale")
         if not qkv_bias or use_mean_pooling or in_chans != 3 or drop_rate or attn_drop_rate:
@@ -88,7 +89,8 @@ def interpolate_pos_embed(model, checkpoint_model):
 
 
 def create_eva_vit_g(img_size=224, drop_path_rate=0.4, norm_layer=nn.LayerNorm, use_checkpoint=True, precision="fp16"):
-    """EVA-g (reference :413-436).  use_checkpoint is accepted; activations stay resident (180 GB HBM)."""
+    """EVA-g (reference :413-436).  use_checkpoint is accepted and ignored: the EVA encoder has no recompute mode and
+    keeps every block's activations for the backward (only the TimeSformer honours grad_ckpt)."""
     return VisionTransformer(img_size=img_size, patch_size=14, use_mean_pooling=False, embed_dim=1408, depth=40,
                              num_heads=1408 // 88, mlp_ratio=4.3637, qkv_bias=True, drop_path_rate=drop_path_rate,
                              norm_layer=norm_layer, use_checkpoint=use_checkpoint)

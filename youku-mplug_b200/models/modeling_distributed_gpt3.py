@@ -68,6 +68,7 @@ class GPT3Config:
         self.apply_residual_connection_post_layernorm = apply_residual_connection_post_layernorm
         self.sequence_parallel = sequence_parallel
         self.eod_id, self.tokens_to_generate, self.top_k, self.top_p = eod_id, tokens_to_generate, top_k, top_p
+        self.checkpoint_activations = False   # set from megatron_cfg by DistributedGPT3
         for k, v in kwargs.items():
             setattr(self, k, v)
         if apply_residual_connection_post_layernorm or sequence_parallel or fp32_residual_connection:
@@ -87,11 +88,13 @@ class GPT3Config:
 
     def engine_cfg(self, training=False):
         """Dims + the dropout setting of one decoder pass: hidden_dropout / attention_dropout are live only in
-        train() mode (the reference keeps the frozen decoder in train mode during training)."""
+        train() mode (the reference keeps the frozen decoder in train mode during training).  checkpoint_activations:
+        a pass that needs a backward recomputes each layer's activations there instead of keeping them."""
         return dict(vocab_size=self.vocab_size, hidden_size=self.hidden_size, ffn_hidden_size=self.ffn_hidden_size,
                     num_hidden_layers=self.num_hidden_layers, num_attention_heads=self.num_attention_heads,
                     max_position_embeddings=self.max_position_embeddings, layernorm_epsilon=self.layernorm_epsilon,
-                    hidden_dropout=self.hidden_dropout, attention_dropout=self.attention_dropout, training=bool(training))
+                    hidden_dropout=self.hidden_dropout, attention_dropout=self.attention_dropout, training=bool(training),
+                    checkpoint_activations=bool(self.checkpoint_activations))
 
 
 # ------------------------------------------------------------------------------------------ tokenizer
@@ -495,8 +498,11 @@ class GPT3Model(nn.Module):
 class DistributedGPT3(nn.Module):
     def __init__(self, model_dir, rank=0, path_load_tag='model', *args, **kwargs):
         super().__init__()
-        _check_tp1(kwargs.pop('megatron_cfg', None))
+        megatron_cfg = kwargs.pop('megatron_cfg', None)
+        _check_tp1(megatron_cfg)
         self.config = GPT3Config.from_pretrained(model_dir)
+        # Megatron-LM's name for per-layer activation checkpointing (off by default)
+        self.config.checkpoint_activations = bool((megatron_cfg or {}).get('checkpoint_activations', False))
         self.dist_model = GPT3Model(self.config)
         kwargs.pop('checkpoint_model_parallel_size', None)
         if kwargs.pop('load_state_dict', True):

@@ -68,9 +68,12 @@ class TimeSformer(nn.Module):
         self.num_frames = num_frames
         self.img_size, self.patch_size = img_size, patch_size
         self.num_patches = (img_size // patch_size) ** 2
-        self.grad_ckpt = grad_ckpt  # accepted; activations are kept resident (180 GB HBM)
+        # grad_ckpt (reference :575-577, one checkpoint per block): the training backward re-runs each block's forward
+        # from its saved input instead of keeping the block's activations (ymp.engine.vit_fwd recompute)
+        self.grad_ckpt = grad_ckpt
         self.vcfg = dict(img_size=img_size, patch_size=patch_size, embed_dim=embed_dim, depth=depth,
-                         num_heads=num_heads, mlp_ratio=mlp_ratio, num_frames=num_frames, clip_model=clip_model)
+                         num_heads=num_heads, mlp_ratio=mlp_ratio, num_frames=num_frames, clip_model=clip_model,
+                         grad_ckpt=bool(grad_ckpt))
         D, hid, std = embed_dim, int(embed_dim * mlp_ratio), init_std
         add_param(self, "cls_token", trunc_normal((1, 1, D), std))
         add_param(self, "pos_embed", trunc_normal((1, self.num_patches + 1, D), std))

@@ -105,8 +105,10 @@ def _spatial_maps(d, prefix_base_in, prefix_base_out):
     return m_in, m_out
 
 
-def vit_block_fwd(W, pre, x, d, save=True):
-    """Block.forward - models/vision_transformer.py:243-275.  x [RB, D] -> [RB, D]."""
+def vit_block_fwd(W, pre, x, d, save=True, compute_out=True):
+    """Block.forward - models/vision_transformer.py:243-275.  x [RB, D] -> [RB, D].
+    compute_out=False skips the mlp.fc2 GEMM and returns None as the output: the recompute in vit_bwd needs only
+    the saved activations (the block output is the next block's input, which the forward kept)."""
     R, RB, D, B, T = d.R, d.RB, d.D, d.B, d.T
     c = Ctx()
     # ---- temporal attention over the T frames of each patch
@@ -133,7 +135,9 @@ def vit_block_fwd(W, pre, x, d, save=True):
     ln_m, c.m_m, c.r_m = ops.layernorm_fwd(y, W[pre + "norm2.weight"], W[pre + "norm2.bias"], d.eps)
     dact = torch.empty((RB, d.hid), device=x.device, dtype=bf16)
     h = ops.gemm(ln_m, W[pre + "mlp.fc1.weight"], bias=W[pre + "mlp.fc1.bias"], act=ACT_GELU_ERF, aux_out=dact)
-    out = ops.gemm(h, W[pre + "mlp.fc2.weight"], bias=W[pre + "mlp.fc2.bias"], residual=y, out_dtype=torch.float32)
+    out = None
+    if compute_out:
+        out = ops.gemm(h, W[pre + "mlp.fc2.weight"], bias=W[pre + "mlp.fc2.bias"], residual=y, out_dtype=torch.float32)
     if save:
         c.update(x=x, ln_t=ln_t, qkv_t=qkv_t, att_t=att_t, proj_t=proj_t, xt=xt, ln_s=ln_s, qkv_s=qkv_s,
                  att_s=att_s, y=y, ln_m=ln_m, dact=dact, h=h)
@@ -193,14 +197,17 @@ def _qkv_wgrad(G, apre, dqkv, x, D, dev):
         ops.colsum(dqkv[:, 2 * D:], G[apre + "v_bias"].view(-1))
 
 
-def vit_fwd(W, video, vcfg, save=True):
+def vit_fwd(W, video, vcfg, save=True, recompute=False):
     """TimeSformer.forward_features - models/vision_transformer.py:544-587.
-    video [B,3,T,H,W] bf16 -> image_embeds [B*(1+T*N), D] in the reference's (t n) order."""
+    video [B,3,T,H,W] bf16 -> image_embeds [B*(1+T*N), D] in the reference's (t n) order.
+    recompute (with save): activation checkpointing per block (the reference's grad_ckpt, :575-577).  Only each
+    block's fp32 input [RB, D] is kept; vit_bwd re-runs the block's forward from it just before its backward."""
     B = video.shape[0]
     d = VitDims(vcfg, B)
     assert video.shape[2] == d.T, f"video has {video.shape[2]} frames, model expects {d.T}"
     dev = video.device
-    c = Ctx(d=d, blocks=[])
+    recompute = bool(save and recompute)
+    c = Ctx(d=d, blocks=[], recompute=recompute)
     video = video.contiguous()
     pos, temb = W[VE + "pos_embed"], W[VE + "temporal_embed"]
     table = (pos[0, 1:, None, :] + temb[0, None, :, :]).reshape(d.N * d.T, d.D).contiguous()
@@ -223,13 +230,22 @@ def vit_fwd(W, video, vcfg, save=True):
     else:
         x = x0
     for i in range(d.depth):
-        x, bc = vit_block_fwd(W, f"{VE}blocks.{i}.", x, d, save)
-        c.blocks.append(bc)
+        out, bc = vit_block_fwd(W, f"{VE}blocks.{i}.", x, d, save and not recompute)
+        c.blocks.append(x if recompute else bc)   # recompute: blocks[i] is the block's input
+        x, bc = out, None
     rows = _final_gather_rows(d, dev)
     out, c.mf, c.rf = ops.layernorm_fwd(x, W[VE + "norm.weight"], W[VE + "norm.bias"], d.eps, in_rows=rows)
     if save:
         c.update(patches=patches, video=video if fused else None, x0=x0, xL=x, rows=rows)
     return out, c
+
+
+def vit_block_saved(W, c, i):
+    """What block i's backward reads: the activations kept by vit_fwd, or in recompute mode the same tensors rebuilt
+    from the block's saved input by the same kernels (the forward is deterministic: bit-identical to the kept ones)."""
+    if not c.recompute:
+        return c.blocks[i]
+    return vit_block_fwd(W, f"{VE}blocks.{i}.", c.blocks[i], c.d, compute_out=False)[1]
 
 
 def vit_bwd(W, G, c, d_out):
@@ -239,8 +255,9 @@ def vit_bwd(W, G, c, d_out):
     dx = ops.layernorm_bwd(d_out, c.xL, W[VE + "norm.weight"], c.mf, c.rf, in_rows=c.rows,
                            dgamma=G.get(VE + "norm.weight"), dbeta=G.get(VE + "norm.bias"))
     for i in reversed(range(d.depth)):
-        dx = vit_block_bwd(W, G, f"{VE}blocks.{i}.", c.blocks[i], dx, d)
-        c.blocks[i] = None  # release activations as we go
+        bc = vit_block_saved(W, c, i)
+        dx = vit_block_bwd(W, G, f"{VE}blocks.{i}.", bc, dx, d)
+        c.blocks[i] = bc = None  # release activations as we go
         if hasattr(G, "ready"):
             G.ready(f"{VE}blocks.{i}.")  # this block's weight gradients are final: their all-reduce may start
     if VE + "norm_pre.weight" in W:
@@ -530,9 +547,10 @@ class GptDims:
         self.scale = 1.0 / math.sqrt(self.hd)
 
 
-def gpt_layer_fwd(W, pre, x, g, B, S, train_w=False, drop=None, li=0):
+def gpt_layer_fwd(W, pre, x, g, B, S, train_w=False, drop=None, li=0, compute_out=True):
     """GPT3ParallelTransformerLayer.forward - models/modeling_distributed_gpt3.py:1034-1089
-    (causal mask over the whole [prefix|text] sequence, :1329-1332; `drop`: GptDrop or None, li: layer index)."""
+    (causal mask over the whole [prefix|text] sequence, :1329-1332; `drop`: GptDrop or None, li: layer index).
+    compute_out=False skips the dense_4h_to_h GEMM and returns None as the output (the recompute in gpt_bwd)."""
     H, hd = g.H, g.hd
     c = Ctx()
     d_at = drop.attn(li) if drop else None
@@ -550,8 +568,10 @@ def gpt_layer_fwd(W, pre, x, g, B, S, train_w=False, drop=None, li=0):
     ln2, c.m2, c.r2 = ops.layernorm_fwd(x1, W[pre + "post_attention_layernorm.weight"], W[pre + "post_attention_layernorm.bias"], g.eps)
     dact = torch.empty((B * S, g.F), device=x.device, dtype=bf16)
     h = ops.gemm(ln2, W[pre + "mlp.dense_h_to_4h.weight"], bias=W[pre + "mlp.dense_h_to_4h.bias"], act=ACT_GELU_TANH, aux_out=dact)
-    out = ops.gemm(h, W[pre + "mlp.dense_4h_to_h.weight"], bias=W[pre + "mlp.dense_4h_to_h.bias"], residual=x1,
-                   out_dtype=torch.float32, drop=d_b2)
+    out = None
+    if compute_out:
+        out = ops.gemm(h, W[pre + "mlp.dense_4h_to_h.weight"], bias=W[pre + "mlp.dense_4h_to_h.bias"], residual=x1,
+                       out_dtype=torch.float32, drop=d_b2)
     c.update(x=x, qkv=qkv, att=att, x1=x1, dact=dact)
     if train_w:
         c.update(ln1=ln1, ln2=ln2, h=h)
@@ -572,10 +592,12 @@ def gpt_layer_bwd(W, G, pre, c, dout, g, B, S, drop=None, li=0, dout_d=None):
     if "ln2" in c:
         linear_wgrad(dpre, c.ln2, pre + "mlp.dense_h_to_4h.weight", pre + "mlp.dense_h_to_4h.bias", G)
     dln2 = linear_dgrad(dpre, W[pre + "mlp.dense_h_to_4h.weight"])
+    del dpre   # temporaries go back to the allocator at their last use: the layer's backward peak is what recompute pays
     d_b1 = drop.bda_attn(li) if drop else None
     r = ops.layernorm_bwd(dln2, c.x1, W[pre + "post_attention_layernorm.weight"], c.m2, c.r2, add=dout,
                           dgamma=G.get(pre + "post_attention_layernorm.weight"), dbeta=G.get(pre + "post_attention_layernorm.bias"),
                           drop=d_b1)
+    del dln2
     dx1, dx1_d = r if d_b1 is not None else (r, r)
     linear_wgrad(dx1_d, c.att, pre + "self_attention.dense.weight", pre + "self_attention.dense.bias", G)
     datt = linear_dgrad(dx1_d, W[pre + "self_attention.dense.weight"])
@@ -588,31 +610,46 @@ def gpt_layer_bwd(W, G, pre, c, dout, g, B, S, drop=None, li=0, dout_d=None):
     if "ln1" in c:
         linear_wgrad(dqkv, c.ln1, pre + "self_attention.query_key_value.weight", pre + "self_attention.query_key_value.bias", G)
     dln1 = linear_dgrad(dqkv, W[pre + "self_attention.query_key_value.weight"])
+    del dqkv, dq, dk, dv, datt
     d_in = (drop.bda_mlp(li - 1) if li > 0 else drop.embed()) if drop else None
     r = ops.layernorm_bwd(dln1, c.x, W[pre + "input_layernorm.weight"], c.m1, c.r1, add=dx1,
                           dgamma=G.get(pre + "input_layernorm.weight"), dbeta=G.get(pre + "input_layernorm.bias"), drop=d_in)
     return r if d_in is not None else (r, r)
 
 
-def gpt_fwd(W, x, gcfg, B, S, train_w=False, save=True, out_rows=None, drop=None):
+def gpt_fwd(W, x, gcfg, B, S, train_w=False, save=True, out_rows=None, drop=None, recompute=False):
     """x [B*S, H] fp32: input embeddings with the learned position embeddings already added
     (GPT3Embedding.forward, :640-666); with `drop` (GptDrop) the embedding dropout (:631) is applied to x IN PLACE
     first.  Returns final-LN hidden states [B*S, H], or only the rows listed in out_rows (int32 row indices,
-    compact [len(out_rows), H]) when the caller needs no others."""
+    compact [len(out_rows), H]) when the caller needs no others.
+    recompute (with save): activation checkpointing per layer (Megatron-LM's checkpoint_activations).  Only each
+    layer's fp32 input [B*S, H] is kept; gpt_bwd re-runs the layer's forward from it, with the pass's own dropout
+    state, just before its backward."""
     g = GptDims(gcfg)
     if drop is not None and drop.p_hidden <= 0 and drop.p_attn <= 0:
         drop = None
-    c = Ctx(g=g, B=B, S=S, layers=[], out_rows=out_rows, drop=drop)
+    recompute = bool(save and recompute)
+    c = Ctx(g=g, B=B, S=S, layers=[], out_rows=out_rows, drop=drop, train_w=train_w, recompute=recompute)
     if drop is not None and drop.embed() is not None:
         ops.dropout(x, drop.embed())
     for i in range(g.layers):
-        x, lc = gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", x, g, B, S, train_w, drop, i)
-        c.layers.append(lc if save else None)
+        out, lc = gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", x, g, B, S, train_w, drop, i)
+        c.layers.append((x if recompute else lc) if save else None)   # recompute: layers[i] is the layer's input
+        x, lc = out, None
     hid, c.mf, c.rf = ops.layernorm_fwd(x, W[GPT + "encoder.final_layernorm.weight"], W[GPT + "encoder.final_layernorm.bias"], g.eps,
                                         in_rows=out_rows)
     if save:
         c.xL = x
     return hid, c
+
+
+def gpt_layer_saved(W, c, i):
+    """What layer i's backward reads: the activations kept by gpt_fwd, or in recompute mode the same tensors rebuilt
+    from the layer's saved input (deterministic kernels, counter-based dropout masks: bit-identical to the kept ones)."""
+    if not c.recompute:
+        return c.layers[i]
+    return gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", c.layers[i], c.g, c.B, c.S, c.train_w, c.drop, i,
+                         compute_out=False)[1]
 
 
 def gpt_bwd(W, G, c, dhid):
@@ -625,10 +662,12 @@ def gpt_bwd(W, G, c, dhid):
     r = ops.layernorm_bwd(dhid, c.xL, W[GPT + "encoder.final_layernorm.weight"], c.mf, c.rf,
                           dgamma=G.get(GPT + "encoder.final_layernorm.weight"), dbeta=G.get(GPT + "encoder.final_layernorm.bias"),
                           in_rows=c.out_rows, dx=dx, drop=d_last)
+    c.xL = None   # the last layer's output is not read again
     dx, dx_d = r if d_last is not None else (r, r)
     for i in reversed(range(g.layers)):
-        dx, dx_d = gpt_layer_bwd(W, G, f"{GPT}encoder.layers.{i}.", c.layers[i], dx, g, B, S, drop, i, dx_d)
-        c.layers[i] = None
+        lc = gpt_layer_saved(W, c, i)
+        dx, dx_d = gpt_layer_bwd(W, G, f"{GPT}encoder.layers.{i}.", lc, dx, g, B, S, drop, i, dx_d)
+        c.layers[i] = lc = None
     return dx_d
 
 

@@ -128,6 +128,16 @@ def gpt_drop(gcfg, dev):
     return engine.GptDrop(_pass_rng(dev), ph, pa)
 
 
+def _vit_recompute(vcfg):
+    """TimeSformer grad_ckpt: recompute every block's activations in the backward instead of keeping them."""
+    return bool(vcfg.get("grad_ckpt", False))
+
+
+def _gpt_recompute(gcfg):
+    """megatron_cfg.checkpoint_activations: recompute every decoder layer's activations in the backward."""
+    return bool(gcfg.get("checkpoint_activations", False))
+
+
 _TEXT_ROWS = {}
 
 
@@ -156,7 +166,7 @@ class PretrainFn(torch.autograd.Function):
         W = {k: as_bf16(p) for k, p in zip(keys, params)}
         B = video.shape[0]
         need_bwd = any(ctx.needs_input_grad[7:])
-        img, cv = engine.vit_fwd(W, video.to(bf16), vcfg, save=need_bwd)
+        img, cv = engine.vit_fwd(W, video.to(bf16), vcfg, save=need_bwd, recompute=need_bwd and _vit_recompute(vcfg))
         q, ca = engine.attn_pool_fwd(W, img, B, vcfg["num_heads"], save=need_bwd)
         Q, L = ca.Q, input_ids.shape[1]
         S = Q + L
@@ -175,7 +185,7 @@ class PretrainFn(torch.autograd.Function):
         text_rows = _text_rows(B, S, Q, video.device)
         targets_t = targets[:, Q:].contiguous()
         hid, cg = engine.gpt_fwd(W, x_in, gcfg, B, S, train_w=train_gpt, save=need_bwd, out_rows=text_rows,
-                                 drop=gpt_drop(gcfg, video.device))
+                                 drop=gpt_drop(gcfg, video.device), recompute=need_bwd and _gpt_recompute(gcfg))
         logits, losses, lse = engine.lm_head_fwd(W, hid, targets_t)
         losses_bs = torch.zeros((B, S), device=video.device, dtype=torch.float32)
         losses_bs[:, Q:] = losses.view(B, L)
@@ -221,7 +231,7 @@ class VitFn(torch.autograd.Function):
         _require_cuda(video, "VitFn")
         W = {k: as_bf16(p) for k, p in zip(keys, params)}
         need_bwd = any(ctx.needs_input_grad[3:])
-        out, c = engine.vit_fwd(W, video.to(bf16), vcfg, save=need_bwd)
+        out, c = engine.vit_fwd(W, video.to(bf16), vcfg, save=need_bwd, recompute=need_bwd and _vit_recompute(vcfg))
         if need_bwd:
             ctx.W, ctx.keys, ctx.c, ctx.params = W, keys, c, params
         return out.view(video.shape[0], -1, out.shape[1])
@@ -419,7 +429,7 @@ class GptFn(torch.autograd.Function):
         need_bwd = any(ctx.needs_input_grad)
         train_gpt = any(n for k, n in zip(keys, ctx.needs_input_grad[5:]) if k.startswith(engine.GPT + "encoder.layers"))
         hid, cg = engine.gpt_fwd(W, x_in, gcfg, B, S, train_w=train_gpt, save=need_bwd,
-                                 drop=gpt_drop(gcfg, input_embeds.device))
+                                 drop=gpt_drop(gcfg, input_embeds.device), recompute=need_bwd and _gpt_recompute(gcfg))
         logits = losses = lse = None
         if labels is not None or want_logits:
             lab = labels if labels is not None else torch.zeros((B, S), dtype=torch.long, device=input_embeds.device)
