@@ -243,7 +243,12 @@ typedef struct ymp_attn_args {
   int32_t q_head_stride, k_head_stride, v_head_stride, o_head_stride;
   ymp_seqmap map_q, map_kv, map_o;
   int32_t n_seq, n_heads, head_dim, s_q, s_kv;
-  int32_t mask;        /* YMP_MASK_NONE | YMP_MASK_CAUSAL | YMP_MASK_BLOCK */
+  int32_t mask;        /* YMP_MASK_NONE | YMP_MASK_CAUSAL | YMP_MASK_BLOCK.  Causal with s_q < s_kv is bottom-right
+                          aligned: query i sits at key position i + (s_kv - s_q) and sees keys j <= i + s_kv - s_q
+                          (a block of queries after a prefix of keys, e.g. text rows whose map_kv puts a shared
+                          prefix first).  Forward only, head_dim 64 / 80 / 88 / 96, no dropout, total_rows or
+                          s_kv_dev; each row is bit-identical to the same row of the square causal call over the
+                          whole key range.  Block masks need s_q == s_kv. */
   int32_t mask_block;  /* YMP_MASK_BLOCK: position i attends j iff i / mask_block == j / mask_block.
                           Packs many short sequences (TimeSformer temporal attention over T frames,
                           vision_transformer.py:246-248) into one tensor-core tile. */

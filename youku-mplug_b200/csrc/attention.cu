@@ -746,7 +746,8 @@ __device__ __forceinline__ void wg_load_tile(uint8_t* dst, const RMat& m, int r0
     if ((64 * CH) % 128 != 0 && idx >= 64 * CH) break;
     const int r = idx / CH, c = idx - r * CH;
     uint8_t* d = dst + (c >> 3) * 8192 + r * 128 + (((c & 7) ^ (r & 7)) << 4);
-    if (r0 + r < n_valid && (DIO == D || c * 8 < DIO)) cp_async16(d, mrow(m, r0 + r) + c * 8);
+    // (unsigned: a query tile of an offset-causal call may start before the first query row)
+    if ((unsigned)(r0 + r) < (unsigned)n_valid && (DIO == D || c * 8 < DIO)) cp_async16(d, mrow(m, r0 + r) + c * 8);
     else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
   }
 }
@@ -806,8 +807,14 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   uint8_t* Qs = sm;
   uint8_t* KVs = sm + TB;  // [stage][K|V]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 64, h = blockIdx.y, s = blockIdx.z;
+  const int h = blockIdx.y, s = blockIdx.z;
   const int g = lane >> 2, t4 = lane & 3;
+  // Causal with s_q < s_kv is bottom-right aligned: query i sits at key position i + qoff and sees keys j <= i + qoff.
+  // Query tiles are aligned to the key tiles (the first starts qoff % 64 rows before query 0, those rows are padding),
+  // so each row meets the same key tiles, masks and arithmetic as the same row of the square causal call over the
+  // whole key range: bit-identical O and lse, and no key tile that is fully masked for a row.
+  const int qoff = p.mask == MASK_CAUSAL ? p.s_kv - p.s_q : 0;
+  const int q0 = blockIdx.x * 64 - (qoff & 63), a0 = q0 + qoff;  // first query row of the tile and its key position
   griddep_launch();   // (programmatic dependent launch; no-ops for an ordinary launch)
   griddep_wait();
   int sq, skv;
@@ -817,7 +824,7 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq);
   const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
   int kv_end = skv;
-  if (p.mask == MASK_CAUSAL) kv_end = min(skv, q0 + 64);
+  if (p.mask == MASK_CAUSAL) kv_end = min(skv, a0 + 64);
   const int ntiles = (kv_end + 63) / 64;
 
   wg_load_tile<D, DIO>(Qs, Mq, q0, sq);
@@ -850,7 +857,7 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
     __syncthreads();
     float sc[8][4];
     wg_scores<D>(sc, smem_u32(Qs), smem_u32(Ks));
-    if (tile_needs_mask(p, q0 + warp * 16, kv0, skv)) apply_mask(p, sc, q0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);
+    if (tile_needs_mask(p, a0 + warp * 16, kv0, skv)) apply_mask(p, sc, a0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);
     float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
 #pragma unroll
     for (int nb = 0; nb < 8; ++nb) {
@@ -901,7 +908,7 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int qi = q0 + warp * 16 + g + r * 8;
-    if (qi >= sq) continue;
+    if (qi < 0 || qi >= sq) continue;
     const float inv = l_i[r] > 0.f ? 1.f / l_i[r] : 0.f;
     __nv_bfloat16* orow = p.o + rrow(mo, qi) * p.ldo + h * p.hso;
 #pragma unroll
@@ -1281,7 +1288,8 @@ static int launch_wg_fwd(const AttnKParams& p, cudaStream_t st) {
   const int smem = 5 * WgTile<D>::BYTES + 1024;
   static DeviceOnce once;
   if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(attn_wg_fwd_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
-  launch_k(attn_wg_fwd_kernel<D, DIO>, dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), dim3(128), smem, st, p);
+  const int lead = p.mask == MASK_CAUSAL ? (p.s_kv - p.s_q) & 63 : 0;  // padding rows before query 0 (offset causal)
+  launch_k(attn_wg_fwd_kernel<D, DIO>, dim3((p.s_q + lead + 63) / 64, p.n_heads, p.n_seq), dim3(128), smem, st, p);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }
@@ -1309,7 +1317,8 @@ static int fill_params(const ymp_attn_args* a, AttnKParams& p, const char* who) 
   YMP_CHECK_ARG(a->q_head_stride % 8 == 0 && a->k_head_stride % 8 == 0 && a->v_head_stride % 8 == 0 && a->o_head_stride % 8 == 0, "%s: head strides must be multiples of 8", who);
   YMP_CHECK_ARG(aligned16(a->q) && aligned16(a->k) && aligned16(a->v), "%s: q/k/v must be 16-byte aligned", who);
   YMP_CHECK_ARG(a->mask >= 0 && a->mask <= 2, "%s: mask must be 0 (none), 1 (causal) or 2 (block-diagonal)", who);
-  YMP_CHECK_ARG(a->mask == YMP_MASK_NONE || a->s_q == a->s_kv, "%s: causal / block masks need s_q == s_kv", who);
+  YMP_CHECK_ARG(a->mask == YMP_MASK_NONE || a->s_q == a->s_kv || (a->mask == YMP_MASK_CAUSAL && a->s_q < a->s_kv),
+                "%s: block masks need s_q == s_kv, causal needs s_q <= s_kv", who);
   YMP_CHECK_ARG(a->mask != YMP_MASK_BLOCK || a->mask_block > 0, "%s: block mask needs mask_block > 0", who);
   YMP_CHECK_ARG(a->total_rows == 0 || (a->s_q == a->s_kv && a->total_rows > (int64_t)(a->n_seq - 1) * a->s_q),
                 "%s: total_rows needs s_q == s_kv and must reach the last sequence", who);
@@ -1371,6 +1380,20 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const bool dropped = p.has_drop;
   YMP_CHECK_ARG(!dropped || a->drop.p < 1.f, "ymp_attn_fwd: dropout p must be < 1");
+  if (a->mask == YMP_MASK_CAUSAL && a->s_q < a->s_kv) {
+    // offset causal (a block of queries at the end of a longer key range): always the wgmma tiles, whatever s_q, so
+    // that every row is bit-identical to the same row of the square causal call over the whole range
+    YMP_CHECK_ARG(a->head_dim != 128, "ymp_attn_fwd: causal with s_q < s_kv needs head_dim 64, 80, 88 or 96");
+    YMP_CHECK_ARG(!dropped, "ymp_attn_fwd: causal with s_q < s_kv takes no dropout");
+    YMP_CHECK_ARG(!a->s_kv_dev, "ymp_attn_fwd: causal with s_q < s_kv takes no s_kv_dev");
+    g_attn_path = YMP_ATTN_PATH_WGMMA;
+    switch (a->head_dim) {
+      case 64: return launch_wg_fwd<64>(p, st);
+      case 80: return launch_wg_fwd<80>(p, st);
+      case 88: return launch_wg_fwd<96, 88>(p, st);
+      default: return launch_wg_fwd<96>(p, st);
+    }
+  }
   if (a->s_q == 1 && a->mask == YMP_MASK_NONE && a->total_rows == 0 && !dropped && a->head_dim != 88 && a->head_dim != 128) {
     g_attn_path = YMP_ATTN_PATH_DECODE;   // one query row per sequence: the streaming kernel (also follows s_kv_dev)
     switch (a->head_dim) {
@@ -1417,6 +1440,7 @@ extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {
   YMP_CHECK_ARG(a->o && a->lse && b->dout && b->dq && b->dk && b->dv && b->delta_ws, "ymp_attn_bwd: null o/lse/dout/dq/dk/dv/delta_ws");
   YMP_CHECK_ARG(b->lddo % 8 == 0 && b->lddq % 8 == 0 && b->lddk % 8 == 0 && b->lddv % 8 == 0, "ymp_attn_bwd: grad row strides must be multiples of 8");
   YMP_CHECK_ARG(!a->s_kv_dev, "ymp_attn_bwd: s_kv_dev is forward only");
+  YMP_CHECK_ARG(a->mask != YMP_MASK_CAUSAL || a->s_q == a->s_kv, "ymp_attn_bwd: causal with s_q < s_kv is forward only");
   YMP_CHECK_ARG(!p.has_drop || a->drop.p < 1.f, "ymp_attn_bwd: dropout p must be < 1");
   p.dout = (const __nv_bfloat16*)b->dout; p.dq = (__nv_bfloat16*)b->dq; p.dk = (__nv_bfloat16*)b->dk; p.dv = (__nv_bfloat16*)b->dv;
   p.delta = b->delta_ws;

@@ -330,6 +330,46 @@ class _PromptClsBase(_PrefixModelBase):
         pooled = hid[torch.arange(hid.shape[0], device=hid.device), Q + att.sum(dim=-1) - 1]
         return self.cls_head(pooled)
 
+    # The evaluations score t texts per video.  When nothing can need a backward through the decoder and its dropout
+    # is off, every video's prefix is computed once for all its texts (DistributedGPT3.forward_shared_prefix) instead
+    # of once per text, and columns past the last one any text attends to are not computed.  The outputs are
+    # bit-identical to the passes above on the repeated prefixes.
+    def _shared_prefix_ok(self, query_features):
+        """True when the eval passes may share the prefixes: no backward can be needed (grad mode off, or neither the
+        query features nor any decoder parameter requires grad) and the decoder's dropout is inactive."""
+        needs_grad = torch.is_grad_enabled() and (query_features.requires_grad
+                                                  or any(p.requires_grad for p in self.text_decoder.parameters()))
+        return not needs_grad and not self.text_decoder.dropout_active()
+
+    def _gen_pass_shared(self, query_features, text):
+        """_gen_pass with text n after prefix n // t, prefixes not repeated: (losses [N, Q+L-1] fp32 with +0 in the prefix
+        and untouched columns, loss_mask [N, Q+L-1]) - the same values as (out.losses, loss_mask) of _gen_pass."""
+        Q = query_features.shape[1]
+        N, L = text.input_ids.shape
+        text_loss_atts = mask_prompt(text.attention_mask[:, 1:].clone(), text.prompt_lengths)
+        targets, loss_mask = build_targets(text.input_ids, text_loss_atts, Q)
+        Le = used_columns(text.attention_mask)
+        emb = self._word_embedding()(text.input_ids[:, :Le]).to(query_features.dtype)
+        out = self.text_decoder.forward_shared_prefix(query_features, emb, labels=targets[:, Q:Q + Le])
+        losses = torch.zeros((N, Q + L), device=out.losses.device, dtype=torch.float32)
+        losses[:, Q:Q + Le] = out.losses
+        return losses[:, :-1].contiguous(), loss_mask
+
+    def _cls_pass_shared(self, query_features, prompt_text):
+        """_cls_pass (eval) with prompt n after prefix n // t, prefixes not repeated; the LM head is not run."""
+        att = prompt_text.attention_mask
+        Le = used_columns(att)
+        emb = self._word_embedding()(prompt_text.input_ids[:, :Le]).to(query_features.dtype)
+        rows = torch.arange(att.shape[0], device=att.device) * Le + att.sum(dim=-1) - 1
+        return self.cls_head(self.text_decoder.forward_shared_prefix(query_features, emb, hidden_rows=rows).hidden)
+
+
+def used_columns(attention_mask):
+    """1 + the last column any sequence attends to (at least 1; one host read).  Causal rows never see later ones, so
+    the columns after it change no value that the evaluations read."""
+    cols = torch.arange(1, attention_mask.shape[1] + 1, device=attention_mask.device)
+    return max(1, int((attention_mask.ne(0).any(0) * cols).max()))
+
 
 class DistributedGPT3_Cls(_PromptClsBase):
     """Video category prediction (:431-657).  Training: generation loss on [prompt+label] (+ optional
@@ -355,10 +395,15 @@ class DistributedGPT3_Cls(_PromptClsBase):
                 loss_cls = out.loss.new_zeros(())
             return out.loss, loss_cls
         num_cls = text.input_ids.shape[0] // B
-        qf = query_features.unsqueeze(1).repeat(1, num_cls, 1, 1).reshape(B * num_cls, Q, -1)
-        out, loss_mask = self._gen_pass(qf, text)
-        generation_logits = (-(out.losses * loss_mask).sum(dim=-1)).view(B, num_cls).softmax(dim=-1)
-        cls_logits = self._cls_pass(query_features, prompt_text, False) if self.use_cls else None
+        if self._shared_prefix_ok(query_features):
+            losses, loss_mask = self._gen_pass_shared(query_features, text)
+            cls_logits = self._cls_pass_shared(query_features, prompt_text) if self.use_cls else None
+        else:
+            qf = query_features.unsqueeze(1).repeat(1, num_cls, 1, 1).reshape(B * num_cls, Q, -1)
+            out, loss_mask = self._gen_pass(qf, text)
+            losses = out.losses
+            cls_logits = self._cls_pass(query_features, prompt_text, False) if self.use_cls else None
+        generation_logits = (-(losses * loss_mask).sum(dim=-1)).view(B, num_cls).softmax(dim=-1)
         return generation_logits, cls_logits
 
 
@@ -387,12 +432,18 @@ class DistributedGPT3_Retrieval_Cls(_PromptClsBase):
             return out.loss, loss_cls
         V = query_features.shape[0]
         t = text.input_ids.shape[0] // V
-        qf = query_features.repeat_interleave(t, dim=0)
-        out, loss_mask = self._gen_pass(qf, text)
-        generation_logits = (-(out.losses * loss_mask).sum(dim=-1)).view(V, t)
+        if self._shared_prefix_ok(query_features):
+            losses, loss_mask = self._gen_pass_shared(query_features, text)
+            cls_pass = partial(self._cls_pass_shared, query_features, prompt_text)
+        else:
+            qf = query_features.repeat_interleave(t, dim=0)
+            out, loss_mask = self._gen_pass(qf, text)
+            losses = out.losses
+            cls_pass = partial(self._cls_pass, qf, prompt_text, False)
+        generation_logits = (-(losses * loss_mask).sum(dim=-1)).view(V, t)
         cls_logits = None
         if self.use_cls:
-            cls_logits = self._cls_pass(qf, prompt_text, False).float().softmax(dim=-1)[:, 1].view(V, t)
+            cls_logits = cls_pass().float().softmax(dim=-1)[:, 1].view(V, t)
         return generation_logits, cls_logits
 
 

@@ -552,6 +552,24 @@ class DistributedGPT3(nn.Module):
         loss = torch.sum(losses.reshape(-1) * lm) / lm.sum()
         return AttrDict(logits=logits, loss=loss, losses=losses, last_hidden_state=hidden)
 
+    def dropout_active(self):
+        """Does a pass in the current mode draw dropout masks (train() mode and a non-zero probability)?"""
+        return YF.gpt_dropout_active(self.config.engine_cfg(self.training))
+
+    def forward_shared_prefix(self, query_embeds, input_embeds, labels=None, hidden_rows=None):
+        """Score N = V*t texts against V visual prefixes without repeating them: text n follows prefix n // t under the
+        same plain causal mask as forward() on torch.cat([query_embeds.repeat_interleave(t, 0), input_embeds], 1).
+        query_embeds [V,Q,H], input_embeds [N,L,H]; labels [N,L] are the targets of the text positions.
+        Forward only and without dropout (evaluation): returns Dict(losses [N,L] fp32 per-token CE of the text
+        positions or None, hidden [len(hidden_rows), H] final hidden states of text rows n*L + j or None), each value
+        bit-identical to the matching position of forward() on the repeated layout."""
+        if self.dropout_active():
+            raise ValueError("forward_shared_prefix: the decoder's dropout is active (train() mode with p > 0)")
+        keys, params = self._param_list()
+        losses, hidden = YF.gpt_shared_prefix(query_embeds, input_embeds.to(query_embeds.dtype), labels, hidden_rows,
+                                              self.config.engine_cfg(self.training), keys, params)
+        return AttrDict(losses=losses, hidden=hidden)
+
     # ------------------------------------------------------------------------------------------ generation
     def _decode(self, tokens, input_embeds, n_query):
         """Inference branch of forward (:1576-1603): one incremental step over the KV cache.  input_embeds

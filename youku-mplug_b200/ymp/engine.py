@@ -547,10 +547,12 @@ class GptDims:
         self.scale = 1.0 / math.sqrt(self.hd)
 
 
-def gpt_layer_fwd(W, pre, x, g, B, S, train_w=False, drop=None, li=0, compute_out=True):
+def gpt_layer_fwd(W, pre, x, g, B, S, train_w=False, drop=None, li=0, compute_out=True, attend=None):
     """GPT3ParallelTransformerLayer.forward - models/modeling_distributed_gpt3.py:1034-1089
     (causal mask over the whole [prefix|text] sequence, :1329-1332; `drop`: GptDrop or None, li: layer index).
-    compute_out=False skips the dense_4h_to_h GEMM and returns None as the output (the recompute in gpt_bwd)."""
+    compute_out=False skips the dense_4h_to_h GEMM and returns None as the output (the recompute in gpt_bwd).
+    attend(qkv, att): a forward-only attention step over the packed [q|k|v] rows of x in place of the causal one over
+    B dense sequences of S rows (gpt_fwd_shared_prefix); such a layer has no backward, so act' is not stored."""
     H, hd = g.H, g.hd
     c = Ctx()
     d_at = drop.attn(li) if drop else None
@@ -558,15 +560,18 @@ def gpt_layer_fwd(W, pre, x, g, B, S, train_w=False, drop=None, li=0, compute_ou
     d_b2 = drop.bda_mlp(li) if drop else None
     ln1, c.m1, c.r1 = ops.layernorm_fwd(x, W[pre + "input_layernorm.weight"], W[pre + "input_layernorm.bias"], g.eps)
     qkv = ops.gemm(ln1, W[pre + "self_attention.query_key_value.weight"], bias=W[pre + "self_attention.query_key_value.bias"])
-    att = torch.empty((B * S, H), device=x.device, dtype=bf16)
-    m = ops.dense_map(S)
-    q, k, v = (TView(qkv, i * hd, 3 * hd, m) for i in range(3))  # rows grouped per head as [q|k|v] (:894-902)
-    c.lse = ops.attn_fwd(q, k, v, TView(att, 0, hd, m), n_seq=B, n_heads=g.heads, head_dim=hd, s_q=S, s_kv=S,
-                         causal=True, scale=g.scale, drop=d_at)
+    att = torch.empty((x.shape[0], H), device=x.device, dtype=bf16)
+    if attend is None:
+        m = ops.dense_map(S)
+        q, k, v = (TView(qkv, i * hd, 3 * hd, m) for i in range(3))  # rows grouped per head as [q|k|v] (:894-902)
+        c.lse = ops.attn_fwd(q, k, v, TView(att, 0, hd, m), n_seq=B, n_heads=g.heads, head_dim=hd, s_q=S, s_kv=S,
+                             causal=True, scale=g.scale, drop=d_at)
+    else:
+        attend(qkv, att)
     x1 = ops.gemm(att, W[pre + "self_attention.dense.weight"], bias=W[pre + "self_attention.dense.bias"], residual=x,
                   out_dtype=torch.float32, drop=d_b1)
     ln2, c.m2, c.r2 = ops.layernorm_fwd(x1, W[pre + "post_attention_layernorm.weight"], W[pre + "post_attention_layernorm.bias"], g.eps)
-    dact = torch.empty((B * S, g.F), device=x.device, dtype=bf16)
+    dact = torch.empty((x.shape[0], g.F), device=x.device, dtype=bf16) if attend is None else None
     h = ops.gemm(ln2, W[pre + "mlp.dense_h_to_4h.weight"], bias=W[pre + "mlp.dense_h_to_4h.bias"], act=ACT_GELU_TANH, aux_out=dact)
     out = None
     if compute_out:
@@ -641,6 +646,48 @@ def gpt_fwd(W, x, gcfg, B, S, train_w=False, save=True, out_rows=None, drop=None
     if save:
         c.xL = x
     return hid, c
+
+
+def shared_prefix_maps(V, t, Q, L):
+    """Sequence maps of gpt_fwd_shared_prefix's attention over rows [N*L text rows | V*Q prefix rows] (N = V*t,
+    sequence n uses prefix n // t): (text rows, keys of a text sequence = its video's prefix then its own text rows,
+    prefix rows)."""
+    N = V * t
+    keys = ops.seqmap(seq_div=t, outer_stride=t * L, inner_stride=L, pos_stride=1, n_prefix=Q, prefix_base=N * L,
+                      prefix_stride=Q, prefix_per_seq=0)
+    return ops.dense_map(L), keys, ops.dense_map(Q)
+
+
+def gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, L, out_rows=None):
+    """Forward-only decoder pass over V prefixes of Q rows, each followed by t texts of L rows (the scoring evaluations:
+    N = V*t sequences [prefix v | text n], v = n // t), without repeating the prefixes.
+    x [N*L + V*Q, H] fp32: rows n*L + j are the text embeddings + positions Q + j, rows N*L + v*Q + i the prefix
+    embeddings + positions i.  Causal attention lets no prefix row see a text row, so each layer runs its LayerNorms
+    and GEMMs once over all rows and attends twice over its packed QKV: square causal over the prefixes, then the text
+    rows causally after their video's prefix (s_q = L < s_kv = Q + L).  Every kernel computes each row on its own, so
+    the text rows are bit-identical to the same rows of gpt_fwd on the repeated [N, Q + L] layout.
+    Returns the final-LayerNorm hidden states of out_rows (int32 indices into x's rows; default: all text rows)."""
+    g = GptDims(gcfg)
+    N, hd = V * t, g.hd
+    T = N * L
+    assert x.shape == (T + V * Q, g.H) and x.dtype == torch.float32
+    m_txt, m_keys, m_pre = shared_prefix_maps(V, t, Q, L)
+
+    def attend(qkv, att):
+        pq, pa = qkv[T:], att[T:]
+        ops.attn_fwd(*(TView(pq, i * hd, 3 * hd, m_pre) for i in range(3)), TView(pa, 0, hd, m_pre), n_seq=V,
+                     n_heads=g.heads, head_dim=hd, s_q=Q, s_kv=Q, causal=True, scale=g.scale)
+        ops.attn_fwd(TView(qkv, 0, 3 * hd, m_txt), TView(qkv, hd, 3 * hd, m_keys), TView(qkv, 2 * hd, 3 * hd, m_keys),
+                     TView(att, 0, hd, m_txt), n_seq=N, n_heads=g.heads, head_dim=hd, s_q=L, s_kv=Q + L, causal=True,
+                     scale=g.scale)
+
+    for i in range(g.layers):
+        x, _ = gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", x, g, None, None, attend=attend)
+    if out_rows is None:
+        out_rows = torch.arange(T, device=x.device, dtype=torch.int32)
+    hid, _, _ = ops.layernorm_fwd(x, W[GPT + "encoder.final_layernorm.weight"], W[GPT + "encoder.final_layernorm.bias"], g.eps,
+                                  in_rows=out_rows)
+    return hid
 
 
 def gpt_layer_saved(W, c, i):

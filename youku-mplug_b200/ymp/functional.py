@@ -128,6 +128,12 @@ def gpt_drop(gcfg, dev):
     return engine.GptDrop(_pass_rng(dev), ph, pa)
 
 
+def gpt_dropout_active(gcfg):
+    """Would gpt_drop draw masks for a pass with this config (without drawing them)?"""
+    return bool(gcfg.get("training", False)) and (float(gcfg.get("hidden_dropout", 0.0) or 0.0) > 0.0
+                                                  or float(gcfg.get("attention_dropout", 0.0) or 0.0) > 0.0)
+
+
 def _vit_recompute(vcfg):
     """TimeSformer grad_ckpt: recompute every block's activations in the backward instead of keeping them."""
     return bool(vcfg.get("grad_ckpt", False))
@@ -461,3 +467,37 @@ class GptFn(torch.autograd.Function):
         if pk in G:
             G[pk].view(-1, H)[:S].add_(dx.view(B, S, H).float().sum(0))
         return (dx.view(B, S, H).to(ctx.in_dtype), None, None, None, None) + store.grads(keys, params)
+
+
+def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, keys, params):
+    """Forward-only decoder pass over [prefix v | text n] for N = V*t texts, text n after prefix v = n // t, with each
+    prefix computed once (engine.gpt_fwd_shared_prefix).  query_embeds [V,Q,H], input_embeds [N,L,H] (positions NOT
+    yet added, the same dtype chain as GptFn on the concatenation), labels [N,L] of the text positions or None,
+    hidden_rows: int tensor of text rows n*L + j whose final hidden states are wanted, or None.
+    Returns (losses [N,L] fp32 or None, hidden [len(hidden_rows), H] bf16 or None); text position j of sequence n is
+    bit-identical to position Q + j of GptFn on the repeated [N, Q+L] layout."""
+    _require_cuda(input_embeds, "gpt_shared_prefix")
+    if gpt_dropout_active(gcfg):
+        raise ValueError("gpt_shared_prefix: the decoder's dropout is active; the shared-prefix pass is for evaluation")
+    W = {k: as_bf16(p) for k, p in zip(keys, params)}
+    V, Q, H = query_embeds.shape
+    N, L, _ = input_embeds.shape
+    if V == 0 or N % V:
+        raise ValueError(f"gpt_shared_prefix: {N} texts do not split evenly over {V} prefixes")
+    T = N * L
+    pos = W[engine.GPT + "embedding.position_embeddings.weight"]
+    x = torch.empty((T + V * Q, H), device=input_embeds.device, dtype=torch.float32)  # [text rows | prefix rows]
+    x[:T] = (input_embeds.float() + pos[Q:Q + L][None].float()).reshape(T, H)
+    x[T:] = (query_embeds.float() + pos[:Q][None].float()).reshape(V * Q, H)
+    rows = None if hidden_rows is None else hidden_rows.to(device=x.device, dtype=torch.int32).contiguous()
+    with torch.no_grad():
+        hid = engine.gpt_fwd_shared_prefix(W, x, gcfg, V, N // V, Q, L, out_rows=None if labels is not None else rows)
+        losses = hidden = None
+        if labels is not None:
+            _, losses, _ = engine.lm_head_fwd(W, hid, labels.contiguous())
+            losses = losses.view(N, L)
+            if rows is not None:
+                hidden = hid.index_select(0, rows.long())
+        else:
+            hidden = hid
+    return losses, hidden
