@@ -132,8 +132,14 @@ typedef struct ymp_gemm_args {
 int ymp_gemm(const ymp_gemm_args* a, void* stream);
 
 /* Skinny GEMM for single-token decoding (KV-cache steps of sample() / beam_search(),
- * models/modeling_distributed_gpt3.py:1620-1886): y[M, N] = epilogue(x[M, K] . w[N, K]^T), 1 <= M <= 8.  One pass over the
- * weights, HBM-bound, no tensor cores (csrc/gemv.cu).  Epilogue: + bias[n], act (YMP_ACT_*), + residual[m, n], store. */
+ * models/modeling_distributed_gpt3.py:1620-1886): y[M, N] = epilogue(x[M, K] . w[N, K]^T).  One pass over the weights on
+ * mma.sync tensor-core instructions fed straight from global memory (csrc/gemv.cu).  Epilogue: + bias[n], act
+ * (YMP_ACT_*), + residual[m, n], store.
+ *   ymp_gemm_skinny      : 1 <= M <= 8 (one beam search, sample()).
+ *   ymp_gemm_skinny_wide : 1 <= M <= 64 (a batched beam search: clips x beams).  M <= 8 runs exactly the launch of
+ *                          ymp_gemm_skinny; 9 <= M <= 64 a kernel with the same per-element arithmetic, so row m of the
+ *                          result is bit-identical to the same row computed by any call with the same N and K.  The
+ *                          fused LayerNorm (ln_out) needs M <= 8; M > 64 is rejected. */
 typedef struct ymp_gemm_skinny_args {
   const void* x;         /* bf16 [M, K], row stride ldx */
   const void* w;         /* bf16 [N, K], row stride ldw (an nn.Linear weight) */
@@ -158,6 +164,7 @@ typedef struct ymp_gemm_skinny_args {
   float ln_eps;
 } ymp_gemm_skinny_args;
 int ymp_gemm_skinny(const ymp_gemm_skinny_args* a, void* stream);
+int ymp_gemm_skinny_wide(const ymp_gemm_skinny_args* a, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * LayerNorm (fp32 statistics, bf16 in/out), one warp per row.

@@ -1,27 +1,35 @@
-// Skinny GEMM for single-token decoding (SURVEY.md 8f N2): y[M, N] = epilogue(x[M, K] . w[N, K]^T) with M <= 8 rows
-// (beam width / decode batch).  Replaces the GPT-3 layer's linears at the KV-cache step of
-// models/modeling_distributed_gpt3.py:868-938,580-595,1348-1350.  With a handful of rows the work is one pass over
-// the weight matrix: HBM-bound.  A 128-row tensor-core tile would occupy N/128 CTAs (16 for N = 2048) and stream the
-// weights at a fraction of the memory bandwidth; a CUDA-core dot product needs ~2.5 issue slots per weight byte-pair
-// (bf16 -> fp32 converts + FMAs for every row) and is issue-bound at a quarter of the bandwidth.  So:
-//   * a warp owns 8 output columns and one K slice and feeds mma.sync.m16n8k16 (bf16, fp32 accumulate) STRAIGHT FROM
-//     GLOBAL MEMORY: lane (g, t) loads 16 bytes (8 consecutive k) of weight row n0+g and of activation row g.  The
-//     tensor-core fragment wants k = {2t, 2t+1, 2t+8, 2t+9} per lane - but a dot product does not care in which order
-//     k is summed as long as both operands use the same order, so the 8 consecutive elements are simply declared to be
-//     those positions of two k-steps (a k permutation inside each 32-element block).  No shared memory, no converts:
-//     two loads and two MMAs per 16 weight bytes per lane.  x is the A operand (rows >= M are zero registers);
-//   * the 8 warps of a CTA are `ksplit` K-slices x (8 / ksplit) column tiles; every lane keeps UNROLL k-blocks
-//     (UNROLL x 16 bytes of weights) in flight, ~8 CTAs resident per SM;
-//   * partial sums meet in shared memory; lane (g, t) of the slice-0 warp owns (row g, columns n0+2t, n0+2t+1) and applies
+// Skinny GEMM for single-token decoding (SURVEY.md 8f N2): y[M, N] = epilogue(x[M, K] . w[N, K]^T) with M <= 64 rows
+// (beam width / decode batch; a batched beam search over several clips).  Replaces the GPT-3 layer's linears at the
+// KV-cache step of models/modeling_distributed_gpt3.py:868-938,580-595,1348-1350.  With a handful of rows the work is
+// one pass over the weight matrix: HBM-bound.  A 128-row tensor-core tile would occupy N/128 CTAs (16 for N = 2048) and
+// stream the weights at a fraction of the memory bandwidth; a CUDA-core dot product needs ~2.5 issue slots per weight
+// byte-pair (bf16 -> fp32 converts + FMAs for every row) and is issue-bound at a quarter of the bandwidth.  So:
+//   * a warp owns 8 output columns and one K slice and feeds tensor-core mma.sync.m16n8k16 (bf16, fp32 accumulate)
+//     STRAIGHT FROM GLOBAL MEMORY: lane (g, t) loads 16 bytes (8 consecutive k) of weight row n0+g and of activation
+//     row g.  The tensor-core fragment wants k = {2t, 2t+1, 2t+8, 2t+9} per lane - but a dot product does not care in
+//     which order k is summed as long as both operands use the same order, so the 8 consecutive elements are simply
+//     declared to be those positions of two k-steps (a k permutation inside each 32-element block).  No shared memory,
+//     no converts: two loads and two MMAs per 16 weight bytes per lane.  x is the A operand;
+//   * M <= 8 (gemm_skinny_kernel): rows 8..15 of the A operand are zero registers;
+//     9 <= M <= 64 (gemm_skinny_wide_kernel): the same warp layout, K slices, k permutation and k-block loop, but each
+//     weight fragment (the B operand) feeds one MMA per group of 16 activation rows, whose a1/a3 registers carry rows
+//     8..15 of the group.  Every output element sees the same MMA chain and the same epilogue as in an M <= 8 call, so
+//     row r of an M-row call is bit-identical to the same row computed alone;
+//   * the 8 warps of a CTA are `ksplit` K-slices x (8 / ksplit) column tiles (ksplit depends on N and K only); every lane
+//     keeps UNROLL k-blocks (UNROLL x 16 bytes of weights) in flight;
+//   * partial sums meet in shared memory and are added in slice order; lane (g, t) of the slice-0 warp owns (row g (+8,
+//     +16, ...), columns n0+2t, n0+2t+1) and applies
 //       v = acc + bias[n] ; v = gelu(v) (optional) ; v += residual[m, n] (bf16 or fp32) ; store bf16 or fp32
 //     (+ an optional second bf16 copy at a device-side row offset: the KV-cache row of the new token).
-// Algorithmic bytes per call: N*K*2 (weights) + M*(K + N)*2..4.
+// Algorithmic bytes per call: N*K*2 (weights) + M*(K + N)*2..4.  The wide kernel re-reads the activations once per
+// 8-column tile (from L2): M*K*2 * N/8 bytes of L2 traffic, 8x the weight bytes at M = 64.
 #include "common.h"
 #include "ptx.cuh"
 
 namespace ymp {
 
 constexpr int SK_MAXM = 8, SK_TILE_N = 8, SK_WARPS = 8;
+constexpr int SK_WIDE_MAXM = 64, SK_WIDE_GROUPS = SK_WIDE_MAXM / 16;
 
 struct SkinnyParams {
   const __nv_bfloat16* x;
@@ -116,6 +124,25 @@ __device__ __forceinline__ void skinny_ln_rows(const SkinnyParams& p, float* red
   skinny_ln_pass<2>(p, mu, rs, red);
 }
 
+// Epilogue of result row m, columns n, n + 1 (the accumulators of one lane): identical for both kernels
+__device__ __forceinline__ void skinny_store(const SkinnyParams& p, int m, int n_base, float acc0, float acc1) {
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int n = n_base + e;
+    if (n >= p.N) continue;
+    float v = e ? acc1 : acc0;
+    if (p.bias) v += __bfloat162float(p.bias[n]);
+    if (p.act == YMP_ACT_GELU_TANH) v = gelu_tanh(v);
+    else if (p.act == YMP_ACT_GELU_ERF) v = gelu_erf(v);
+    if (p.residual)
+      v += p.res_f32 ? reinterpret_cast<const float*>(p.residual)[(size_t)m * p.ldr + n]
+                     : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[(size_t)m * p.ldr + n]);
+    if (p.out_f32) reinterpret_cast<float*>(p.y)[(size_t)m * p.ldy + n] = v;
+    else reinterpret_cast<__nv_bfloat16*>(p.y)[(size_t)m * p.ldy + n] = __float2bfloat16(v);
+    if (p.y2) p.y2[(long long)m * p.ldy2 + *p.y2_off * p.y2_stride + n] = __float2bfloat16(v);
+  }
+}
+
 __device__ __forceinline__ void mma16816_bf16(float (&c)[4], uint32_t a0, uint32_t a2, uint32_t b0, uint32_t b1) {
   // rows 8..15 of the A operand (a1, a3) are zero: only M <= 8 activation rows exist
   asm volatile(
@@ -187,21 +214,7 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (LN ? 2 : 1)) gemm_skinny_kerne
       for (int j = 1; j < ks; ++j) { acc[0] += part[warp + j][2 * lane]; acc[1] += part[warp + j][2 * lane + 1]; }
   }
   if (live && kpart == 0 && g < p.M) {
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int n = n0 + 2 * t + e;
-      if (n >= p.N) continue;
-      float v = acc[e];
-      if (p.bias) v += __bfloat162float(p.bias[n]);
-      if (p.act == YMP_ACT_GELU_TANH) v = gelu_tanh(v);
-      else if (p.act == YMP_ACT_GELU_ERF) v = gelu_erf(v);
-      if (p.residual)
-        v += p.res_f32 ? reinterpret_cast<const float*>(p.residual)[(size_t)g * p.ldr + n]
-                       : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[(size_t)g * p.ldr + n]);
-      if (p.out_f32) reinterpret_cast<float*>(p.y)[(size_t)g * p.ldy + n] = v;
-      else reinterpret_cast<__nv_bfloat16*>(p.y)[(size_t)g * p.ldy + n] = __float2bfloat16(v);
-      if (p.y2) p.y2[(long long)g * p.ldy2 + *p.y2_off * p.y2_stride + n] = __float2bfloat16(v);
-    }
+    skinny_store(p, g, n0 + 2 * t, acc[0], acc[1]);
     if (LN) __threadfence();   // this thread's rows are visible device-wide before its CTA takes a ticket
   }
   if constexpr (LN) {
@@ -219,13 +232,103 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (LN ? 2 : 1)) gemm_skinny_kerne
   }
 }
 
+__device__ __forceinline__ void mma16816_bf16_rows16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                     uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// 9 <= M <= 64: gemm_skinny_kernel's grid, warp roles, K slices, weight stream and k-block loop (SK_UNROLL = 4, the same
+// zero-padded tail), with one accumulator set per group of 16 rows.  Group j's lane (g, t) holds rows 16j + g (acc[j][0..1])
+// and 16j + 8 + g (acc[j][2..3]).  The activation chunks of the k-block being consumed are loaded from global memory
+// (L2-resident: every CTA reads them) next to the MMAs; only the weights are double-buffered in registers.
+template <int SK_UNROLL>
+__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(const SkinnyParams p) {
+  __shared__ float part[SK_WARPS][32 * 4 * SK_WIDE_GROUPS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int g = lane >> 2, t = lane & 3;
+  const int ks = p.ksplit, kpart = warp % ks, tile = blockIdx.x * (SK_WARPS / ks) + warp / ks;
+  const int n0 = tile * SK_TILE_N;
+  const int groups = (p.M + 15) >> 4;
+  const bool live = n0 < p.N;
+  float acc[SK_WIDE_GROUPS][4];
+#pragma unroll
+  for (int j = 0; j < SK_WIDE_GROUPS; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+  griddep_launch();
+  if (live) {
+    const int nchunk = p.K >> 3, nblk = (nchunk + 3) >> 2;
+    const int b_lo = (int)((long)nblk * kpart / ks), b_hi = (int)((long)nblk * (kpart + 1) / ks);
+    const uint4* wr = reinterpret_cast<const uint4*>(p.w + (size_t)min(n0 + g, p.N - 1) * p.ldw);
+    uint4 wv[SK_UNROLL];
+    auto fetch_w = [&](int b, uint4 (&wd)[SK_UNROLL]) {
+#pragma unroll
+      for (int u = 0; u < SK_UNROLL; ++u) {
+        const int c = (b + u) * 4 + t;
+        wd[u] = ((b + u) < b_hi && c < nchunk) ? ld_nc_v4(wr + c) : make_uint4(0, 0, 0, 0);
+      }
+    };
+    // activation chunk c of row r (zero past the slice, past K and for rows >= M)
+    auto fetch_x = [&](int r, int b, int c) {
+      return (b < b_hi && c < nchunk && r < p.M) ? __ldg(reinterpret_cast<const uint4*>(p.x + (size_t)r * p.ldx) + c)
+                                                 : make_uint4(0, 0, 0, 0);
+    };
+    fetch_w(b_lo, wv);
+    griddep_wait();
+    for (int b = b_lo; b < b_hi; b += SK_UNROLL) {
+      uint4 wn[SK_UNROLL];
+      fetch_w(b + SK_UNROLL, wn);
+#pragma unroll
+      for (int u = 0; u < SK_UNROLL; ++u) {
+        const int c = (b + u) * 4 + t;
+#pragma unroll
+        for (int j = 0; j < SK_WIDE_GROUPS; ++j) {
+          if (j < groups) {
+            const uint4 lo = fetch_x(16 * j + g, b + u, c), hi = fetch_x(16 * j + 8 + g, b + u, c);
+            mma16816_bf16_rows16(acc[j], lo.x, hi.x, lo.y, hi.y, wv[u].x, wv[u].y);
+            mma16816_bf16_rows16(acc[j], lo.z, hi.z, lo.w, hi.w, wv[u].z, wv[u].w);
+          }
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < SK_UNROLL; ++u) wv[u] = wn[u];
+    }
+  } else {
+    griddep_wait();
+  }
+  if (ks > 1) {
+#pragma unroll
+    for (int j = 0; j < SK_WIDE_GROUPS; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) part[warp][(j * 4 + e) * 32 + lane] = acc[j][e];
+    __syncthreads();
+    if (kpart == 0)
+      for (int s = 1; s < ks; ++s)
+#pragma unroll
+        for (int j = 0; j < SK_WIDE_GROUPS; ++j)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) acc[j][e] += part[warp + s][(j * 4 + e) * 32 + lane];
+  }
+  if (live && kpart == 0) {
+#pragma unroll
+    for (int j = 0; j < SK_WIDE_GROUPS; ++j) {
+      if (16 * j + g < p.M) skinny_store(p, 16 * j + g, n0 + 2 * t, acc[j][0], acc[j][1]);
+      if (16 * j + 8 + g < p.M) skinny_store(p, 16 * j + 8 + g, n0 + 2 * t, acc[j][2], acc[j][3]);
+    }
+  }
+}
+
 }  // namespace ymp
 
 using namespace ymp;
 
-extern "C" int ymp_gemm_skinny(const ymp_gemm_skinny_args* a, void* stream) {
+// ymp_gemm_skinny (max_m = 8) and ymp_gemm_skinny_wide (max_m = 64): the same arguments, checks and M <= 8 launch
+static int gemm_skinny_call(const ymp_gemm_skinny_args* a, void* stream, int max_m) {
   YMP_CHECK_ARG(a && a->x && a->w && a->y, "ymp_gemm_skinny: null pointer");
-  YMP_CHECK_ARG(a->M >= 1 && a->M <= SK_MAXM && a->N > 0 && a->K > 0 && a->K % 8 == 0, "ymp_gemm_skinny: needs 1 <= M <= 8, K %% 8 == 0 (M=%d K=%d)", a->M, a->K);
+  YMP_CHECK_ARG(a->M >= 1 && a->M <= max_m && a->N > 0 && a->K > 0 && a->K % 8 == 0, "ymp_gemm_skinny%s: needs 1 <= M <= %d, K %% 8 == 0 (M=%d K=%d)",
+                max_m > SK_MAXM ? "_wide" : "", max_m, a->M, a->K);
+  YMP_CHECK_ARG(!a->ln_out || a->M <= SK_MAXM, "ymp_gemm_skinny_wide: the fused LayerNorm (ln_out) needs M <= 8 (M=%d)", a->M);
   YMP_CHECK_ARG(a->ldx % 8 == 0 && a->ldw % 8 == 0 && a->ldx >= a->K && a->ldw >= a->K && aligned16(a->x) && aligned16(a->w), "ymp_gemm_skinny: x / w rows must be 16-byte aligned");
   YMP_CHECK_ARG(a->act >= 0 && a->act <= 2, "ymp_gemm_skinny: bad act");
   SkinnyParams p;
@@ -252,10 +355,17 @@ extern "C" int ymp_gemm_skinny(const ymp_gemm_skinny_args* a, void* stream) {
   const int blocks = (tiles + tiles_per_cta - 1) / tiles_per_cta;
   static const int unroll = [] { const char* e = getenv("YMP_SKINNY_UNROLL"); return e ? atoi(e) : 4; }();
   cudaStream_t st = (cudaStream_t)stream;
-  if (ln) launch_k(gemm_skinny_kernel<4, true>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
+  if (a->M > SK_MAXM) launch_k(gemm_skinny_wide_kernel<4>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
+  else if (ln) launch_k(gemm_skinny_kernel<4, true>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
   else if (unroll == 8) launch_k(gemm_skinny_kernel<8, false>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
   else if (unroll == 2) launch_k(gemm_skinny_kernel<2, false>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
   else launch_k(gemm_skinny_kernel<4, false>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
+}
+
+extern "C" int ymp_gemm_skinny(const ymp_gemm_skinny_args* a, void* stream) { return gemm_skinny_call(a, stream, SK_MAXM); }
+
+extern "C" int ymp_gemm_skinny_wide(const ymp_gemm_skinny_args* a, void* stream) {
+  return gemm_skinny_call(a, stream, SK_WIDE_MAXM);
 }

@@ -291,15 +291,14 @@ class DistributedGPT3_Caption(_PrefixModelBase):
     @torch.no_grad()
     def generate(self, image, text):
         """Per-sample beam search (beam 5) over the visual prefix (:790-809): list of [1, len] LongTensors on
-        the CPU.  prompt_length = attention_mask.sum(-1) - 1, stop token = the tokenizer's <|endoftext|>."""
+        the CPU.  prompt_length = attention_mask.sum(-1) - 1, stop token = the tokenizer's <|endoftext|>.
+        All clips are decoded together (DistributedGPT3.beam_search with B > 1: one decoding step serves up to
+        64 // beam clips); each result equals the beam search of that clip alone."""
         _, _, _, query_features = self.visual_prefix(image)
         eos = self.tokenizer.tokenizer.eos if self.tokenizer is not None else self.text_decoder.config.eod_id
-        res = []
-        for i in range(len(text.input_ids)):
-            out = self.text_decoder.generate(text.input_ids[i:i + 1], query_embeds=query_features[i:i + 1], termination_id=eos,
-                                             do_sample=False, prompt_length=text.attention_mask.sum(-1)[i] - 1)
-            res.append(out.sequences.cpu())
-        return res
+        out = self.text_decoder.generate(text.input_ids, query_embeds=query_features, termination_id=eos, do_sample=False,
+                                         prompt_length=text.attention_mask.sum(-1) - 1)
+        return [o.sequences.cpu() for o in (out if isinstance(out, list) else [out])]
 
 
 class _PromptClsBase(_PrefixModelBase):

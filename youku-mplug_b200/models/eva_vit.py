@@ -67,7 +67,7 @@ class VisionTransformer(nn.Module):
         assert H == self.image_size and W == self.image_size, \
             f"Input image size ({H}*{W}) doesn't match model ({self.image_size}*{self.image_size})."
         keys, params = named_param_list(self, "visual_encoder.")
-        return YF.EvaFn.apply(x, self.ecfg, keys, *params)
+        return YF.EvaFn.apply(x, self.ecfg, torch.is_grad_enabled(), keys, *params)
 
     def forward(self, x):
         x = self.forward_features(x)

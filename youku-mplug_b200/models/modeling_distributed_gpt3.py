@@ -324,6 +324,11 @@ class InferenceParams:
         self.key_value_memory_dict = {}
         self.cache = None
         self.token_step = None   # ymp.engine.TokenStep once this call's single-token steps have been validated
+        # batched beam search: single-token steps of up to ops.SKINNY_WIDE_MAX_ROWS rows run the captured skinny step
+        # (otherwise rows beyond ops.SKINNY_MAX_ROWS take the tensor-core path), and the first call fills cache slot
+        # b * prefill_stride from input row b
+        self.wide_step = False
+        self.prefill_stride = 1
 
     def swap_key_value_dict(self, batch_idx):
         'swap between batches'
@@ -454,6 +459,92 @@ def run_beam_search(step, reorder, tokens, prompt_length, n_query, *, beam_size,
     best = sorted(pool.beams, key=lambda x: float(x[0]), reverse=True)[:min(num_return_gen, len(pool.beams))]
     return AttrDict(sequences=torch.stack([h for _, h, _ in best], dim=0),
                     scores=torch.stack([torch.as_tensor(sc, device=dev).reshape(-1)[0] for sc, _, _ in best], dim=0))
+
+def run_beam_search_batched(step, reorder, tokens, prompt_length, n_query, *, beam_size, num_return_gen, stop_token,
+                            tokens_to_generate, max_position_embeddings):
+    """run_beam_search for B clips at once (tokens [B, L], one prompt length) over one decode callback with B*beam rows:
+    clip c owns rows c*beam .. c*beam + beam - 1.  Each clip keeps its own ranking, BeamHypotheses and stopping rule,
+    so its result equals run_beam_search on that clip alone.  A step sorts every clip's candidates in one device sort
+    and copies the top 2*beam of all clips to the host in one transfer.  Rows of a finished clip keep stepping and are
+    never read; the loop ends when every clip is done or the length limit is reached.
+    step(new_tokens [B*beam, n], first) -> logits [B*beam, V] (the first call may return one row per clip, [B, V]);
+    reorder(idx [B*beam]) permutes the callback's KV cache.  Returns a list of B AttrDict(sequences, scores)."""
+    B, dev = tokens.size(0), tokens.device
+    tokens = torch.cat((tokens, torch.full((B, tokens_to_generate), stop_token, dtype=torch.long, device=dev)), dim=-1)
+    final_len = min(tokens.size(1), max_position_embeddings)
+    if prompt_length >= final_len:
+        raise ValueError('context length + tokens_to_generate too large')
+    pools = [BeamHypotheses(beam_size) for _ in range(B)]
+    done = [False] * B
+    scores = torch.zeros(B * beam_size, 1, dtype=torch.float32, device=dev)
+    tokens = tokens.repeat_interleave(beam_size, dim=0)
+    top = 2 * beam_size
+    prev = 0
+    ctx = prompt_length
+    for ctx in range(prompt_length, final_len):
+        first = ctx == prompt_length
+        logits = step(tokens[:, prev:ctx], first)
+        vocab = logits.size(-1)
+        if first:  # identical beams: only the first beam of every clip is ranked
+            cand = torch.log_softmax(logits.view(B, -1, vocab)[:, 0].float(), dim=-1) + scores.view(B, beam_size)[:, :1]
+        else:
+            cand = (torch.log_softmax(logits.float(), dim=-1) + scores).view(B, -1)
+        ranked_scores, ranked = torch.sort(cand, dim=-1, descending=True)
+        ranked, ranked_scores = ranked[:, :top], ranked_scores[:, :top]
+        host = torch.cat((ranked.double(), ranked_scores.double()), dim=1).cpu()   # indices < 2**53 and fp32 are exact
+        idx = host[:, :top].long()
+        beam_of, word_of = torch.div(idx, vocab, rounding_mode='floor').tolist(), (idx % vocab).tolist()
+        best_score = host[:, top:].max(dim=1).values.tolist()
+        keep, words, picked = [], [], []
+        for c in range(B):
+            base = c * beam_size
+            if not done[c]:
+                survivors = []
+                for rank, (word, beam) in enumerate(zip(word_of[c], beam_of[c])):
+                    if word == stop_token:
+                        if rank >= beam_size:  # a finished hypothesis outside the top beam_size candidates is dropped
+                            continue
+                        pools[c].add(tokens[base + beam].clone(), ranked_scores[c, rank], ctx + 1 - prompt_length)
+                    else:
+                        survivors.append((word, rank, beam))
+                    if len(survivors) == beam_size:
+                        break
+                done[c] = pools[c].is_done(best_score[c], ctx + 1 - prompt_length)
+            if done[c]:  # rows that are never read again: keep them in place
+                survivors = [(stop_token, b, b) for b in range(beam_size)]
+            keep += [base + b for _, _, b in survivors]
+            words += [w for w, _, _ in survivors]
+            picked += [c * top + r for _, r, _ in survivors]
+        if all(done):
+            break
+        keep = torch.tensor(keep, dtype=torch.long, device=dev)
+        tokens = tokens[keep, :]
+        tokens[:, ctx] = torch.tensor(words, dtype=torch.long, device=dev)
+        scores = ranked_scores.reshape(-1)[torch.tensor(picked, dtype=torch.long, device=dev)].reshape(-1, 1).float()
+        reorder(keep)
+        prev = ctx
+    out = []
+    for c in range(B):
+        pool, base = pools[c], c * beam_size
+        if not done[c]:
+            for b in range(beam_size):
+                pool.add(tokens[base + b].clone(), scores[base + b], ctx + 1 - prompt_length)
+        best = sorted(pool.beams, key=lambda x: float(x[0]), reverse=True)[:min(num_return_gen, len(pool.beams))]
+        out.append(AttrDict(sequences=torch.stack([h for _, h, _ in best], dim=0),
+                            scores=torch.stack([torch.as_tensor(sc, device=dev).reshape(-1)[0] for sc, _, _ in best], dim=0)))
+    return out
+
+
+def beam_search_chunks(prompt_lengths, beam_size, max_rows):
+    """How a batched beam search splits its clips: clips grouped by prompt length (in order of first appearance),
+    each group cut into chunks of at most max_rows // beam_size clips.  Returns [(prompt_length, [clip indices])]."""
+    per = max_rows // beam_size
+    if per < 1:
+        raise ValueError(f"beam_size {beam_size} exceeds the {max_rows} rows of one decoding step")
+    groups = {}
+    for i, p in enumerate(prompt_lengths):
+        groups.setdefault(int(p), []).append(i)
+    return [(p, idx[s:s + per]) for p, idx in groups.items() for s in range(0, len(idx), per)]
 
 
 class GPT3Model(nn.Module):
@@ -601,8 +692,9 @@ class DistributedGPT3(nn.Module):
             ip.cache.reset()
             ip.key_value_memory_dict = {i + 1: t for i, t in enumerate(ip.cache.qkv)}
         off = ip.sequence_len_offset
-        assert off == ip.cache.len and B == ip.cache.B
-        if n == 1 and off > 0 and B <= ops.SKINNY_MAX_ROWS:
+        stride = ip.prefill_stride if off == 0 else 1
+        assert off == ip.cache.len and B * stride == ip.cache.B
+        if n == 1 and off > 0 and B <= (ops.SKINNY_WIDE_MAX_ROWS if ip.wide_step else ops.SKINNY_MAX_ROWS):
             # single-token step: skinny GEMMs + device-side cache length, replayed as one CUDA graph
             sig = (params[0].data_ptr(), params[-1].data_ptr(), sum(p._version for p in params))
             ts = ip.cache.token
@@ -621,7 +713,7 @@ class DistributedGPT3(nn.Module):
             W = {k: YF.as_bf16(p) for k, p in zip(keys, params)}
             pos = W[engine.GPT + "embedding.position_embeddings.weight"]
             x = (input_embeds.float() + pos[off:off + n][None].float()).reshape(B * n, H).contiguous()
-            hid = engine.gpt_decode(W, x, ip.cache, n)
+            hid = engine.gpt_decode(W, x, ip.cache, n, seq_stride=stride)
             logits = ops.gemm(hid, W[engine.GPT + "embedding.word_embeddings.weight"]).float()
         ip.sequence_len_offset += n  # tokens.size(1) + query_embeds.size(1) of the reference
         return AttrDict(logits=logits.view(B, 1, -1), loss=None, losses=None, last_hidden_state=hid.view(B, 1, H))
@@ -654,12 +746,16 @@ class DistributedGPT3(nn.Module):
 
     @torch.no_grad()
     def beam_search(self, tokens, query_embeds=None, beam_size=5, num_return_gen=1, stop_token=None, **kwargs):
-        """Beam search for one sample (:1743-1875): Dict(sequences [n, len], scores [n])."""
+        """Beam search (:1743-1875).  One sample (tokens [1, L]): Dict(sequences [n, len], scores [n]).
+        B > 1 samples (prompt_length an int or a [B] tensor): a list of B such Dicts, each equal to the call for that
+        sample alone, computed by batched beam searches over chunks of samples that share a prompt length."""
         cfg = self.config
-        assert tokens.size(0) == 1
-        prompt_length = int(kwargs.pop('prompt_length', tokens.size(1)))
+        prompt_length = kwargs.pop('prompt_length', tokens.size(1))
         if stop_token is None:
             stop_token = cfg.eod_id
+        if tokens.size(0) > 1:
+            return self._beam_search_batched(tokens, query_embeds, beam_size, num_return_gen, stop_token, prompt_length)
+        prompt_length = int(prompt_length)
         nq = 0 if query_embeds is None else query_embeds.size(1)
         final_len = min(tokens.size(1) + cfg.tokens_to_generate, cfg.max_position_embeddings)
         self.inference_params = InferenceParams(beam_size, final_len + nq)
@@ -668,6 +764,35 @@ class DistributedGPT3(nn.Module):
         return run_beam_search(step, reorder, tokens, prompt_length, nq, beam_size=beam_size, num_return_gen=num_return_gen,
                                stop_token=stop_token, tokens_to_generate=cfg.tokens_to_generate,
                                max_position_embeddings=cfg.max_position_embeddings)
+
+    def _beam_search_batched(self, tokens, query_embeds, beam_size, num_return_gen, stop_token, prompt_length):
+        from ymp import ops
+        cfg = self.config
+        B = tokens.size(0)
+        lengths = torch.as_tensor(prompt_length).reshape(-1).tolist()
+        if len(lengths) == 1:
+            lengths = lengths * B
+        assert len(lengths) == B
+        nq = 0 if query_embeds is None else query_embeds.size(1)
+        final_len = min(tokens.size(1) + cfg.tokens_to_generate, cfg.max_position_embeddings)
+        res = [None] * B
+        for plen, clips in beam_search_chunks(lengths, beam_size, ops.SKINNY_WIDE_MAX_ROWS):
+            sel = torch.tensor(clips, dtype=torch.long, device=tokens.device)
+            ip = self.inference_params = InferenceParams(len(clips) * beam_size, final_len + nq)
+            ip.wide_step, ip.prefill_stride = True, beam_size
+            step, reorder = self._decode_callbacks(None if query_embeds is None else query_embeds[sel])
+
+            def first_beams(new_tokens, first, step=step):
+                # the prefill runs each clip's [prefix | prompt] once, into its first beam slot; the first reorder
+                # copies it to the other slots
+                return step(new_tokens[::beam_size] if first else new_tokens, first)
+            outs = run_beam_search_batched(first_beams, reorder, tokens[sel], plen, nq, beam_size=beam_size,
+                                           num_return_gen=num_return_gen, stop_token=stop_token,
+                                           tokens_to_generate=cfg.tokens_to_generate,
+                                           max_position_embeddings=cfg.max_position_embeddings)
+            for i, o in zip(clips, outs):
+                res[i] = o
+        return res
 
     @torch.no_grad()
     def generate(self, tokens, do_sample=True, termination_id=None, *args, **kwargs):

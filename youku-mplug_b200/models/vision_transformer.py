@@ -101,7 +101,7 @@ class TimeSformer(nn.Module):
         assert H == self.img_size and W == self.img_size, \
             f"Input image size ({H}*{W}) doesn't match model ({self.img_size}*{self.img_size})."
         keys, params = named_param_list(self, "visual_encoder.")
-        return YF.VitFn.apply(x, self.vcfg, keys, *params)
+        return YF.VitFn.apply(x, self.vcfg, torch.is_grad_enabled(), keys, *params)
 
     def forward(self, image_input):
         feats = self.forward_features(image_input)
@@ -146,7 +146,7 @@ class AttentionPool(nn.Module):
             queries_param = x[:1]
         keys, params = named_param_list(self, "attn_pool.")
         keys = ["learnable_queries"] + keys
-        return YF.AttnPoolFn.apply(k, self.num_heads, keys, queries_param, *params)
+        return YF.AttnPoolFn.apply(k, self.num_heads, torch.is_grad_enabled(), keys, queries_param, *params)
 
 
 def _convert_pretrained_vit(vit_pretrained_weights):

@@ -757,8 +757,8 @@ class KVCache:
 
 
 class TokenStep:
-    """The single-token decoding step (n == 1, cache not empty) for at most ops.SKINNY_MAX_ROWS sequences, as ONE CUDA
-    graph: every linear is a skinny GEMM (one pass over its weights, csrc/gemv.cu), the new K/V row goes into the cache
+    """The single-token decoding step (n == 1, cache not empty) for at most ops.SKINNY_WIDE_MAX_ROWS sequences, as ONE
+    CUDA graph: every linear is a skinny GEMM (one pass over its weights, csrc/gemv.cu), the new K/V row goes into the cache
     at the device-side position `len_idx`, attention reads `len1` keys (ymp_attn_args.s_kv_dev), and the graph ends by
     advancing both counters - so one captured graph serves every position of every generate() call that reuses this
     cache.  ~8 kernels per layer; the latency floor is the weight stream (2.6 GB at 1.3B)."""
@@ -798,7 +798,10 @@ class TokenStep:
         # YMP_DECODE_FUSED_LN=1: every LayerNorm but the first is computed by the last CTA of the GEMM that completes its
         # input (one kernel boundary less per sub-layer).  Off by default: the ticket + three L2 round trips of the tail
         # cost about what the stand-alone kernel and its launch gap cost.
-        fused_ln = os.environ.get("YMP_DECODE_FUSED_LN", "0") == "1"
+        # The fused LayerNorm serves at most ops.SKINNY_MAX_ROWS rows.
+        fused_ln = os.environ.get("YMP_DECODE_FUSED_LN", "0") == "1" and B <= ops.SKINNY_MAX_ROWS
+        # more rows than ymp_gemm_skinny takes (a batched beam search): the wide entry point, same per-row results
+        skinny = ops.gemm_skinny if B <= ops.SKINNY_MAX_ROWS else ops.gemm_skinny_wide
 
         def ln_of(prefix):
             return (W[prefix + ".weight"], W[prefix + ".bias"], g.eps, self.ticket)
@@ -806,9 +809,9 @@ class TokenStep:
         def gemm_ln(a, wname, residual, ln_prefix):
             """fp32 residual-stream GEMM followed by the LayerNorm of its complete result: (y, LN(y))."""
             if fused_ln:  # the LayerNorm is computed by the GEMM's last CTA
-                return ops.gemm_skinny(a, W[wname + ".weight"], bias=W[wname + ".bias"], residual=residual, out_dtype=torch.float32,
-                                       ln=ln_of(ln_prefix))
-            y = ops.gemm_skinny(a, W[wname + ".weight"], bias=W[wname + ".bias"], residual=residual, out_dtype=torch.float32)
+                return skinny(a, W[wname + ".weight"], bias=W[wname + ".bias"], residual=residual, out_dtype=torch.float32,
+                              ln=ln_of(ln_prefix))
+            y = skinny(a, W[wname + ".weight"], bias=W[wname + ".bias"], residual=residual, out_dtype=torch.float32)
             return y, ops.layernorm_fwd(y, W[ln_prefix + ".weight"], W[ln_prefix + ".bias"], g.eps, stats=False)[0]
 
         ln1, _, _ = ops.layernorm_fwd(x, W[f"{GPT}encoder.layers.0.input_layernorm.weight"], W[f"{GPT}encoder.layers.0.input_layernorm.bias"],
@@ -818,19 +821,19 @@ class TokenStep:
             st = self.stage
             buf = c.qkv[i]
             # [q|k|v] of the new token: into the staging rows (q for this step) and into cache row b*ML + len (k, v)
-            ops.gemm_skinny(ln1, W[pre + "self_attention.query_key_value.weight"], bias=W[pre + "self_attention.query_key_value.bias"],
-                            out=st, out2=buf, out2_row_stride=ML, out2_off=c.len_idx)
+            skinny(ln1, W[pre + "self_attention.query_key_value.weight"], bias=W[pre + "self_attention.query_key_value.bias"],
+                   out=st, out2=buf, out2_row_stride=ML, out2_off=c.len_idx)
             att = torch.empty((B, H), device=x.device, dtype=bf16)
             q = TView(st, 0, 3 * hd, ops.dense_map(1))
             k, v = TView(buf, hd, 3 * hd, mkv), TView(buf, 2 * hd, 3 * hd, mkv)
             ops.attn_fwd(q, k, v, TView(att, 0, hd, ops.dense_map(1)), n_seq=B, n_heads=g.heads, head_dim=hd, s_q=1, s_kv=ML,
                          causal=False, scale=g.scale, s_kv_dev=c.len1)
             x1, ln2 = gemm_ln(att, pre + "self_attention.dense", x, pre + "post_attention_layernorm")
-            h = ops.gemm_skinny(ln2, W[pre + "mlp.dense_h_to_4h.weight"], bias=W[pre + "mlp.dense_h_to_4h.bias"], act=ACT_GELU_TANH)
+            h = skinny(ln2, W[pre + "mlp.dense_h_to_4h.weight"], bias=W[pre + "mlp.dense_h_to_4h.bias"], act=ACT_GELU_TANH)
             nxt = f"{GPT}encoder.layers.{i + 1}.input_layernorm" if i + 1 < g.layers else GPT + "encoder.final_layernorm"
             x, ln1 = gemm_ln(h, pre + "mlp.dense_4h_to_h", x1, nxt)
         hid = ln1
-        logits = ops.gemm_skinny(hid, W[GPT + "embedding.word_embeddings.weight"], out_dtype=torch.float32)
+        logits = skinny(hid, W[GPT + "embedding.word_embeddings.weight"], out_dtype=torch.float32)
         c.len_idx += 1
         c.len1 += 1
         return hid, logits
@@ -863,13 +866,20 @@ def decode_graph_enabled():
     return os.environ.get("YMP_DECODE_GRAPH", "1") != "0"
 
 
-def gpt_decode(W, x, cache, n):
+def gpt_decode(W, x, cache, n, seq_stride=1):
     """n new positions per sequence through all layers with the KV cache.  x [B*n, H] fp32 = embeddings +
     learned positions of positions cache.len .. cache.len+n-1 (rows b*n + i).  Either the first call
     (cache empty: causal attention inside the block) or single-token steps (n == 1: the query sees every
-    cached key).  Returns the final-LayerNorm hidden state of the LAST new position of every sequence [B, H]."""
-    g, B, ML, off = cache.g, cache.B, cache.max_len, cache.len
+    cached key).  Returns the final-LayerNorm hidden state of the LAST new position of every sequence [B, H].
+    seq_stride > 1 (first call only): x holds B = cache.B / seq_stride sequences and sequence b goes into cache slot
+    b * seq_stride (a batched beam search fills each clip's first beam slot and copies it to the others with
+    KVCache.reorder)."""
+    g, ML, off = cache.g, cache.max_len, cache.len
     H, hd = g.H, g.hd
+    assert cache.B % seq_stride == 0 and (seq_stride == 1 or off == 0)
+    B = cache.B // seq_stride
+    assert x.shape[0] == B * n
+    SL = ML * seq_stride   # cache rows from one sequence to the next
     if off + n > ML:
         raise ValueError(f"KV cache overflow: {off} + {n} > {ML}")
     if off > 0 and n != 1:
@@ -880,10 +890,10 @@ def gpt_decode(W, x, cache, n):
         buf = cache.qkv[i]
         new_rows = buf[off:]  # GEMM row (b, i) -> buffer row b*max_len + off + i
         ops.gemm(ln1, W[pre + "self_attention.query_key_value.weight"], bias=W[pre + "self_attention.query_key_value.bias"],
-                 out=new_rows, d_row_block=n, d_row_stride=ML)
+                 out=new_rows, d_row_block=n, d_row_stride=SL)
         att = torch.empty((B * n, H), device=x.device, dtype=bf16)
-        mq = ops.seqmap(seq_div=1, outer_stride=ML, pos_stride=1)
-        mkv = ops.dense_map(ML)
+        mq = ops.seqmap(seq_div=1, outer_stride=SL, pos_stride=1)
+        mkv = ops.dense_map(SL)
         q = TView(new_rows, 0, 3 * hd, mq)
         k, v = TView(buf, hd, 3 * hd, mkv), TView(buf, 2 * hd, 3 * hd, mkv)
         ops.attn_fwd(q, k, v, TView(att, 0, hd, ops.dense_map(n)), n_seq=B, n_heads=g.heads, head_dim=hd, s_q=n, s_kv=off + n,

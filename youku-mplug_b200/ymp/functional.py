@@ -230,13 +230,15 @@ class PretrainFn(torch.autograd.Function):
 
 
 class VitFn(torch.autograd.Function):
-    """TimeSformer.forward_features: video -> image_embeds [B, 1+T*N, D]."""
+    """TimeSformer.forward_features: video -> image_embeds [B, 1+T*N, D].  grad: the caller's grad mode
+    (torch.is_grad_enabled() where the module is called; inside forward it is always off): without it no block
+    activations are kept."""
 
     @staticmethod
-    def forward(ctx, video, vcfg, keys, *params):
+    def forward(ctx, video, vcfg, grad, keys, *params):
         _require_cuda(video, "VitFn")
         W = {k: as_bf16(p) for k, p in zip(keys, params)}
-        need_bwd = any(ctx.needs_input_grad[3:])
+        need_bwd = grad and any(ctx.needs_input_grad[4:])
         out, c = engine.vit_fwd(W, video.to(bf16), vcfg, save=need_bwd, recompute=need_bwd and _vit_recompute(vcfg))
         if need_bwd:
             ctx.W, ctx.keys, ctx.c, ctx.params = W, keys, c, params
@@ -244,20 +246,21 @@ class VitFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout):
-        store = _GradStore(ctx.keys, ctx.params, ctx.needs_input_grad[3:], dout.device)
+        store = _GradStore(ctx.keys, ctx.params, ctx.needs_input_grad[4:], dout.device)
         engine.vit_bwd(ctx.W, store.G, ctx.c, dout.reshape(-1, dout.shape[-1]).to(bf16).contiguous())
         ctx.c = None
-        return (None, None, None) + store.grads(ctx.keys, ctx.params)
+        return (None, None, None, None) + store.grads(ctx.keys, ctx.params)
 
 
 class EvaFn(torch.autograd.Function):
-    """EVA image encoder (models/eva_vit.py VisionTransformer.forward_features): image [B,3,H,W] -> tokens [B, 1+N, D]."""
+    """EVA image encoder (models/eva_vit.py VisionTransformer.forward_features): image [B,3,H,W] -> tokens [B, 1+N, D].
+    grad: the caller's grad mode, as for VitFn."""
 
     @staticmethod
-    def forward(ctx, image, ecfg, keys, *params):
+    def forward(ctx, image, ecfg, grad, keys, *params):
         _require_cuda(image, "EvaFn")
         W = {k: as_bf16(p) for k, p in zip(keys, params)}
-        need_bwd = any(ctx.needs_input_grad[3:])
+        need_bwd = grad and any(ctx.needs_input_grad[4:])
         out, c = engine.eva_fwd(W, image.to(bf16), ecfg, save=need_bwd)
         if need_bwd:
             ctx.W, ctx.keys, ctx.c, ctx.params = W, keys, c, params
@@ -265,21 +268,22 @@ class EvaFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout):
-        store = _GradStore(ctx.keys, ctx.params, ctx.needs_input_grad[3:], dout.device)
+        store = _GradStore(ctx.keys, ctx.params, ctx.needs_input_grad[4:], dout.device)
         engine.eva_bwd(ctx.W, store.G, ctx.c, dout.reshape(-1, dout.shape[-1]).to(bf16).contiguous())
         ctx.c = None
-        return (None, None, None) + store.grads(ctx.keys, ctx.params)
+        return (None, None, None, None) + store.grads(ctx.keys, ctx.params)
 
 
 class AttnPoolFn(torch.autograd.Function):
-    """AttentionPool on learnable_queries.repeat(B): image_embeds [B,K1,D] -> [B,Q,D]."""
+    """AttentionPool on learnable_queries.repeat(B): image_embeds [B,K1,D] -> [B,Q,D].  grad: the caller's grad mode,
+    as for VitFn."""
 
     @staticmethod
-    def forward(ctx, image_embeds, heads, keys, *params):
+    def forward(ctx, image_embeds, heads, grad, keys, *params):
         _require_cuda(image_embeds, "AttnPoolFn")
         W = {k: as_bf16(p) for k, p in zip(keys, params)}
         B, K1, D = image_embeds.shape
-        need_bwd = any(ctx.needs_input_grad)
+        need_bwd = grad and any(ctx.needs_input_grad)
         out, c = engine.attn_pool_fwd(W, image_embeds.reshape(B * K1, D).to(bf16).contiguous(), B, heads, save=need_bwd)
         if need_bwd:
             ctx.W, ctx.keys, ctx.c, ctx.params, ctx.shape = W, keys, c, params, (B, K1, D)
@@ -287,10 +291,10 @@ class AttnPoolFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout):
-        store = _GradStore(ctx.keys, ctx.params, ctx.needs_input_grad[3:], dout.device)
+        store = _GradStore(ctx.keys, ctx.params, ctx.needs_input_grad[4:], dout.device)
         d_img = engine.attn_pool_bwd(ctx.W, store.G, ctx.c, dout.reshape(-1, dout.shape[-1]).to(bf16).contiguous())
         ctx.c = None
-        return (d_img.view(ctx.shape), None, None) + store.grads(ctx.keys, ctx.params)
+        return (d_img.view(ctx.shape), None, None, None) + store.grads(ctx.keys, ctx.params)
 
 
 def _pad8(n):

@@ -166,6 +166,7 @@ def _declare(name, argstruct):
 
 _gemm = _declare("ymp_gemm", GemmArgs)
 _gemm_skinny = _declare("ymp_gemm_skinny", GemmSkinnyArgs)
+_gemm_skinny_wide = _declare("ymp_gemm_skinny_wide", GemmSkinnyArgs)
 _ln_fwd = _declare("ymp_layernorm_fwd", LayerNormArgs)
 _ln_bwd = _declare("ymp_layernorm_bwd", LayerNormBwdArgs)
 _attn_fwd = _declare("ymp_attn_fwd", AttnArgs)

@@ -114,7 +114,8 @@ def gemm(a, b, *, a_t=False, b_t=False, bias=None, residual=None, act=ACT_NONE, 
     return out
 
 
-SKINNY_MAX_ROWS = 8
+SKINNY_MAX_ROWS = 8        # rows of ymp_gemm_skinny (the decode step of sample() and of one beam search)
+SKINNY_WIDE_MAX_ROWS = 64  # rows of ymp_gemm_skinny_wide (a batched beam search: clips x beams)
 
 
 def gemm_skinny(x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_dtype=bf16, out2=None, out2_row_stride=0,
@@ -125,8 +126,20 @@ def gemm_skinny(x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_d
     m * out2_row_stride + out2_off (the KV-cache row at the device-side cache length).
     ln = (gamma, beta, eps, counter): also returns LN(y) [M, N] bf16, computed inside the same kernel by the CTA that
     finishes last (counter: uint32/int32 device scalar, zero at launch, reset by the kernel); result is then (y, ln_y)."""
+    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, ln, wide=False)
+
+
+def gemm_skinny_wide(x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_dtype=bf16, out2=None, out2_row_stride=0,
+                     out2_off=None, ln=None):
+    """gemm_skinny for up to SKINNY_WIDE_MAX_ROWS = 64 rows (ymp_gemm_skinny_wide): M <= 8 runs gemm_skinny's launch,
+    9 <= M <= 64 a kernel with the same per-element arithmetic, so row m of the result is bit-identical to the same row
+    computed by gemm_skinny.  The library rejects ln with more than 8 rows and any call with more than 64."""
+    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, ln, wide=True)
+
+
+def _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, ln, wide):
     _chk2d(x, "x"); _chk2d(w, "w")
-    assert x.dtype == bf16 and w.dtype == bf16 and x.shape[1] == w.shape[1] and x.shape[0] <= SKINNY_MAX_ROWS
+    assert x.dtype == bf16 and w.dtype == bf16 and x.shape[1] == w.shape[1] and (wide or x.shape[0] <= SKINNY_MAX_ROWS)
     M, K, N = x.shape[0], x.shape[1], w.shape[0]
     if out is None:
         out = torch.empty((M, N), device=x.device, dtype=out_dtype)
@@ -155,7 +168,10 @@ def gemm_skinny(x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_d
         ln_out = torch.empty((M, N), device=x.device, dtype=bf16)
         a.ln_gamma, a.ln_beta, a.ln_out, a.ln_counter = gamma.data_ptr(), beta.data_ptr(), ln_out.data_ptr(), counter.data_ptr()
         a.ld_ln, a.ln_eps = ln_out.stride(0), eps
-    L.call(L._gemm_skinny, a, "ymp_gemm_skinny")
+    if wide:
+        L.call(L._gemm_skinny_wide, a, "ymp_gemm_skinny_wide")
+    else:
+        L.call(L._gemm_skinny, a, "ymp_gemm_skinny")
     return out if ln is None else (out, ln_out)
 
 
