@@ -316,7 +316,7 @@ def test_attn_timesformer_spatial_map(cuda):
 @pytest.mark.parametrize("S,heads,hd,n", [(8, 8, 96, 37), (4, 2, 96, 16), (2, 2, 64, 5), (16, 4, 80, 9), (12, 2, 64, 7)])
 def test_attn_temporal_packed(cuda, S, heads, hd, n):
     """Short sequences packed into 64-row tiles with a block-diagonal mask (ragged last tile)."""
-    from ymp import ops
+    from ymp import lib, ops
     torch.manual_seed(5)
     C = heads * hd
     R = n * S
@@ -324,6 +324,7 @@ def test_attn_temporal_packed(cuda, S, heads, hd, n):
     out = torch.zeros(R, C, device=cuda, dtype=bf16)
     scale = hd ** -0.5
     lse = ops.attn_temporal_fwd(qkv, out, R=R, n_heads=heads, T=S, D=hd, scale=scale)
+    assert lib.attn_last_path() == lib.ATTN_PATH_SMALL
     q5 = qkv.float().view(n, S, 3, heads, hd)
     q, k, v = (q5[:, :, i].permute(0, 2, 1, 3).contiguous().requires_grad_() for i in range(3))
     ref = _attn_ref(q, k, v, scale, False)
@@ -332,6 +333,7 @@ def test_attn_temporal_packed(cuda, S, heads, hd, n):
     ref.backward(dout.float().view(n, S, heads, hd).permute(0, 2, 1, 3))
     dqkv = torch.zeros_like(qkv)
     ops.attn_temporal_bwd(qkv, out, lse, dout, dqkv, R=R, n_heads=heads, T=S, D=hd, scale=scale)
+    assert lib.attn_last_path() == lib.ATTN_PATH_SMALL
     d5 = dqkv.float().view(n, S, 3, heads, hd)
     for i, gr in enumerate((q.grad, k.grad, v.grad)):
         assert _rel(d5[:, :, i].permute(0, 2, 1, 3), gr) < 3e-2, i
