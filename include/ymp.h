@@ -267,6 +267,14 @@ typedef struct ymp_attn_args {
   const int32_t* s_kv_dev; /* optional DEVICE scalar: only the first min(s_kv, *s_kv_dev) keys exist.  Lets a captured
                              CUDA graph of the single-token decoding step follow the growing KV cache (forward only,
                              served by the mma.sync kernels) */
+  const int32_t* kv_rows;  /* optional DEVICE row table [n_seq, kv_rows_ld]: key j of sequence s is row
+                              kv_rows[s * kv_rows_ld + j] of k / v (head offset, ldk / ldv as usual; map_kv is not
+                              used).  Lets a beam search permute its beams by gathering this table instead of the KV
+                              cache.  Every entry j < s_kv must name a valid row, also past *s_kv_dev (the first keys
+                              are requested before the device-side count is read).  Forward only, s_q == 1, no mask,
+                              dropout or total_rows: the streaming decode kernel at head_dim 64 / 80 / 96, the
+                              mma.sync tiles at 88 / 128. */
+  int64_t kv_rows_ld;      /* entries between consecutive sequences of kv_rows, >= s_kv */
 } ymp_attn_args;
 int ymp_attn_fwd(const ymp_attn_args* a, void* stream);
 

@@ -1,15 +1,18 @@
 """Time caption generation: the per-clip beam-search loop against the batched DistributedGPT3_Caption.generate.
 
-    python tools/caption_generate.py [--shapes caption_1.3B caption_2.7B] [--rounds 3] [--kernel] [--counts]
+    python tools/caption_generate.py [--shapes caption_1.3B caption_2.7B] [--rounds 3] [--kernel] [--counts] [--profile]
 
 Each shape builds DistributedGPT3_Caption with the shipped decoder json, random bf16 weights in eval mode, 128 queries
 and 16 frames, and decodes the caption eval's batch (24 clips at 1.3B, 36 at 2.7B): prompt ids [B, 20] with one
-common prompt length, beam 5, 100 tokens to generate.  Two arms, alternating in one process after a warm-up call of
+common prompt length, beam 5, 100 tokens to generate.  Three arms, alternating in one process after a warm-up call of
 each, every call ending in a device synchronise; the median of --rounds calls is reported:
-  per_clip - the composition before batching: the visual prefix, then one beam search per clip;
-  batched  - model.generate(video, text): one beam search over all clips (chunks of 64 // beam clips per decode step).
+  per_clip       - the composition before batching: the visual prefix, then one beam search per clip;
+  batched_moving - the batched call with the beams permuted by moving the cached K/V rows (KVCache.reorder);
+  batched        - model.generate(video, text): one beam search over all clips (chunks of 64 // beam clips per decode
+                   step), beams permuted through the cache's row table (KVCache.reindex).
 One JSON line per shape: card name, power limit and max SM clock, ms per call, decode steps, peak allocated memory and
-whether the two arms' sequences and scores are bit-equal.
+whether the three arms' sequences and scores are bit-equal.
+--profile prints the device-time share of each kernel family in one batched 12-clip, 40-token call of each batched arm.
 --kernel times ymp_gemm_skinny_wide alone per decoder linear and for the LM head at M in {5, 8, 16, 32, 60, 64} rows (CUDA
 events over many launches, weights rotated through copies larger than L2): microseconds and GB/s next to the H100
 SXM data sheet's 3.35 TB/s.  --counts prints the weight and KV-cache bytes counted from shapes, without a GPU.
@@ -50,7 +53,10 @@ def linears(name):
 
 def counts(name, clips=None):
     """Weight bytes one decode step streams, weight passes per eval batch of each arm (one per token step; the prefill
-    passes are not counted) and the KV-cache bytes of one batched chunk."""
+    passes are not counted), the KV-cache bytes of one batched chunk, and the bytes one beam reorder moves at the mean
+    cached length of a full-length decode: the moving KVCache.reorder (index_select into a temporary, copy back: each
+    cached [q|k|v] row read twice and written twice) against KVCache.reindex (the same four passes over the int32 row
+    table's cached columns)."""
     g = gpt_cfg(name)
     h, layers = g["hidden_size"], g["num_hidden_layers"]
     B = clips or SHAPES[name][1]
@@ -60,11 +66,16 @@ def counts(name, clips=None):
         [N * K * 2 for nm, N, K in linears(name) if nm == "lm_head"][0]
     positions = Q + L + NEW   # KV-cache positions of one sequence
     rows = min(B, per_chunk) * BEAM
+    mean_len = Q + L + NEW / 2
+    moving = 4 * layers * rows * mean_len * 3 * h * 2
+    indexed = 4 * rows * mean_len * 4
     return dict(clips=B, beam=BEAM, tokens_to_generate=NEW, weight_gb_per_step=round(step_bytes / 1e9, 3),
                 passes_per_clip_arm=B * NEW, passes_batched_arm=chunks * NEW, chunks=chunks, rows_per_chunk=rows,
                 weight_tb_per_clip_arm=round(B * NEW * step_bytes / 1e12, 2),
                 weight_tb_batched_arm=round(chunks * NEW * step_bytes / 1e12, 2),
-                kv_cache_gb_per_chunk=round(layers * rows * positions * 3 * h * 2 / 1e9, 2), kv_positions=positions)
+                kv_cache_gb_per_chunk=round(layers * rows * positions * 3 * h * 2 / 1e9, 2), kv_positions=positions,
+                reorder_mean_len=mean_len, reorder_moving_gb=round(moving / 1e9, 2), reorder_indexed_kb=round(indexed / 1e3, 1),
+                reorder_moving_min_ms_at_3_35_tb_s=round(moving / (HBM_TBS * 1e12) * 1e3, 2))
 
 
 def card_info():
@@ -109,16 +120,38 @@ def _per_clip(model, video, text):
     return res
 
 
-def run(model, vis, name, rounds):
+def moving_generate(model, video, text):
+    """The batched call with the beam loop's reorder callback moving the cached rows (KVCache.reorder: every cached
+    [q|k|v] row of every layer permuted in place) instead of gathering the row table (KVCache.reindex)."""
+    dec = model.text_decoder
+    callbacks = dec._decode_callbacks
+
+    def moving(query_embeds):
+        step, _ = callbacks(query_embeds)
+        return step, lambda idx: dec.inference_params.cache.reorder(idx)
+    dec._decode_callbacks = moving
+    try:
+        return model.generate(video, text)
+    finally:
+        del dec._decode_callbacks
+
+
+def inputs(vis, name, B):
     import torch
     import models.modeling_distributed_gpt3 as G
     dev = torch.device("cuda:0")
-    B = SHAPES[name][1]
     vocab = gpt_cfg(name)["vocab_size"]
     gen = torch.Generator().manual_seed(1)
     video = torch.randn(B, 3, FRAMES, vis["img_size"], vis["img_size"], generator=gen).to(dev).bfloat16()
     ids = torch.randint(3, vocab, (B, L), generator=gen)
     text = G.BatchEncoding(dict(input_ids=ids.to(dev), attention_mask=torch.ones(B, L, dtype=torch.long, device=dev)))
+    return video, text
+
+
+def run(model, vis, name, rounds):
+    import torch
+    B = SHAPES[name][1]
+    video, text = inputs(vis, name, B)
     dec = model.text_decoder
     orig = dec.beam_search
     found, steps = [], [0]
@@ -134,15 +167,19 @@ def run(model, vis, name, rounds):
         steps[0] += 1
         return orig_decode(*a, **k)
     dec._decode = counting_decode
-    arms = dict(per_clip=lambda: per_clip_generate(model, video, text), batched=lambda: model.generate(video, text))
+    arms = dict(per_clip=lambda: per_clip_generate(model, video, text),
+                batched_moving=lambda: moving_generate(model, video, text), batched=lambda: model.generate(video, text))
     ms = {a: [] for a in arms}
     peak = {a: 0 for a in arms}
     n_steps, outs = {}, {}
-    for r in range(rounds + 1):   # round 0 warms up both arms
+    for r in range(rounds + 1):   # round 0 warms up every arm
         for a, fn in arms.items():
             found.clear()
             outs.pop(a, None)
             steps[0] = 0
+            # the decoder pools one KV cache + captured step per shape on the model: every arm allocates (and counts in
+            # its peak) and captures its own, rather than one arm inheriting the cache of the arm before it
+            dec.__dict__.pop("_decode_pool", None)
             torch.cuda.synchronize()
             base = torch.cuda.memory_allocated()
             torch.cuda.reset_peak_memory_stats()
@@ -156,8 +193,8 @@ def run(model, vis, name, rounds):
                 ms[a].append(dt)
                 peak[a] = max(peak[a], torch.cuda.max_memory_allocated() - base)
     del dec.beam_search, dec._decode
-    equal = len(outs["per_clip"]) == len(outs["batched"]) == B and all(
-        torch.equal(s0, s1) and torch.equal(c0, c1) for (s0, c0), (s1, c1) in zip(outs["per_clip"], outs["batched"]))
+    equal = all(len(outs[a]) == B and all(torch.equal(s0, s1) and torch.equal(c0, c1)
+                                          for (s0, c0), (s1, c1) in zip(outs["per_clip"], outs[a])) for a in arms)
     res = dict(shape=name, clips=B, frames=FRAMES, queries=Q, beam=BEAM, tokens_to_generate=NEW, **card_info())
     for a in arms:
         res[f"{a}_ms"] = round(statistics.median(ms[a]), 1)
@@ -165,10 +202,50 @@ def run(model, vis, name, rounds):
         res[f"{a}_decoder_calls"] = n_steps[a]
         res[f"{a}_peak_gb"] = round(peak[a] / 1e9, 2)
     res["speedup"] = round(res["per_clip_ms"] / res["batched_ms"], 2)
+    res["speedup_over_moving"] = round(res["batched_moving_ms"] / res["batched_ms"], 2)
     res["bit_equal"] = bool(equal)
     res["counts"] = counts(name)
     print(json.dumps(res), flush=True)
     return res
+
+
+def profile(model, vis, name, clips=12, new=40):
+    """torch.profiler over one batched call of each batched arm (one 60-row chunk, `new` tokens), after a warm-up call:
+    device time per kernel family - decode / prefill attention, skinny GEMMs, and the index_select / copy kernels
+    (the moving reorder's two passes, or the indexed arm's table gather, with the step's small copies)."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile as tprofile
+    dec = model.text_decoder
+    dec.config.tokens_to_generate = new
+    video, text = inputs(vis, name, clips)
+    arms = dict(batched_moving=lambda: moving_generate(model, video, text), batched=lambda: model.generate(video, text))
+    info = card_info()
+    try:
+        for a, fn in arms.items():
+            with torch.no_grad():
+                fn()
+                torch.cuda.synchronize()
+                with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
+                    fn()
+                    torch.cuda.synchronize()
+            fam, per_kernel = {}, {}
+            for e in prof.events():
+                if e.device_type != torch.autograd.DeviceType.CUDA:
+                    continue
+                k = e.name
+                per_kernel[k] = per_kernel.get(k, 0.0) + e.time_range.elapsed_us()
+                f = ("attn_decode" if "attn_decode_kernel" in k else "attn_other" if "attn_" in k else
+                     "gemm_skinny" if "gemm_skinny" in k else
+                     "index_select_copy" if any(w in k.lower() for w in ("index", "gather", "copy")) else "other")
+                fam[f] = fam.get(f, 0.0) + e.time_range.elapsed_us()
+            total = sum(fam.values())
+            top = sorted(per_kernel.items(), key=lambda kv: -kv[1])[:6]
+            print(json.dumps(dict(shape=name, arm=a, clips=clips, tokens_to_generate=new, device_ms=round(total / 1e3, 1),
+                                  **{f"{f}_ms": round(v / 1e3, 1) for f, v in sorted(fam.items())},
+                                  **{f"{f}_share": round(v / total, 3) for f, v in sorted(fam.items())},
+                                  top_kernels_ms={k[:80]: round(v / 1e3, 1) for k, v in top}, **info)), flush=True)
+    finally:
+        dec.config.tokens_to_generate = NEW
 
 
 def kernel(name, iters=50):
@@ -207,6 +284,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--kernel", action="store_true", help="time ymp_gemm_skinny_wide per decoder linear and M")
     ap.add_argument("--counts", action="store_true", help="print the counted bytes only (no GPU)")
+    ap.add_argument("--profile", action="store_true", help="device-time shares of one batched 12-clip, 40-token call per "
+                                                           "batched arm (torch.profiler)")
     args = ap.parse_args()
     if args.counts:
         for s in args.shapes:
@@ -220,7 +299,10 @@ def main():
             kernel(s)
             continue
         model, vis = build(s, torch.device("cuda:0"))
-        run(model, vis, s, args.rounds)
+        if args.profile:
+            profile(model, vis, s)
+        else:
+            run(model, vis, s, args.rounds)
         del model
         torch.cuda.empty_cache()
 

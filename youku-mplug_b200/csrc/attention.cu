@@ -119,6 +119,8 @@ struct AttnKParams {
   int lddo, hsdo, lddq, lddk, lddv, hsdq, hsdk, hsdv;
   SeqMap mdo, mdq, mdkv;
   const int* skv_dev;  // optional device scalar: number of keys that exist (KV-cache decoding under a CUDA graph)
+  const int* kv_rows;  // optional device row table (decode kernel only): key j of sequence s is k / v row kv_rows[s * kv_rows_ld + j]
+  long kv_rows_ld;
   DropSpec drop;       // dropout of the probabilities (has_drop): row = (seq*heads + head)*s_q + query, column = key
   int has_drop;
 };
@@ -173,8 +175,10 @@ __device__ __forceinline__ void apply_mask(const AttnKParams& p, float (&sc)[8][
 }
 
 // Asynchronously load a [64 x D] bf16 tile (positions r0..r0+63 of the resolved sequence); columns DIO..D-1 are zero.
+// rows (the forward's kv_rows table of this sequence, or null): position i is row rows[i] of m.
 template <int D, int DIO>
-__device__ __forceinline__ void load_tile_async(__nv_bfloat16* dst, const RMat& m, int r0, int n_valid) {
+__device__ __forceinline__ void load_tile_async(__nv_bfloat16* dst, const RMat& m, int r0, int n_valid,
+                                                const int* rows = nullptr) {
   constexpr int CH = D / 8, LDS = D + 8;
 #pragma unroll
   for (int it = 0; it < (64 * CH + 127) / 128; ++it) {
@@ -182,7 +186,7 @@ __device__ __forceinline__ void load_tile_async(__nv_bfloat16* dst, const RMat& 
     if ((64 * CH) % 128 != 0 && idx >= 64 * CH) break;
     const int r = idx / CH, c = idx - r * CH;
     __nv_bfloat16* d = dst + r * LDS + c * 8;
-    if (r0 + r < n_valid && (DIO == D || c * 8 < DIO)) cp_async16(d, mrow(m, r0 + r) + c * 8);
+    if (r0 + r < n_valid && (DIO == D || c * 8 < DIO)) cp_async16(d, mrow(m, rows ? __ldg(rows + r0 + r) : r0 + r) + c * 8);
     else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
   }
 }
@@ -202,7 +206,9 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   int sq, skv;
   eff_len(p, s, sq, skv);
   if (q0 >= sq) return;
-  const RSeq mkv = resolve(p.mkv, s), mo = resolve(p.mo, s);
+  // kv_rows (single-query decoding at head_dim 88 / 128): key j is physical row table[j] of k / v
+  const int* table = p.kv_rows ? p.kv_rows + s * p.kv_rows_ld : nullptr;
+  const RSeq mkv = table ? RSeq{0, 1, 0, 0} : resolve(p.mkv, s), mo = resolve(p.mo, s);
   const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq);
   const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
 
@@ -216,8 +222,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   const int ntiles = (kv_end - kv_begin + 63) / 64;
 
   load_tile_async<D, DIO>(Qs, Mq, q0, sq);
-  load_tile_async<D, DIO>(KVs, Mk, kv_begin, skv);
-  load_tile_async<D, DIO>(KVs + TILE, Mv, kv_begin, skv);
+  load_tile_async<D, DIO>(KVs, Mk, kv_begin, skv, table);
+  load_tile_async<D, DIO>(KVs + TILE, Mv, kv_begin, skv, table);
   cp_async_commit();
 
   uint32_t qf[KS][4];
@@ -236,8 +242,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
     __nv_bfloat16* Vs = Ks + TILE;
     if (t + 1 < ntiles) {
       __nv_bfloat16* Kn = KVs + ((t + 1) & 1) * 2 * TILE;
-      load_tile_async<D, DIO>(Kn, Mk, kv0 + 64, skv);
-      load_tile_async<D, DIO>(Kn + TILE, Mv, kv0 + 64, skv);
+      load_tile_async<D, DIO>(Kn, Mk, kv0 + 64, skv, table);
+      load_tile_async<D, DIO>(Kn + TILE, Mv, kv0 + 64, skv, table);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -1175,6 +1181,9 @@ __global__ void __launch_bounds__(128) attn_wg_bwd_dkdv_kernel(const AttnKParams
 // running maximum, and the 128 private rows meet once at the end through shared memory.  Nothing waits on a tile:
 // one round trip to the cache per 128 keys instead of a load / mma.sync / softmax pipeline on a 64-row tile with a
 // single live row.  Algorithmic bytes: 2 * s_kv * D * 2 per (sequence, head).
+// With a row table (kv_rows) each lane first loads its key's table entry, then that row's K and V: a beam search
+// permutes its beams by gathering the small table, and the cache rows are never moved.  The per-key arithmetic and the
+// lane <-> key assignment are the same either way, so O and lse are bit-identical to a call on the gathered cache.
 template <int D>
 __global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
   constexpr int CH = D / 8;
@@ -1186,28 +1195,33 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
   const int h = blockIdx.x, s = blockIdx.y;
   griddep_launch();
   griddep_wait();
-  const RSeq mkv = resolve(p.mkv, s);
+  const int* table = p.kv_rows ? p.kv_rows + s * p.kv_rows_ld : nullptr;
+  // with a table, mrow(Mk, r) is plain physical row r of k (and of v for Mv)
+  const RSeq mkv = table ? RSeq{0, 1, 0, 0} : resolve(p.mkv, s);
   const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
   const __nv_bfloat16* qrow = p.q + rrow(resolve(p.mq, s), 0) * p.ldq + h * p.hsq;
   constexpr bool TWO_PHASE = D > 80;   // wide heads: V is requested after K has been consumed (register budget)
   uint4 qv[CH], kv[CH], vv[CH];
 #pragma unroll
   for (int c = 0; c < CH; ++c) qv[c] = __ldg(reinterpret_cast<const uint4*>(qrow) + c);
-  auto fetch_k = [&](int key) {
-    const uint4* kr = reinterpret_cast<const uint4*>(mrow(Mk, key));
+  auto row_of = [&](int key) { return table ? __ldg(table + key) : key; };
+  auto fetch_k = [&](int row) {
+    const uint4* kr = reinterpret_cast<const uint4*>(mrow(Mk, row));
 #pragma unroll
     for (int c = 0; c < CH; ++c) kv[c] = __ldg(kr + c);
   };
-  auto fetch_v = [&](int key) {
-    const uint4* vr = reinterpret_cast<const uint4*>(mrow(Mv, key));
+  auto fetch_v = [&](int row) {
+    const uint4* vr = reinterpret_cast<const uint4*>(mrow(Mv, row));
 #pragma unroll
     for (int c = 0; c < CH; ++c) vv[c] = __ldg(vr + c);
   };
   // the first 128 keys are requested before the device-side key count is known (rows < s_kv always exist in the cache
-  // buffer; what lies past the count is masked below), so the count's own load is off the critical path
+  // buffer, and every table entry < s_kv names one; what lies past the count is masked below), so the count's own load
+  // is off the critical path
   if (warp * 32 + lane < p.s_kv) {
-    fetch_k(warp * 32 + lane);
-    if (!TWO_PHASE) fetch_v(warp * 32 + lane);
+    const int row = row_of(warp * 32 + lane);
+    fetch_k(row);
+    if (!TWO_PHASE) fetch_v(row);
   }
   int sq, skv;
   eff_len(p, s, sq, skv);
@@ -1219,8 +1233,9 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
     const int key = k0 + warp * 32 + lane;
     const bool valid = key < skv;
     if (k0 > 0 && valid) {
-      fetch_k(key);
-      if (!TWO_PHASE) fetch_v(key);
+      const int row = row_of(key);
+      fetch_k(row);
+      if (!TWO_PHASE) fetch_v(row);
     }
     float sc = -CUDART_INF_F;
     if (valid) {
@@ -1233,7 +1248,7 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
       }
       sc = (a0 + a1) * p.scale_log2;
     }
-    if (TWO_PHASE && valid) fetch_v(key);
+    if (TWO_PHASE && valid) fetch_v(row_of(key));   // the table entry again (an L1 hit): no register held across the dot
     const float m_new = fmaxf(m_run, warp_max(sc));   // finite: key k0 + warp*32 is valid whenever this warp has any key
     if (m_new == -CUDART_INF_F) continue;              // (a warp past the end of a short cache)
     const float corr = exp2f(m_run - m_new), pr = valid ? exp2f(sc - m_new) : 0.f;
@@ -1331,6 +1346,7 @@ static int fill_params(const ymp_attn_args* a, AttnKParams& p, const char* who) 
   p.mask = a->mask; p.mask_block = a->mask_block > 0 ? a->mask_block : 1; p.total_rows = a->total_rows;
   p.scale = a->scale; p.scale_log2 = a->scale * 1.4426950408889634f;
   p.skv_dev = a->s_kv_dev;
+  p.kv_rows = a->kv_rows; p.kv_rows_ld = a->kv_rows_ld;
   p.has_drop = (a->drop.rng && a->drop.p > 0.f) ? 1 : 0;
   p.drop.rng = (const uint64_t*)a->drop.rng; p.drop.site = a->drop.site; p.drop.p = a->drop.p;
   return YMP_OK;
@@ -1380,6 +1396,11 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const bool dropped = p.has_drop;
   YMP_CHECK_ARG(!dropped || a->drop.p < 1.f, "ymp_attn_fwd: dropout p must be < 1");
+  if (a->kv_rows) {   // the row table is read by the decode kernel (head_dim 64 / 80 / 96) and the mma.sync tiles (88 / 128)
+    YMP_CHECK_ARG(a->s_q == 1 && a->mask == YMP_MASK_NONE && !dropped && a->total_rows == 0,
+                  "ymp_attn_fwd: kv_rows needs s_q == 1, mask none, no dropout and no total_rows");
+    YMP_CHECK_ARG(a->kv_rows_ld >= a->s_kv, "ymp_attn_fwd: kv_rows_ld must be >= s_kv");
+  }
   if (a->mask == YMP_MASK_CAUSAL && a->s_q < a->s_kv) {
     // offset causal (a block of queries at the end of a longer key range): always the wgmma tiles, whatever s_q, so
     // that every row is bit-identical to the same row of the square causal call over the whole range
@@ -1405,13 +1426,13 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   const bool dev_len = a->s_kv_dev != nullptr;  // key count read on the device: the mma.sync kernels bound their KV loop by it
   YMP_CHECK_ARG(!dev_len || (!dropped && a->mask == YMP_MASK_NONE && a->total_rows == 0 && a->head_dim != 88),
                 "ymp_attn_fwd: s_kv_dev needs mask none, no dropout, no total_rows, head_dim in {64,80,96,128}");
-  if (!dropped && !dev_len) {
+  if (!dropped && !dev_len && !a->kv_rows) {
     rc = attn_small_fwd_try(a, st);  // short dense block-diagonal sequences (attention_small.cu)
     if (rc != YMP_ENOSUP) { g_attn_path = YMP_ATTN_PATH_SMALL; return rc; }
   }
   // warpgroup-MMA tiles for head_dim <= 96; the mma.sync tiles for head_dim 128, the packed block-diagonal mask (they
-  // skip the masked chunks warp by warp), the device-side key count and a few query rows against a long cache
-  if (a->head_dim != 128 && a->mask != YMP_MASK_BLOCK && !dev_len && !(a->s_q < 16 && a->s_kv > 256)) {
+  // skip the masked chunks warp by warp), the device-side key count, a row table and a few query rows against a long cache
+  if (a->head_dim != 128 && a->mask != YMP_MASK_BLOCK && !dev_len && !a->kv_rows && !(a->s_q < 16 && a->s_kv > 256)) {
     g_attn_path = YMP_ATTN_PATH_WGMMA;
     switch (a->head_dim) {
       case 64: return launch_wg_fwd<64>(p, st);
@@ -1440,6 +1461,7 @@ extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {
   YMP_CHECK_ARG(a->o && a->lse && b->dout && b->dq && b->dk && b->dv && b->delta_ws, "ymp_attn_bwd: null o/lse/dout/dq/dk/dv/delta_ws");
   YMP_CHECK_ARG(b->lddo % 8 == 0 && b->lddq % 8 == 0 && b->lddk % 8 == 0 && b->lddv % 8 == 0, "ymp_attn_bwd: grad row strides must be multiples of 8");
   YMP_CHECK_ARG(!a->s_kv_dev, "ymp_attn_bwd: s_kv_dev is forward only");
+  YMP_CHECK_ARG(!a->kv_rows, "ymp_attn_bwd: kv_rows is forward only");
   YMP_CHECK_ARG(a->mask != YMP_MASK_CAUSAL || a->s_q == a->s_kv, "ymp_attn_bwd: causal with s_q < s_kv is forward only");
   YMP_CHECK_ARG(!p.has_drop || a->drop.p < 1.f, "ymp_attn_bwd: dropout p must be < 1");
   p.dout = (const __nv_bfloat16*)b->dout; p.dq = (__nv_bfloat16*)b->dq; p.dk = (__nv_bfloat16*)b->dk; p.dv = (__nv_bfloat16*)b->dv;

@@ -724,7 +724,9 @@ class DistributedGPT3(nn.Module):
             return out.logits[:, -1, :]
 
         def reorder(idx):
-            self.inference_params.swap_key_value_dict(idx)
+            # the beam loops own the cache: permute the row table the decoding steps read keys through, move no K/V
+            # row (swap_key_value_dict keeps the reference's physical permutation)
+            self.inference_params.cache.reindex(idx)
         return step, reorder
 
     @torch.no_grad()
@@ -783,8 +785,8 @@ class DistributedGPT3(nn.Module):
             step, reorder = self._decode_callbacks(None if query_embeds is None else query_embeds[sel])
 
             def first_beams(new_tokens, first, step=step):
-                # the prefill runs each clip's [prefix | prompt] once, into its first beam slot; the first reorder
-                # copies it to the other slots
+                # the prefill runs each clip's [prefix | prompt] once, into its first beam slot; the cache's row table
+                # points the clip's other beams at it
                 return step(new_tokens[::beam_size] if first else new_tokens, first)
             outs = run_beam_search_batched(first_beams, reorder, tokens[sel], plen, nq, beam_size=beam_size,
                                            num_return_gen=num_return_gen, stop_token=stop_token,

@@ -724,7 +724,14 @@ class KVCache:
     per-head [q|k|v] column layout of the QKV GEMM, so new rows are written by the GEMM epilogue itself
     (row re-blocking) and the attention kernels read K/V of all cached positions in place.  All layers live in
     one allocation that never moves (the captured single-token step holds its pointers), and the number of
-    cached positions is mirrored on the device (`len_idx`, `len1`) for that graph."""
+    cached positions is mirrored on the device (`len_idx`, `len1`) for that graph.
+
+    `rows` [B, max_len] int32 (also allocated once) is the row table the single-token steps read keys through: position p
+    of sequence b lives in cache row rows[b, p].  Each position's K/V row is written once, by sequence b at step p into
+    its own slot b * max_len + p, and never changes; so a beam search permutes its beams with `reindex`, which gathers
+    the table's cached columns and moves no K/V byte.  Columns >= len are never gathered and stay the identity
+    b * max_len + p, so every entry always names a valid row (the decode kernel requests keys before it reads the
+    device-side count)."""
 
     def __init__(self, gcfg, batch, max_len, device):
         g = GptDims(gcfg)
@@ -733,6 +740,9 @@ class KVCache:
         self.qkv = [self.store[i] for i in range(g.layers)]
         self.len_idx = torch.zeros(1, device=device, dtype=torch.int64)   # = len: position / cache row of the next token
         self.len1 = torch.ones(1, device=device, dtype=torch.int32)       # = len + 1: keys the next token attends to
+        self._identity = torch.arange(batch * max_len, device=device, dtype=torch.int32).view(batch, max_len)
+        self.rows = self._identity.clone()
+        self._indexed = False   # rows differs from the identity
         self.token = None   # TokenStep of the single-token steps (built by the caller that owns the weights)
 
     def reset(self):
@@ -740,16 +750,51 @@ class KVCache:
         self.len = 0
         self.len_idx.zero_()
         self.len1.fill_(1)
+        self._reset_rows()
+
+    def _reset_rows(self):
+        if self._indexed:
+            self.rows.copy_(self._identity)
+            self._indexed = False
 
     def _set_len(self, n):
         self.len = n
         self.len_idx.fill_(n)
         self.len1.fill_(n + 1)
 
+    def share_prefill(self, stride):
+        """After a prefill that wrote only slots b * stride (gpt_decode's seq_stride): every sequence of a group of
+        `stride` reads the cached positions from its group's first slot."""
+        if stride == 1 or self.len == 0:
+            return
+        self.rows[:, :self.len] = self._identity[::stride, :self.len].repeat_interleave(stride, 0)
+        self._indexed = True
+
+    def reindex(self, idx):
+        """Sequence b becomes old sequence idx[b] (beam search) by gathering the row table's cached columns: no K/V byte
+        moves.  Single-token steps read through the table; sequence b's next rows still go into its own slots."""
+        assert idx.numel() == self.B
+        if self.len == 0:
+            return
+        self.rows[:, :self.len] = self.rows[:, :self.len].index_select(0, idx)
+        self._indexed = True
+
+    def _materialize(self):
+        """Move the cached rows so that slot b * max_len + p holds position p of sequence b, and reset the table."""
+        if not self._indexed:
+            return
+        if self.len > 0:
+            v = self.store.view(self.g.layers, self.B, self.max_len, -1)
+            src = self.store.index_select(1, self.rows[:, :self.len].reshape(-1).to(torch.long))
+            v[:, :, :self.len].copy_(src.view(self.g.layers, self.B, self.len, -1))
+        self._reset_rows()
+
     def reorder(self, idx):
         """Row b of the cache becomes old row idx[b] (beam search, swap_key_value_dict :1460-1473), in place and for
-        the cached positions only: two launches for all layers."""
+        the cached positions only: two launches for all layers.  A table left by reindex / share_prefill is first
+        materialised, so the physical rows always end up as the all-moving history would have left them."""
         assert idx.numel() == self.B
+        self._materialize()
         if self.len == 0:
             return
         v = self.store.view(self.g.layers, self.B, self.max_len, -1)[:, :, :self.len]
@@ -827,7 +872,7 @@ class TokenStep:
             q = TView(st, 0, 3 * hd, ops.dense_map(1))
             k, v = TView(buf, hd, 3 * hd, mkv), TView(buf, 2 * hd, 3 * hd, mkv)
             ops.attn_fwd(q, k, v, TView(att, 0, hd, ops.dense_map(1)), n_seq=B, n_heads=g.heads, head_dim=hd, s_q=1, s_kv=ML,
-                         causal=False, scale=g.scale, s_kv_dev=c.len1)
+                         causal=False, scale=g.scale, s_kv_dev=c.len1, kv_rows=c.rows)
             x1, ln2 = gemm_ln(att, pre + "self_attention.dense", x, pre + "post_attention_layernorm")
             h = skinny(ln2, W[pre + "mlp.dense_h_to_4h.weight"], bias=W[pre + "mlp.dense_h_to_4h.bias"], act=ACT_GELU_TANH)
             nxt = f"{GPT}encoder.layers.{i + 1}.input_layernorm" if i + 1 < g.layers else GPT + "encoder.final_layernorm"
@@ -872,8 +917,8 @@ def gpt_decode(W, x, cache, n, seq_stride=1):
     (cache empty: causal attention inside the block) or single-token steps (n == 1: the query sees every
     cached key).  Returns the final-LayerNorm hidden state of the LAST new position of every sequence [B, H].
     seq_stride > 1 (first call only): x holds B = cache.B / seq_stride sequences and sequence b goes into cache slot
-    b * seq_stride (a batched beam search fills each clip's first beam slot and copies it to the others with
-    KVCache.reorder)."""
+    b * seq_stride (a batched beam search fills each clip's first beam slot); the row table then points the other
+    slots of the group at it, so no cached row is copied.  The single-token steps read keys through the row table."""
     g, ML, off = cache.g, cache.max_len, cache.len
     H, hd = g.H, g.hd
     assert cache.B % seq_stride == 0 and (seq_stride == 1 or off == 0)
@@ -897,7 +942,7 @@ def gpt_decode(W, x, cache, n, seq_stride=1):
         q = TView(new_rows, 0, 3 * hd, mq)
         k, v = TView(buf, hd, 3 * hd, mkv), TView(buf, 2 * hd, 3 * hd, mkv)
         ops.attn_fwd(q, k, v, TView(att, 0, hd, ops.dense_map(n)), n_seq=B, n_heads=g.heads, head_dim=hd, s_q=n, s_kv=off + n,
-                     causal=(off == 0 and n > 1), scale=g.scale)
+                     causal=(off == 0 and n > 1), scale=g.scale, kv_rows=cache.rows if n == 1 and off > 0 else None)
         x1 = ops.gemm(att, W[pre + "self_attention.dense.weight"], bias=W[pre + "self_attention.dense.bias"], residual=x,
                       out_dtype=torch.float32)
         ln2, _, _ = ops.layernorm_fwd(x1, W[pre + "post_attention_layernorm.weight"], W[pre + "post_attention_layernorm.bias"], g.eps,
@@ -906,6 +951,7 @@ def gpt_decode(W, x, cache, n, seq_stride=1):
         x = ops.gemm(h, W[pre + "mlp.dense_4h_to_h.weight"], bias=W[pre + "mlp.dense_4h_to_h.bias"], residual=x1,
                      out_dtype=torch.float32)
     cache._set_len(off + n)
+    cache.share_prefill(seq_stride)
     last = torch.arange(B, device=x.device, dtype=torch.int32) * n + (n - 1)
     hid, _, _ = ops.layernorm_fwd(x, W[GPT + "encoder.final_layernorm.weight"], W[GPT + "encoder.final_layernorm.bias"], g.eps,
                                   in_rows=last, stats=False)

@@ -255,7 +255,7 @@ class TView:
 
 
 def _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, mask_block=0, total_rows=0, drop=None,
-               s_kv_dev=None):
+               s_kv_dev=None, kv_rows=None):
     a = L.AttnArgs()
     a.q, a.k, a.v, a.o, a.lse = q.p, k.p, v.p, o.p, L.ptr(lse)
     a.ldq, a.ldk, a.ldv, a.ldo = q.ld, k.ld, v.ld, o.ld
@@ -268,16 +268,22 @@ def _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, sca
     if s_kv_dev is not None:
         assert s_kv_dev.dtype == torch.int32 and s_kv_dev.is_cuda and s_kv_dev.numel() == 1
         a.s_kv_dev = s_kv_dev.data_ptr()
+    if kv_rows is not None:
+        assert kv_rows.dtype == torch.int32 and kv_rows.is_cuda and kv_rows.dim() == 2 and kv_rows.stride(1) == 1
+        assert kv_rows.shape[0] == n_seq and kv_rows.shape[1] >= s_kv, (tuple(kv_rows.shape), n_seq, s_kv)
+        a.kv_rows, a.kv_rows_ld = kv_rows.data_ptr(), kv_rows.stride(0)
     return a
 
 
 def attn_fwd(q, k, v, o, *, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, lse=None, mask_block=0,
-             total_rows=0, drop=None, s_kv_dev=None):
+             total_rows=0, drop=None, s_kv_dev=None, kv_rows=None):
     """q,k,v,o: TView.  Returns lse [n_seq, n_heads, s_q] fp32.  s_kv_dev: int32 device scalar, only the first
-    min(s_kv, s_kv_dev) keys exist (the captured decoding step)."""
+    min(s_kv, s_kv_dev) keys exist (the captured decoding step).  kv_rows: int32 CUDA tensor [n_seq, >= s_kv], key j of
+    sequence s is row kv_rows[s, j] of k's / v's tensor (their seqmap is not used; s_q == 1 only, the decode kernel)."""
     if lse is None:
         lse = torch.empty((n_seq, n_heads, s_q), device=q.t.device, dtype=torch.float32)
-    a = _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, mask_block, total_rows, drop, s_kv_dev)
+    a = _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, mask_block, total_rows, drop, s_kv_dev,
+                   kv_rows)
     L.call(L._attn_fwd, a, "ymp_attn_fwd")
     return lse
 
