@@ -86,20 +86,34 @@ def test_layernorm_bwd_second_output_is_dropout_backward(cuda):
     assert torch.equal(dxgd[sel] != 0, (keep & (dxg != 0))[sel])
 
 
-def _attn_ref(q, k, v, scale, causal, keep, p):
+def _attn_ref(q, k, v, scale, causal, keep, p, mask_block=0):
     s = (q @ k.transpose(-1, -2)) * scale
     if causal:
         m = torch.ones(s.shape[-2:], dtype=torch.bool, device=s.device).triu(1)
         s = s.masked_fill(m, -10000.0)
+    if mask_block:
+        blk = torch.arange(s.shape[-1], device=s.device) // mask_block
+        s = s.masked_fill(blk[:, None] != blk[None, :], -10000.0)
     pr = s.softmax(-1)
     return (pr * keep / (1 - p)) @ v
 
 
-@pytest.mark.parametrize("hd,heads,S,causal", [(64, 4, 256, True), (64, 2, 100, True), (80, 2, 384, True), (96, 2, 197, False),
-                                               (64, 2, 520, False)])
-def test_attention_dropout_fwd_bwd(cuda, hd, heads, S, causal):
-    """O = dropout(P) V forward and backward on the wgmma kernels (GPT3CoreAttention, :768-782), masks regenerated in
-    the backward from (seed, offset, site, row, key)."""
+def _drop_case(hd, heads, S, causal, mask_block, path):
+    return pytest.param(hd, heads, S, causal, mask_block, path,
+                        id=f"{hd}-{heads}-{S}-{causal}" + (f"-block{mask_block}" if mask_block else ""))
+
+
+@pytest.mark.parametrize("hd,heads,S,causal,mask_block,path", [
+    _drop_case(64, 4, 256, True, 0, "WGMMA"), _drop_case(64, 2, 100, True, 0, "WGMMA"),
+    _drop_case(80, 2, 384, True, 0, "WGMMA"), _drop_case(96, 2, 197, False, 0, "WGMMA"),
+    _drop_case(64, 2, 520, False, 0, "WGMMA"),
+    # the mma.sync kernels: head_dim 128, and block-diagonal masks too wide for attention_small.cu (the dK / dV kernel
+    # draws its keep bits per element at head_dim 96, by a quad exchange otherwise)
+    _drop_case(128, 2, 256, True, 0, "MMA_SYNC"), _drop_case(128, 2, 200, False, 0, "MMA_SYNC"),
+    _drop_case(64, 2, 200, False, 20, "MMA_SYNC"), _drop_case(96, 2, 200, False, 24, "MMA_SYNC")])
+def test_attention_dropout_fwd_bwd(cuda, hd, heads, S, causal, mask_block, path):
+    """O = dropout(P) V forward and backward on the wgmma and mma.sync kernels (GPT3CoreAttention, :768-782), masks
+    regenerated in the backward from (seed, offset, site, row, key)."""
     from ymp import lib, ops
     torch.manual_seed(3)
     n, p, site = 2, 0.1, 4 * 5 + 1
@@ -111,11 +125,12 @@ def test_attention_dropout_fwd_bwd(cuda, hd, heads, S, causal):
     tq, tk, tv = (ops.TView(qkv, i * hd, 3 * hd, m) for i in range(3))
     to = ops.TView(out, 0, hd, m)
     drop = ops.Drop(_rng(cuda), site, p)
-    kw = dict(n_seq=n, n_heads=heads, head_dim=hd, s_q=S, s_kv=S, causal=causal, scale=hd ** -0.5, drop=drop)
+    kw = dict(n_seq=n, n_heads=heads, head_dim=hd, s_q=S, s_kv=S, causal=ops.MASK_BLOCK if mask_block else causal,
+              mask_block=mask_block, scale=hd ** -0.5, drop=drop)
     lse = ops.attn_fwd(tq, tk, tv, to, **kw)
-    assert lib.attn_last_path() == lib.ATTN_PATH_WGMMA
+    assert lib.attn_last_path() == getattr(lib, "ATTN_PATH_" + path)
     keep = torch.from_numpy(philox.keep_mask(SEED, OFFSET, site, np.arange(n * heads * S), S, p)).to(cuda).view(n, heads, S, S).float()
-    ref = _attn_ref(q, k, v, hd ** -0.5, causal, keep, p)
+    ref = _attn_ref(q, k, v, hd ** -0.5, causal, keep, p, mask_block)
     assert _rel(out.view(n, S, heads, hd).permute(0, 2, 1, 3), ref) < 2e-2
     # lse is that of the undropped probabilities
     lse_plain = ops.attn_fwd(tq, tk, tv, ops.TView(torch.zeros_like(out), 0, hd, m), **dict(kw, drop=None))
@@ -125,6 +140,7 @@ def test_attention_dropout_fwd_bwd(cuda, hd, heads, S, causal):
     dqkv = torch.zeros_like(qkv)
     tdq, tdk, tdv = (ops.TView(dqkv, i * hd, 3 * hd, m) for i in range(3))
     ops.attn_bwd(tq, tk, tv, to, lse, ops.TView(dout, 0, hd, m), tdq, tdk, tdv, **kw)
+    assert lib.attn_last_path() == getattr(lib, "ATTN_PATH_" + path)
     d5 = dqkv.float().view(n, S, heads, 3, hd)
     dq, dk, dv = (d5[:, :, :, i].permute(0, 2, 1, 3) for i in range(3))
     assert _rel(dq, q.grad) < 3e-2 and _rel(dk, k.grad) < 3e-2 and _rel(dv, v.grad) < 3e-2

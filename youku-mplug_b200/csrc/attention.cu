@@ -4,6 +4,9 @@
 // tiling, masking and softmax: warpgroup MMA (wgmma, head_dim 64 / 80 / 88 / 96: every dense, causal and cross shape
 // of the models) and warp-level mma.sync (m16n8k16; head_dim 128, packed block-diagonal masks, the device-side key
 // count, a few query rows against a long cache).  head_dim 88 is computed zero-padded to 96 in shared memory.
+// Both families hold their accumulators in the same per-warp C-fragment layout, so every step around the MMAs is one
+// helper that both call (tile loads, key-tile range, masks, online softmax, dropout, dS, the lse / delta staging and
+// the epilogues); each kernel keeps its own MMA issue, shared-memory carving and pipelining.
 // Optional dropout of the probabilities (Philox, philox.cuh): the forward drops P after the softmax normaliser, the
 // backward regenerates the same bits.  ymp_attn_fwd / ymp_attn_bwd (bottom of the file) dispatch first to
 // attention_small.cu (block-diagonal sequences of <= 16 rows: TimeSformer temporal attention) and to the
@@ -77,31 +80,8 @@ __device__ __forceinline__ const __nv_bfloat16* mrow(const RMat& m, int i) {
   return i < m.n_prefix ? m.prefix + (long)i * m.ld : m.base + (long)(i - m.n_prefix) * m.stride;
 }
 
-__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-      "{%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-
 constexpr int MASK_NONE = 0, MASK_CAUSAL = 1, MASK_BLOCK = 2;
+constexpr float LOG2E = 1.4426950408889634f;  // natural log -> the log2 units of the exp2f softmax
 
 struct AttnKParams {
   const __nv_bfloat16 *q, *k, *v;
@@ -132,6 +112,7 @@ __device__ __forceinline__ void drop2(const DropState& ds, uint32_t row, uint32_
   a = w0 >= ds.thresh ? a * ds.scale : 0.f;
   b = w1 >= ds.thresh ? b * ds.scale : 0.f;
 }
+// keep-or-drop of the single key column col of `row`: a * scale or zero
 __device__ __forceinline__ float drop1(const DropState& ds, uint32_t row, uint32_t col, float a) {
   const uint4 w = drop_words(ds, row, col >> 2);
   const uint32_t c = col & 3, wc = c == 0 ? w.x : c == 1 ? w.y : c == 2 ? w.z : w.w;
@@ -173,20 +154,288 @@ __device__ __forceinline__ void apply_mask(const AttnKParams& p, float (&sc)[8][
     }
   }
 }
+// The same rule on a transposed C-fragment tile (rows: keys k_lo + g (+8), cols: queries qi0 + nb*8 + t4*2 (+1)), fill
+// -inf.  BLOCK: the caller is served block-diagonal masks (the mma.sync kernels; the wgmma ones never are).
+template <bool BLOCK>
+__device__ __forceinline__ void apply_mask_t(const AttnKParams& p, float (&st)[8][4], int k_lo, int qi0, int skv, int g,
+                                             int t4) {
+  bool need = k_lo + 16 > skv;
+  if (p.mask == MASK_CAUSAL) need |= k_lo + 15 > qi0;
+  if (BLOCK && p.mask == MASK_BLOCK) need = true;
+  if (!need) return;
+  const int k0 = k_lo + g, k1 = k0 + 8;
+  int kb0 = 0, kb1 = 0;
+  if (BLOCK && p.mask == MASK_BLOCK) { kb0 = k0 / p.mask_block; kb1 = k1 / p.mask_block; }
+#pragma unroll
+  for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int qc = qi0 + nb * 8 + t4 * 2 + e;
+      bool m0 = k0 >= skv, m1 = k1 >= skv;
+      if (p.mask == MASK_CAUSAL) { m0 |= k0 > qc; m1 |= k1 > qc; }
+      else if (BLOCK && p.mask == MASK_BLOCK) { const int qb = qc / p.mask_block; m0 |= qb != kb0; m1 |= qb != kb1; }
+      if (m0) st[nb][e] = -CUDART_INF_F;
+      if (m1) st[nb][2 + e] = -CUDART_INF_F;
+    }
+  }
+}
 
-// Asynchronously load a [64 x D] bf16 tile (positions r0..r0+63 of the resolved sequence); columns DIO..D-1 are zero.
-// rows (the forward's kv_rows table of this sequence, or null): position i is row rows[i] of m.
+// Key tiles [kv_begin, kv_begin + 64 * ntiles) of the query tile whose rows sit at key positions a_lo .. a_lo + 63
+// (sq: the rows that exist, for the block mask); returns ntiles.  BLOCK as for apply_mask_t.
+template <bool BLOCK>
+__device__ __forceinline__ int key_tiles(const AttnKParams& p, int a_lo, int sq, int skv, int& kv_begin) {
+  int kv_end = skv;
+  kv_begin = 0;
+  if (p.mask == MASK_CAUSAL) kv_end = min(skv, a_lo + 64);
+  if (BLOCK && p.mask == MASK_BLOCK) {  // only key blocks that intersect this tile's query blocks
+    kv_begin = (a_lo / p.mask_block) * p.mask_block / 64 * 64;
+    kv_end = min(skv, ((min(a_lo + 64, sq) - 1) / p.mask_block + 1) * p.mask_block);
+  }
+  return (kv_end - kv_begin + 63) / 64;
+}
+// Key columns of tile kv0 that the mma.sync warp of query rows r_lo .. r_lo + 15 needs (warp-uniform): the 16-column
+// groups from nb_lo (block mask: only its own diagonal blocks) below column nv
+__device__ __forceinline__ void warp_key_span(const AttnKParams& p, int r_lo, int kv0, int skv, int& nv, int& nb_lo) {
+  nv = min(64, skv - kv0);
+  nb_lo = 0;
+  if (p.mask == MASK_CAUSAL) nv = min(nv, r_lo + 16 - kv0);
+  if (p.mask == MASK_BLOCK) {
+    const int c_lo = (r_lo / p.mask_block) * p.mask_block, c_hi = ((r_lo + 15) / p.mask_block + 1) * p.mask_block;
+    nb_lo = max(0, (c_lo - kv0) / 16);
+    nv = min(nv, c_hi - kv0);
+  }
+}
+
+// Online softmax over one 16 x 64 tile of raw scores (the softmax scale is folded into one FFMA per element): sc becomes
+// the unnormalised probabilities, the running row maxima m_i and this thread's partial row sums l_i advance, and the
+// output accumulator is rescaled to the new maxima.
+template <int ND>
+__device__ __forceinline__ void softmax_step(const AttnKParams& p, float (&sc)[8][4], float (&m_i)[2], float (&l_i)[2],
+                                             float (&o_acc)[ND][4]) {
+  float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
+#pragma unroll
+  for (int nb = 0; nb < 8; ++nb) {
+    mx[0] = fmaxf(mx[0], fmaxf(sc[nb][0], sc[nb][1]));
+    mx[1] = fmaxf(mx[1], fmaxf(sc[nb][2], sc[nb][3]));
+  }
+  float alpha[2], ms[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+    const float mnew = fmaxf(m_i[r], mx[r]);
+    ms[r] = (mnew == -CUDART_INF_F) ? 0.f : mnew * p.scale_log2;
+    alpha[r] = exp2f(m_i[r] * p.scale_log2 - ms[r]);
+    m_i[r] = mnew;
+    l_i[r] *= alpha[r];
+  }
+#pragma unroll
+  for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float pv = exp2f(fmaf(sc[nb][e], p.scale_log2, -ms[e >> 1]));
+      sc[nb][e] = pv;
+      l_i[e >> 1] += pv;
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < ND; ++i) {
+    o_acc[i][0] *= alpha[0]; o_acc[i][1] *= alpha[0];
+    o_acc[i][2] *= alpha[1]; o_acc[i][3] *= alpha[1];
+  }
+}
+// Dropout of a 16 x 64 tile of P (forward) or dP (dQ kernel) in place: rows drow0 (+8), key columns kv0 + nb*8 + t4*2
+// (+1); the same keep bits and scale in both
+__device__ __forceinline__ void drop_tile(const DropState& ds, uint32_t drow0, int kv0, int t4, float (&f)[8][4]) {
+#pragma unroll
+  for (int nb = 0; nb < 8; ++nb) {
+    const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
+    drop2(ds, drow0, col, f[nb][0], f[nb][1]);
+    drop2(ds, drow0 + 8, col, f[nb][2], f[nb][3]);
+  }
+}
+// dS = P o (dP - delta) in place of the (masked) raw scores sc, with P = exp2(S * scale_log2 - lse) (lse in log2 units)
+__device__ __forceinline__ void scores_to_ds(const AttnKParams& p, float (&sc)[8][4], const float (&dp)[8][4],
+                                             const float (&lse_r)[2], const float (&del_r)[2]) {
+#pragma unroll
+  for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float pv = exp2f(fmaf(sc[nb][e], p.scale_log2, -lse_r[e >> 1]));
+      sc[nb][e] = pv * (dp[nb][e] - del_r[e >> 1]);
+    }
+  }
+}
+// The transposed frame of the dK / dV kernels (rows: keys k_lo + g (+8), cols: queries qi0 + nb*8 + t4*2 (+1)):
+// st becomes P^T (Z^T = dropout(P)^T under dropout; dV += Z^T dO) and dpt becomes dS^T = P^T o (dZ^T - delta), where
+// dZ^T = dropout'(V dO^T).  stat: lse (log2 units; +inf for absent queries, so P = 0) [64] | delta [64] of the query
+// tile; qrow0: the dropout row of query qi0.
+// QUAD_EXCHANGE: the dropout keep bits of a block come from one Philox call per lane, shared within each quad of lanes;
+// otherwise each element makes its own call.  Same bits either way.
+template <bool QUAD_EXCHANGE>
+__device__ __forceinline__ void probs_t(const AttnKParams& p, const DropState& ds, float (&st)[8][4], float (&dpt)[8][4],
+                                        const float* stat, uint32_t qrow0, int k_lo, int lane) {
+  const int g = lane >> 2, t4 = lane & 3;
+#pragma unroll
+  for (int nb = 0; nb < 8; ++nb) {
+    // dropout keep bits of the four (query, key) pairs this thread holds, bit e for element e: queries q, q + 1 and keys
+    // k0, k1 = k0 + 8.  The four lanes g = 4a .. 4a+3 (same t4) need the same four Philox calls (rows q / q + 1, key
+    // groups of k0 / k1), each a different word of them: lane j = g & 3 makes call j and the words are exchanged.
+    uint32_t keep = 0xFu;
+    if (QUAD_EXCHANGE && p.has_drop) {
+      const int j = g & 3;
+      const uint32_t qr = qrow0 + (uint32_t)(nb * 8 + t4 * 2 + (j & 1));
+      const uint4 w = drop_words(ds, qr, (uint32_t)(k_lo + (g & ~3) + (j >> 1) * 8) >> 2);
+      keep = 0;
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int comp = (j + r) & 3, c = (j - r) & 3;  // send word comp, receive call c's word j
+        const uint32_t v = comp == 0 ? w.x : comp == 1 ? w.y : comp == 2 ? w.z : w.w;
+        const uint32_t got = __shfl_sync(0xffffffffu, v, (lane & ~0xC) | (c << 2));
+        keep |= (got >= ds.thresh ? 1u : 0u) << c;
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int ql = nb * 8 + t4 * 2 + (e & 1);
+      const float pv = exp2f(fmaf(st[nb][e], p.scale_log2, -stat[ql]));
+      float dz = dpt[nb][e];
+      if (p.has_drop) {
+        float kf;
+        if constexpr (QUAD_EXCHANGE) {
+          kf = (keep >> e) & 1u ? ds.scale : 0.f;
+        } else {
+          const uint32_t qrow = qrow0 + (uint32_t)ql, key = (uint32_t)(k_lo + g + (e >> 1) * 8);
+          kf = drop1(ds, qrow, key, 1.f);
+        }
+        dz *= kf;
+        st[nb][e] = pv * kf;
+      } else {
+        st[nb][e] = pv;
+      }
+      dpt[nb][e] = pv * (dz - stat[64 + ql]);
+    }
+  }
+}
+
+// dQ kernels, before the key loop: delta = rowsum(dO o O) of this warp's 16 query rows q_lo .. q_lo + 15 into p.delta
+// (for the dK / dV kernel, which runs after this one) and stat[64 + r], their lse in log2 units into stat[r].  Straight
+// from global (O is not needed anywhere else): lane -> (row = lane/2, every other 8-column chunk of the head dim =
+// lane%2), all 16-byte loads independent.
+template <int DIO>
+__device__ __forceinline__ void stage_dq_stats(const AttnKParams& p, int s, int h, int q_lo, int sq, const RSeq& mo,
+                                               const RSeq& mdo, float* stat) {
+  const int lane = threadIdx.x & 31, r = lane >> 1, hf = lane & 1;
+  const int qi = q_lo + r;
+  float acc = 0.f;
+  if (qi < sq) {
+    const uint4* orow = reinterpret_cast<const uint4*>(p.o + rrow(mo, qi) * p.ldo + h * p.hso);
+    const uint4* drow = reinterpret_cast<const uint4*>(p.dout + rrow(mdo, qi) * p.lddo + h * p.hsdo);
+#pragma unroll
+    for (int c = hf; c < DIO / 8; c += 2) {
+      const uint4 a = __ldg(orow + c), b = __ldg(drow + c);
+      acc += bf16_lo(a.x) * bf16_lo(b.x) + bf16_hi(a.x) * bf16_hi(b.x) + bf16_lo(a.y) * bf16_lo(b.y) +
+             bf16_hi(a.y) * bf16_hi(b.y) + bf16_lo(a.z) * bf16_lo(b.z) + bf16_hi(a.z) * bf16_hi(b.z) +
+             bf16_lo(a.w) * bf16_lo(b.w) + bf16_hi(a.w) * bf16_hi(b.w);
+    }
+  }
+  acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+  if (hf == 0) {
+    const size_t li = ((size_t)s * p.n_heads + h) * p.s_q + qi;
+    stat[64 + r] = acc;
+    stat[r] = (qi < sq) ? p.lse[li] * LOG2E : CUDART_INF_F;
+    if (qi < sq) p.delta[li] = acc;
+  }
+}
+// dK / dV kernels, with each Q / dO stage: lse (log2 units; +inf for absent queries) and delta of query rows
+// qi0 .. qi0 + 63 into stat[0..63] / stat[64..127].  stat_base: the lse / delta index of query 0 of this (seq, head).
+__device__ __forceinline__ void stage_dkdv_stats(const AttnKParams& p, size_t stat_base, int qi0, int sq, float* stat) {
+  if (threadIdx.x < 64) {
+    const int qi = qi0 + threadIdx.x;
+    stat[threadIdx.x] = (qi < sq) ? p.lse[stat_base + qi] * LOG2E : CUDART_INF_F;
+    stat[64 + threadIdx.x] = (qi < sq) ? p.delta[stat_base + qi] : 0.f;
+  }
+}
+
+// Epilogues of a warp's 16 rows (row_lo + g, + 8) from their C fragments; columns DIO..D-1 are never stored.
+// Forward: O = o_acc / l (after the quad sums this thread's partial l_i) and lse = m * scale + log(l).
 template <int D, int DIO>
-__device__ __forceinline__ void load_tile_async(__nv_bfloat16* dst, const RMat& m, int r0, int n_valid,
-                                                const int* rows = nullptr) {
-  constexpr int CH = D / 8, LDS = D + 8;
+__device__ __forceinline__ void store_o_lse(const AttnKParams& p, const float (&o_acc)[D / 8][4], const float (&m_i)[2],
+                                            float (&l_i)[2], int row_lo, int sq, int s, int h, const RSeq& mo, int g,
+                                            int t4) {
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_i[r] += __shfl_xor_sync(0xffffffffu, l_i[r], 1);
+    l_i[r] += __shfl_xor_sync(0xffffffffu, l_i[r], 2);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int qi = row_lo + g + r * 8;
+    if ((unsigned)qi >= (unsigned)sq) continue;  // (unsigned: the padding rows before query 0 of an offset-causal tile)
+    const float inv = l_i[r] > 0.f ? 1.f / l_i[r] : 0.f;
+    __nv_bfloat16* orow = p.o + rrow(mo, qi) * p.ldo + h * p.hso;
+#pragma unroll
+    for (int nb = 0; nb < DIO / 8; ++nb)
+      *reinterpret_cast<uint32_t*>(orow + nb * 8 + t4 * 2) = pack_bf16(o_acc[nb][2 * r] * inv, o_acc[nb][2 * r + 1] * inv);
+    if (p.lse && t4 == 0) p.lse[((size_t)s * p.n_heads + h) * p.s_q + qi] = m_i[r] * p.scale + logf(l_i[r]);
+  }
+}
+// dQ = scale * dq_acc
+template <int D, int DIO>
+__device__ __forceinline__ void store_dq(const AttnKParams& p, const float (&dq_acc)[D / 8][4], int row_lo, int sq, int h,
+                                         const RSeq& mdq, int g, int t4) {
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int qi = row_lo + g + r * 8;
+    if (qi >= sq) continue;
+    __nv_bfloat16* dqrow = p.dq + rrow(mdq, qi) * p.lddq + h * p.hsdq;
+#pragma unroll
+    for (int nb = 0; nb < DIO / 8; ++nb)
+      *reinterpret_cast<uint32_t*>(dqrow + nb * 8 + t4 * 2) = pack_bf16(dq_acc[nb][2 * r] * p.scale, dq_acc[nb][2 * r + 1] * p.scale);
+  }
+}
+// dK = scale * dk_acc, dV = dv_acc (rows are keys)
+template <int D, int DIO>
+__device__ __forceinline__ void store_dkdv(const AttnKParams& p, const float (&dk_acc)[D / 8][4],
+                                           const float (&dv_acc)[D / 8][4], int row_lo, int skv, int h, const RSeq& mdkv,
+                                           int g, int t4) {
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int kvr = row_lo + g + r * 8;
+    if (kvr >= skv) continue;
+    const long row = rrow(mdkv, kvr);
+    __nv_bfloat16* dkrow = p.dk + row * p.lddk + h * p.hsdk;
+    __nv_bfloat16* dvrow = p.dv + row * p.lddv + h * p.hsdv;
+#pragma unroll
+    for (int nb = 0; nb < DIO / 8; ++nb) {
+      *reinterpret_cast<uint32_t*>(dkrow + nb * 8 + t4 * 2) = pack_bf16(dk_acc[nb][2 * r] * p.scale, dk_acc[nb][2 * r + 1] * p.scale);
+      *reinterpret_cast<uint32_t*>(dvrow + nb * 8 + t4 * 2) = pack_bf16(dv_acc[nb][2 * r], dv_acc[nb][2 * r + 1]);
+    }
+  }
+}
+
+// Shared-memory layout of a [64 x D] bf16 operand tile
+enum TileLayout {
+  PADDED,       // mma.sync: rows of D + 8 elements (the ldmatrix rows of a 16-byte column fall in different banks)
+  SWIZZLE_128B  // wgmma: the K-major layout that TMA writes, 64-column panels of 64 rows x 128 bytes, 16-byte chunk c
+                // of row r at chunk c ^ (r & 7)
+};
+// Asynchronously load a [64 x D] bf16 tile: positions r0..r0+63 of the resolved sequence, zero outside [0, n_valid)
+// and in columns DIO..D-1.  rows (the forward's kv_rows table of this sequence, or null): position i is row rows[i] of m.
+template <TileLayout L, int D, int DIO>
+__device__ __forceinline__ void load_tile(void* dst, const RMat& m, int r0, int n_valid, const int* rows = nullptr) {
+  constexpr int CH = D / 8;
 #pragma unroll
   for (int it = 0; it < (64 * CH + 127) / 128; ++it) {
     const int idx = threadIdx.x + it * 128;
     if ((64 * CH) % 128 != 0 && idx >= 64 * CH) break;
     const int r = idx / CH, c = idx - r * CH;
-    __nv_bfloat16* d = dst + r * LDS + c * 8;
-    if (r0 + r < n_valid && (DIO == D || c * 8 < DIO)) cp_async16(d, mrow(m, rows ? __ldg(rows + r0 + r) : r0 + r) + c * 8);
+    // (pointer steps as written: one summed byte offset costs the mma.sync backward kernels registers and spills)
+    uint8_t* d = L == PADDED ? reinterpret_cast<uint8_t*>(static_cast<__nv_bfloat16*>(dst) + r * (D + 8) + c * 8)
+                             : static_cast<uint8_t*>(dst) + (c >> 3) * 8192 + r * 128 + (((c & 7) ^ (r & 7)) << 4);
+    // (unsigned: a query tile of an offset-causal call may start before the first query row)
+    if ((unsigned)(r0 + r) < (unsigned)n_valid && (DIO == D || c * 8 < DIO))
+      cp_async16(d, mrow(m, rows ? __ldg(rows + r0 + r) : r0 + r) + c * 8);
     else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
   }
 }
@@ -211,19 +460,12 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   const RSeq mkv = table ? RSeq{0, 1, 0, 0} : resolve(p.mkv, s), mo = resolve(p.mo, s);
   const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq);
   const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
+  int kv_begin;
+  const int ntiles = key_tiles<true>(p, q0, sq, skv, kv_begin);
 
-  int kv_end = skv;
-  if (p.mask == MASK_CAUSAL) kv_end = min(skv, q0 + 64);
-  int kv_begin = 0;
-  if (p.mask == MASK_BLOCK) {  // only key blocks that intersect this tile's query blocks
-    kv_begin = (q0 / p.mask_block) * p.mask_block / 64 * 64;
-    kv_end = min(skv, ((min(q0 + 64, sq) - 1) / p.mask_block + 1) * p.mask_block);
-  }
-  const int ntiles = (kv_end - kv_begin + 63) / 64;
-
-  load_tile_async<D, DIO>(Qs, Mq, q0, sq);
-  load_tile_async<D, DIO>(KVs, Mk, kv_begin, skv, table);
-  load_tile_async<D, DIO>(KVs + TILE, Mv, kv_begin, skv, table);
+  load_tile<PADDED, D, DIO>(Qs, Mq, q0, sq);
+  load_tile<PADDED, D, DIO>(KVs, Mk, kv_begin, skv, table);
+  load_tile<PADDED, D, DIO>(KVs + TILE, Mv, kv_begin, skv, table);
   cp_async_commit();
 
   uint32_t qf[KS][4];
@@ -242,8 +484,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
     __nv_bfloat16* Vs = Ks + TILE;
     if (t + 1 < ntiles) {
       __nv_bfloat16* Kn = KVs + ((t + 1) & 1) * 2 * TILE;
-      load_tile_async<D, DIO>(Kn, Mk, kv0 + 64, skv, table);
-      load_tile_async<D, DIO>(Kn + TILE, Mv, kv0 + 64, skv, table);
+      load_tile<PADDED, D, DIO>(Kn, Mk, kv0 + 64, skv, table);
+      load_tile<PADDED, D, DIO>(Kn + TILE, Mv, kv0 + 64, skv, table);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -256,16 +498,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
         ldsm_x4(qf[kk], smem_u32(Qs + (warp * 16 + (lane & 15)) * LDS + kk * 16 + (lane >> 4) * 8));
     }
     if (warp_active) {
-      // number of key columns of this tile this warp actually needs (warp-uniform)
-      int nv = min(64, skv - kv0);
-      int nb_lo = 0;  // first 16-column group this warp needs (block mask: only its own diagonal blocks)
-      if (p.mask == MASK_CAUSAL) nv = min(nv, q0 + warp * 16 + 16 - kv0);
-      if (p.mask == MASK_BLOCK) {
-        const int r_lo = q0 + warp * 16;
-        const int c_lo = (r_lo / p.mask_block) * p.mask_block, c_hi = ((r_lo + 15) / p.mask_block + 1) * p.mask_block;
-        nb_lo = max(0, (c_lo - kv0) / 16);
-        nv = min(nv, c_hi - kv0);
-      }
+      int nv, nb_lo;
+      warp_key_span(p, q0 + warp * 16, kv0, skv, nv, nb_lo);
       float sc[8][4];
 #pragma unroll
       for (int i = 0; i < 8; ++i) { sc[i][0] = sc[i][1] = sc[i][2] = sc[i][3] = 0.f; }
@@ -281,48 +515,11 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
           }
         }
       }
-      // raw scores; the softmax scale is folded into one FFMA per element below
       if (tile_needs_mask(p, q0 + warp * 16, kv0, skv))
         apply_mask(p, sc, q0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);
-      float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
-#pragma unroll
-      for (int nb = 0; nb < 8; ++nb) {
-        mx[0] = fmaxf(mx[0], fmaxf(sc[nb][0], sc[nb][1]));
-        mx[1] = fmaxf(mx[1], fmaxf(sc[nb][2], sc[nb][3]));
-      }
-      float alpha[2], ms[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        const float mnew = fmaxf(m_i[r], mx[r]);
-        ms[r] = (mnew == -CUDART_INF_F) ? 0.f : mnew * p.scale_log2;
-        alpha[r] = exp2f(m_i[r] * p.scale_log2 - ms[r]);
-        m_i[r] = mnew;
-        l_i[r] *= alpha[r];
-      }
-#pragma unroll
-      for (int nb = 0; nb < 8; ++nb) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float pv = exp2f(fmaf(sc[nb][e], p.scale_log2, -ms[e >> 1]));
-          sc[nb][e] = pv;
-          l_i[e >> 1] += pv;
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < D / 8; ++i) {
-        o_acc[i][0] *= alpha[0]; o_acc[i][1] *= alpha[0];
-        o_acc[i][2] *= alpha[1]; o_acc[i][3] *= alpha[1];
-      }
-      if (p.has_drop) {  // O = dropout(P) V; the normaliser stays that of the undropped P (softmax, then dropout)
-#pragma unroll
-        for (int nb = 0; nb < 8; ++nb) {
-          const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
-          drop2(ds, drow0, col, sc[nb][0], sc[nb][1]);
-          drop2(ds, drow0 + 8, col, sc[nb][2], sc[nb][3]);
-        }
-      }
+      softmax_step(p, sc, m_i, l_i, o_acc);
+      // O = dropout(P) V; the normaliser stays that of the undropped P (softmax, then dropout)
+      if (p.has_drop) drop_tile(ds, drow0, kv0, t4, sc);
 #pragma unroll
       for (int kk2 = 0; kk2 < 4; ++kk2) {
         if (kk2 * 16 < nv && kk2 >= nb_lo) {
@@ -344,24 +541,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
     __syncthreads();
   }
   if (!warp_active) return;
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    l_i[r] += __shfl_xor_sync(0xffffffffu, l_i[r], 1);
-    l_i[r] += __shfl_xor_sync(0xffffffffu, l_i[r], 2);
-  }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int qi = q0 + warp * 16 + g + r * 8;
-    if (qi >= sq) continue;
-    const float inv = l_i[r] > 0.f ? 1.f / l_i[r] : 0.f;
-    __nv_bfloat16* orow = p.o + rrow(mo, qi) * p.ldo + h * p.hso;
-#pragma unroll
-    for (int nb = 0; nb < DIO / 8; ++nb)
-      *reinterpret_cast<uint32_t*>(orow + nb * 8 + t4 * 2) =
-          pack_bf16(o_acc[nb][2 * r] * inv, o_acc[nb][2 * r + 1] * inv);
-    if (p.lse && t4 == 0)
-      p.lse[((size_t)s * p.n_heads + h) * p.s_q + qi] = m_i[r] * p.scale + logf(l_i[r]);
-  }
+  store_o_lse<D, DIO>(p, o_acc, m_i, l_i, q0 + warp * 16, sq, s, h, mo, g, t4);
 }
 
 // ------------------------------------------------------------------------------ backward: dQ
@@ -383,44 +563,15 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
   const RSeq mkv = resolve(p.mkv, s), mo = resolve(p.mo, s), mdo = resolve(p.mdo, s), mdq = resolve(p.mdq, s);
   const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq), Mdo = rmat(p.dout, mdo, p.lddo, h * p.hsdo);
   const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
-  int kv_end = skv, kv_begin = 0;
-  if (p.mask == MASK_CAUSAL) kv_end = min(skv, q0 + 64);
-  if (p.mask == MASK_BLOCK) {
-    kv_begin = (q0 / p.mask_block) * p.mask_block / 64 * 64;
-    kv_end = min(skv, ((min(q0 + 64, sq) - 1) / p.mask_block + 1) * p.mask_block);
-  }
-  const int ntiles = (kv_end - kv_begin + 63) / 64;
+  int kv_begin;
+  const int ntiles = key_tiles<true>(p, q0, sq, skv, kv_begin);
 
-  load_tile_async<D, DIO>(Qs, Mq, q0, sq);
-  load_tile_async<D, DIO>(dOs, Mdo, q0, sq);
-  load_tile_async<D, DIO>(KVs, Mk, kv_begin, skv);
-  load_tile_async<D, DIO>(KVs + TILE, Mv, kv_begin, skv);
+  load_tile<PADDED, D, DIO>(Qs, Mq, q0, sq);
+  load_tile<PADDED, D, DIO>(dOs, Mdo, q0, sq);
+  load_tile<PADDED, D, DIO>(KVs, Mk, kv_begin, skv);
+  load_tile<PADDED, D, DIO>(KVs + TILE, Mv, kv_begin, skv);
   cp_async_commit();
-  // delta / lse for this warp's 16 rows, straight from global (O is not needed anywhere else):
-  // lane -> (row = lane/2, every other 8-column chunk of the head dim = lane%2), all 16-byte loads independent
-  {
-    const int r = lane >> 1, hf = lane & 1;
-    const int qi = q0 + warp * 16 + r;
-    float acc = 0.f;
-    if (qi < sq) {
-      const uint4* orow = reinterpret_cast<const uint4*>(p.o + rrow(mo, qi) * p.ldo + h * p.hso);
-      const uint4* drow = reinterpret_cast<const uint4*>(p.dout + rrow(mdo, qi) * p.lddo + h * p.hsdo);
-#pragma unroll
-      for (int c = hf; c < DIO / 8; c += 2) {
-        const uint4 a = __ldg(orow + c), b = __ldg(drow + c);
-        acc += bf16_lo(a.x) * bf16_lo(b.x) + bf16_hi(a.x) * bf16_hi(b.x) + bf16_lo(a.y) * bf16_lo(b.y) +
-               bf16_hi(a.y) * bf16_hi(b.y) + bf16_lo(a.z) * bf16_lo(b.z) + bf16_hi(a.z) * bf16_hi(b.z) +
-               bf16_lo(a.w) * bf16_lo(b.w) + bf16_hi(a.w) * bf16_hi(b.w);
-      }
-    }
-    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-    if (hf == 0) {
-      const size_t li = ((size_t)s * p.n_heads + h) * p.s_q + qi;
-      stat[64 + warp * 16 + r] = acc;
-      stat[warp * 16 + r] = (qi < sq) ? p.lse[li] * 1.4426950408889634f : CUDART_INF_F;
-      if (qi < sq) p.delta[li] = acc;
-    }
-  }
+  stage_dq_stats<DIO>(p, s, h, q0 + warp * 16, sq, mo, mdo, stat + warp * 16);
 
   uint32_t qf[KS][4], dof[KS][4];
   float dq_acc[D / 8][4];
@@ -438,8 +589,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
     __nv_bfloat16* Vs = Ks + TILE;
     if (t + 1 < ntiles) {
       __nv_bfloat16* Kn = KVs + ((t + 1) & 1) * 2 * TILE;
-      load_tile_async<D, DIO>(Kn, Mk, kv0 + 64, skv);
-      load_tile_async<D, DIO>(Kn + TILE, Mv, kv0 + 64, skv);
+      load_tile<PADDED, D, DIO>(Kn, Mk, kv0 + 64, skv);
+      load_tile<PADDED, D, DIO>(Kn + TILE, Mv, kv0 + 64, skv);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -457,15 +608,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
       del_r[0] = stat[64 + warp * 16 + g]; del_r[1] = stat[64 + warp * 16 + g + 8];
     }
     if (warp_active) {
-      int nv = min(64, skv - kv0);
-      int nb_lo = 0;  // first 16-column group this warp needs (block mask: only its own diagonal blocks)
-      if (p.mask == MASK_CAUSAL) nv = min(nv, q0 + warp * 16 + 16 - kv0);
-      if (p.mask == MASK_BLOCK) {
-        const int r_lo = q0 + warp * 16;
-        const int c_lo = (r_lo / p.mask_block) * p.mask_block, c_hi = ((r_lo + 15) / p.mask_block + 1) * p.mask_block;
-        nb_lo = max(0, (c_lo - kv0) / 16);
-        nv = min(nv, c_hi - kv0);
-      }
+      int nv, nb_lo;
+      warp_key_span(p, q0 + warp * 16, kv0, skv, nv, nb_lo);
       float sc[8][4], dp[8][4];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -490,22 +634,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
       }
       if (tile_needs_mask(p, q0 + warp * 16, kv0, skv))
         apply_mask(p, sc, q0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);  // exp2(-inf) = 0
-      if (p.has_drop) {  // dP = dropout'(dO V^T): the same keep bits and scale as the forward
-#pragma unroll
-        for (int nb = 0; nb < 8; ++nb) {
-          const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
-          drop2(ds, drow0, col, dp[nb][0], dp[nb][1]);
-          drop2(ds, drow0 + 8, col, dp[nb][2], dp[nb][3]);
-        }
-      }
-#pragma unroll
-      for (int nb = 0; nb < 8; ++nb) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float pv = exp2f(fmaf(sc[nb][e], p.scale_log2, -lse_r[e >> 1]));
-          sc[nb][e] = pv * (dp[nb][e] - del_r[e >> 1]);  // dS
-        }
-      }
+      if (p.has_drop) drop_tile(ds, drow0, kv0, t4, dp);  // dP = dropout'(dO V^T)
+      scores_to_ds(p, sc, dp, lse_r, del_r);
 #pragma unroll
       for (int kk2 = 0; kk2 < 4; ++kk2) {
         if (kk2 * 16 < nv && kk2 >= nb_lo) {
@@ -527,16 +657,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnKParams p) {
     __syncthreads();
   }
   if (!warp_active) return;
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int qi = q0 + warp * 16 + g + r * 8;
-    if (qi >= sq) continue;
-    __nv_bfloat16* dqrow = p.dq + rrow(mdq, qi) * p.lddq + h * p.hsdq;
-#pragma unroll
-    for (int nb = 0; nb < DIO / 8; ++nb)
-      *reinterpret_cast<uint32_t*>(dqrow + nb * 8 + t4 * 2) =
-          pack_bf16(dq_acc[nb][2 * r] * p.scale, dq_acc[nb][2 * r + 1] * p.scale);
-  }
+  store_dq<D, DIO>(p, dq_acc, q0 + warp * 16, sq, h, mdq, g, t4);
 }
 
 // ------------------------------------------------------------------------------ backward: dK, dV
@@ -568,18 +689,13 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
 
   auto load_stage = [&](int stage, int qi0) {
     __nv_bfloat16* Qn = QDs + stage * 2 * TILE;
-    load_tile_async<D, DIO>(Qn, Mq, qi0, sq);
-    load_tile_async<D, DIO>(Qn + TILE, Mdo, qi0, sq);
-    if (threadIdx.x < 64) {
-      const int qi = qi0 + threadIdx.x;
-      float* st = stat + stage * 128;
-      st[threadIdx.x] = (qi < sq) ? p.lse[stat_base + qi] * 1.4426950408889634f : CUDART_INF_F;
-      st[64 + threadIdx.x] = (qi < sq) ? p.delta[stat_base + qi] : 0.f;
-    }
+    load_tile<PADDED, D, DIO>(Qn, Mq, qi0, sq);
+    load_tile<PADDED, D, DIO>(Qn + TILE, Mdo, qi0, sq);
+    stage_dkdv_stats(p, stat_base, qi0, sq, stat + stage * 128);
   };
 
-  load_tile_async<D, DIO>(Ks, Mk, kv0, skv);
-  load_tile_async<D, DIO>(Vs, Mv, kv0, skv);
+  load_tile<PADDED, D, DIO>(Ks, Mk, kv0, skv);
+  load_tile<PADDED, D, DIO>(Vs, Mv, kv0, skv);
   load_stage(0, q_begin);
   cp_async_commit();
 
@@ -592,7 +708,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
   const bool warp_active = (kv0 + warp * 16) < skv;
   DropState ds;  // only read when has_drop
   if (p.has_drop) ds = drop_state(p.drop);
-  const uint32_t dbase = (uint32_t)(((long)s * p.n_heads + h) * p.s_q);
+  const uint32_t dbase = (uint32_t)stat_base;
 
   for (int t = 0; t < ntiles; ++t) {
     const int qi0 = q_begin + t * 64;
@@ -644,48 +760,10 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
           }
         }
       }
-      {
-        // transposed tile: rows are keys, columns are queries
-        const int k_lo = kv0 + warp * 16;
-        bool need = (k_lo + 16 > skv);
-        if (p.mask == MASK_CAUSAL) need |= (k_lo + 15 > qi0);
-        if (p.mask == MASK_BLOCK) need = true;
-        if (need) {
-          const int k0 = k_lo + g, k1 = k0 + 8;
-          int kb0 = 0, kb1 = 0;
-          if (p.mask == MASK_BLOCK) { kb0 = k0 / p.mask_block; kb1 = k1 / p.mask_block; }
-#pragma unroll
-          for (int nb = 0; nb < 8; ++nb) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int qc = qi0 + nb * 8 + t4 * 2 + e;
-              bool m0 = k0 >= skv, m1 = k1 >= skv;
-              if (p.mask == MASK_CAUSAL) { m0 |= k0 > qc; m1 |= k1 > qc; }
-              else if (p.mask == MASK_BLOCK) { const int qb = qc / p.mask_block; m0 |= qb != kb0; m1 |= qb != kb1; }
-              if (m0) st_[nb][e] = -CUDART_INF_F;
-              if (m1) st_[nb][2 + e] = -CUDART_INF_F;
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int nb = 0; nb < 8; ++nb) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int ql = nb * 8 + t4 * 2 + (e & 1);
-          const float pv = exp2f(fmaf(st_[nb][e], p.scale_log2, -st[ql]));  // lse=+inf for absent queries -> 0
-          float dz = dpt[nb][e];
-          if (p.has_drop) {  // Z = dropout(P): dV += Z^T dO, dP = dropout'(dZ)
-            const uint32_t qrow = dbase + (uint32_t)(qi0 + ql), key = (uint32_t)(kv0 + warp * 16 + g + (e >> 1) * 8);
-            const float keep = drop1(ds, qrow, key, 1.f);
-            dz *= keep;
-            st_[nb][e] = pv * keep;                    // Z^T
-          } else {
-            st_[nb][e] = pv;                           // P^T
-          }
-          dpt[nb][e] = pv * (dz - st[64 + ql]);        // dS^T
-        }
-      }
+      apply_mask_t<true>(p, st_, kv0 + warp * 16, qi0, skv, g, t4);
+      // This kernel runs at the 255-register limit.  With nvcc 12.9 the quad exchange spills least at head_dim 64 / 80 /
+      // 128 and the per-element calls at 88 / 96 (none there; 52 bytes with the exchange).
+      probs_t<D != 96>(p, ds, st_, dpt, st, dbase + (uint32_t)qi0, kv0 + warp * 16, lane);
 #pragma unroll
       for (int kk2 = 0; kk2 < 4; ++kk2) {
         if (kk2 * 16 < nv && kk2 >= nb_lo) {
@@ -715,20 +793,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
     __syncthreads();
   }
   if (!warp_active) return;
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int kvr = kv0 + warp * 16 + g + r * 8;
-    if (kvr >= skv) continue;
-    const long row = rrow(mdkv, kvr);
-    __nv_bfloat16* dkrow = p.dk + row * p.lddk + h * p.hsdk;
-    __nv_bfloat16* dvrow = p.dv + row * p.lddv + h * p.hsdv;
-#pragma unroll
-    for (int nb = 0; nb < DIO / 8; ++nb) {
-      *reinterpret_cast<uint32_t*>(dkrow + nb * 8 + t4 * 2) =
-          pack_bf16(dk_acc[nb][2 * r] * p.scale, dk_acc[nb][2 * r + 1] * p.scale);
-      *reinterpret_cast<uint32_t*>(dvrow + nb * 8 + t4 * 2) = pack_bf16(dv_acc[nb][2 * r], dv_acc[nb][2 * r + 1]);
-    }
-  }
+  store_dkdv<D, DIO>(p, dk_acc, dv_acc, kv0 + warp * 16, skv, h, mdkv, g, t4);
 }
 
 // ------------------------------------------------------------------------------ wgmma kernels (head_dim 64 / 80 / 96)
@@ -736,27 +801,12 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const AttnKParams p)
 // four warps issue warpgroup MMAs together: S / dP tiles are wgmma m64n64k16 with both operands in shared memory, and
 // the P.V / dS.K / P^T.dO / dS^T.Q products are wgmma m64nDk16 with the probabilities as the register A operand (the
 // m64 accumulator of a warp is exactly the A fragment of the next product) and the shared tile read MN-major.
-// Operand tiles are 64 rows x D bf16 in the SWIZZLE_128B K-major layout that TMA writes (64-column panels of
-// 64 rows x 128 bytes, 16-byte chunk c of row r at chunk c ^ (r & 7)), filled by cp.async through the seqmaps.
+// Operand tiles are 64 rows x D bf16 in the SWIZZLE_128B layout, filled by cp.async through the seqmaps.
 // head_dim 88 is computed as 96 with zero-filled tail columns that are never stored.
 template <int D>
 struct WgTile {
   static constexpr int BYTES = ((D + 63) / 64) * 8192;
 };
-template <int D, int DIO>
-__device__ __forceinline__ void wg_load_tile(uint8_t* dst, const RMat& m, int r0, int n_valid) {
-  constexpr int CH = D / 8;
-#pragma unroll
-  for (int it = 0; it < (64 * CH + 127) / 128; ++it) {
-    const int idx = threadIdx.x + it * 128;
-    if ((64 * CH) % 128 != 0 && idx >= 64 * CH) break;
-    const int r = idx / CH, c = idx - r * CH;
-    uint8_t* d = dst + (c >> 3) * 8192 + r * 128 + (((c & 7) ^ (r & 7)) << 4);
-    // (unsigned: a query tile of an offset-causal call may start before the first query row)
-    if ((unsigned)(r0 + r) < (unsigned)n_valid && (DIO == D || c * 8 < DIO)) cp_async16(d, mrow(m, r0 + r) + c * 8);
-    else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
-  }
-}
 // k-step ks (16 head-dim columns) of a tile whose rows are the M / N dimension
 __device__ __forceinline__ uint64_t wg_desc_k(uint32_t base, int ks) {
   return make_smem_desc(base + (ks >> 2) * 8192 + (ks & 3) * 32, 16, 1024, 1);
@@ -829,13 +879,12 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   const RSeq mkv = resolve(p.mkv, s), mo = resolve(p.mo, s);
   const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq);
   const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
-  int kv_end = skv;
-  if (p.mask == MASK_CAUSAL) kv_end = min(skv, a0 + 64);
-  const int ntiles = (kv_end + 63) / 64;
+  int kv_begin;
+  const int ntiles = key_tiles<false>(p, a0, sq, skv, kv_begin);
 
-  wg_load_tile<D, DIO>(Qs, Mq, q0, sq);
-  wg_load_tile<D, DIO>(KVs, Mk, 0, skv);
-  wg_load_tile<D, DIO>(KVs + TB, Mv, 0, skv);
+  load_tile<SWIZZLE_128B, D, DIO>(Qs, Mq, q0, sq);
+  load_tile<SWIZZLE_128B, D, DIO>(KVs, Mk, kv_begin, skv);
+  load_tile<SWIZZLE_128B, D, DIO>(KVs + TB, Mv, kv_begin, skv);
   cp_async_commit();
 
   float o_acc[D / 8][4];
@@ -847,13 +896,13 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   const uint32_t drow0 = (uint32_t)(((long)s * p.n_heads + h) * p.s_q + q0 + warp * 16 + g);
 
   for (int t = 0; t < ntiles; ++t) {
-    const int kv0 = t * 64;
+    const int kv0 = kv_begin + t * 64;
     uint8_t* Ks = KVs + (t & 1) * 2 * TB;
     uint8_t* Vs = Ks + TB;
     if (t + 1 < ntiles) {
       uint8_t* Kn = KVs + ((t + 1) & 1) * 2 * TB;
-      wg_load_tile<D, DIO>(Kn, Mk, kv0 + 64, skv);
-      wg_load_tile<D, DIO>(Kn + TB, Mv, kv0 + 64, skv);
+      load_tile<SWIZZLE_128B, D, DIO>(Kn, Mk, kv0 + 64, skv);
+      load_tile<SWIZZLE_128B, D, DIO>(Kn + TB, Mv, kv0 + 64, skv);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -864,64 +913,13 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
     float sc[8][4];
     wg_scores<D>(sc, smem_u32(Qs), smem_u32(Ks));
     if (tile_needs_mask(p, a0 + warp * 16, kv0, skv)) apply_mask(p, sc, a0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);
-    float mx[2] = {-CUDART_INF_F, -CUDART_INF_F};
-#pragma unroll
-    for (int nb = 0; nb < 8; ++nb) {
-      mx[0] = fmaxf(mx[0], fmaxf(sc[nb][0], sc[nb][1]));
-      mx[1] = fmaxf(mx[1], fmaxf(sc[nb][2], sc[nb][3]));
-    }
-    float alpha[2], ms[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float mnew = fmaxf(m_i[r], mx[r]);
-      ms[r] = (mnew == -CUDART_INF_F) ? 0.f : mnew * p.scale_log2;
-      alpha[r] = exp2f(m_i[r] * p.scale_log2 - ms[r]);
-      m_i[r] = mnew;
-      l_i[r] *= alpha[r];
-    }
-#pragma unroll
-    for (int nb = 0; nb < 8; ++nb) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float pv = exp2f(fmaf(sc[nb][e], p.scale_log2, -ms[e >> 1]));
-        sc[nb][e] = pv;
-        l_i[e >> 1] += pv;
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < D / 8; ++i) {
-      o_acc[i][0] *= alpha[0]; o_acc[i][1] *= alpha[0];
-      o_acc[i][2] *= alpha[1]; o_acc[i][3] *= alpha[1];
-    }
-    if (p.has_drop) {  // O = dropout(P) V; the normaliser stays that of the undropped P (softmax, then dropout)
-#pragma unroll
-      for (int nb = 0; nb < 8; ++nb) {
-        const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
-        drop2(ds, drow0, col, sc[nb][0], sc[nb][1]);
-        drop2(ds, drow0 + 8, col, sc[nb][2], sc[nb][3]);
-      }
-    }
+    softmax_step(p, sc, m_i, l_i, o_acc);
+    // O = dropout(P) V; the normaliser stays that of the undropped P (softmax, then dropout)
+    if (p.has_drop) drop_tile(ds, drow0, kv0, t4, sc);
     wg_pv<D>(o_acc, sc, smem_u32(Vs));
     __syncthreads();  // every warpgroup MMA of this stage has retired before it is refilled
   }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    l_i[r] += __shfl_xor_sync(0xffffffffu, l_i[r], 1);
-    l_i[r] += __shfl_xor_sync(0xffffffffu, l_i[r], 2);
-  }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int qi = q0 + warp * 16 + g + r * 8;
-    if (qi < 0 || qi >= sq) continue;
-    const float inv = l_i[r] > 0.f ? 1.f / l_i[r] : 0.f;
-    __nv_bfloat16* orow = p.o + rrow(mo, qi) * p.ldo + h * p.hso;
-#pragma unroll
-    for (int nb = 0; nb < DIO / 8; ++nb)
-      *reinterpret_cast<uint32_t*>(orow + nb * 8 + t4 * 2) = pack_bf16(o_acc[nb][2 * r] * inv, o_acc[nb][2 * r + 1] * inv);
-    if (p.lse && t4 == 0) p.lse[((size_t)s * p.n_heads + h) * p.s_q + qi] = m_i[r] * p.scale + logf(l_i[r]);
-  }
+  store_o_lse<D, DIO>(p, o_acc, m_i, l_i, q0 + warp * 16, sq, s, h, mo, g, t4);
 }
 
 // dQ (and delta = rowsum(dO * O) for the dK / dV kernel, which runs after this one)
@@ -943,38 +941,15 @@ __global__ void __launch_bounds__(128) attn_wg_bwd_dq_kernel(const AttnKParams p
   const RSeq mkv = resolve(p.mkv, s), mo = resolve(p.mo, s), mdo = resolve(p.mdo, s), mdq = resolve(p.mdq, s);
   const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq), Mdo = rmat(p.dout, mdo, p.lddo, h * p.hsdo);
   const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
-  int kv_end = skv;
-  if (p.mask == MASK_CAUSAL) kv_end = min(skv, q0 + 64);
-  const int ntiles = (kv_end + 63) / 64;
+  int kv_begin;
+  const int ntiles = key_tiles<false>(p, q0, sq, skv, kv_begin);
 
-  wg_load_tile<D, DIO>(Qs, Mq, q0, sq);
-  wg_load_tile<D, DIO>(dOs, Mdo, q0, sq);
-  wg_load_tile<D, DIO>(KVs, Mk, 0, skv);
-  wg_load_tile<D, DIO>(KVs + TB, Mv, 0, skv);
+  load_tile<SWIZZLE_128B, D, DIO>(Qs, Mq, q0, sq);
+  load_tile<SWIZZLE_128B, D, DIO>(dOs, Mdo, q0, sq);
+  load_tile<SWIZZLE_128B, D, DIO>(KVs, Mk, kv_begin, skv);
+  load_tile<SWIZZLE_128B, D, DIO>(KVs + TB, Mv, kv_begin, skv);
   cp_async_commit();
-  {
-    const int r = lane >> 1, hf = lane & 1;
-    const int qi = q0 + warp * 16 + r;
-    float acc = 0.f;
-    if (qi < sq) {
-      const uint4* orow = reinterpret_cast<const uint4*>(p.o + rrow(mo, qi) * p.ldo + h * p.hso);
-      const uint4* drow = reinterpret_cast<const uint4*>(p.dout + rrow(mdo, qi) * p.lddo + h * p.hsdo);
-#pragma unroll
-      for (int c = hf; c < DIO / 8; c += 2) {
-        const uint4 a = __ldg(orow + c), b = __ldg(drow + c);
-        acc += bf16_lo(a.x) * bf16_lo(b.x) + bf16_hi(a.x) * bf16_hi(b.x) + bf16_lo(a.y) * bf16_lo(b.y) +
-               bf16_hi(a.y) * bf16_hi(b.y) + bf16_lo(a.z) * bf16_lo(b.z) + bf16_hi(a.z) * bf16_hi(b.z) +
-               bf16_lo(a.w) * bf16_lo(b.w) + bf16_hi(a.w) * bf16_hi(b.w);
-      }
-    }
-    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-    if (hf == 0) {
-      const size_t li = ((size_t)s * p.n_heads + h) * p.s_q + qi;
-      stat[64 + warp * 16 + r] = acc;
-      stat[warp * 16 + r] = (qi < sq) ? p.lse[li] * 1.4426950408889634f : CUDART_INF_F;
-      if (qi < sq) p.delta[li] = acc;
-    }
-  }
+  stage_dq_stats<DIO>(p, s, h, q0 + warp * 16, sq, mo, mdo, stat + warp * 16);
   float dq_acc[D / 8][4];
 #pragma unroll
   for (int i = 0; i < D / 8; ++i) { dq_acc[i][0] = dq_acc[i][1] = dq_acc[i][2] = dq_acc[i][3] = 0.f; }
@@ -984,13 +959,13 @@ __global__ void __launch_bounds__(128) attn_wg_bwd_dq_kernel(const AttnKParams p
   const uint32_t drow0 = (uint32_t)(((long)s * p.n_heads + h) * p.s_q + q0 + warp * 16 + g);
 
   for (int t = 0; t < ntiles; ++t) {
-    const int kv0 = t * 64;
+    const int kv0 = kv_begin + t * 64;
     uint8_t* Ks = KVs + (t & 1) * 2 * TB;
     uint8_t* Vs = Ks + TB;
     if (t + 1 < ntiles) {
       uint8_t* Kn = KVs + ((t + 1) & 1) * 2 * TB;
-      wg_load_tile<D, DIO>(Kn, Mk, kv0 + 64, skv);
-      wg_load_tile<D, DIO>(Kn + TB, Mv, kv0 + 64, skv);
+      load_tile<SWIZZLE_128B, D, DIO>(Kn, Mk, kv0 + 64, skv);
+      load_tile<SWIZZLE_128B, D, DIO>(Kn + TB, Mv, kv0 + 64, skv);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -1006,34 +981,12 @@ __global__ void __launch_bounds__(128) attn_wg_bwd_dq_kernel(const AttnKParams p
     wg_scores<D>(sc, smem_u32(Qs), smem_u32(Ks));
     wg_scores<D>(dp, smem_u32(dOs), smem_u32(Vs));
     if (tile_needs_mask(p, q0 + warp * 16, kv0, skv)) apply_mask(p, sc, q0 + warp * 16, kv0, skv, g, t4, -CUDART_INF_F);
-    if (p.has_drop) {  // dP = dropout'(dO V^T): the same keep bits and scale as the forward
-#pragma unroll
-      for (int nb = 0; nb < 8; ++nb) {
-        const uint32_t col = (uint32_t)(kv0 + nb * 8 + t4 * 2);
-        drop2(ds, drow0, col, dp[nb][0], dp[nb][1]);
-        drop2(ds, drow0 + 8, col, dp[nb][2], dp[nb][3]);
-      }
-    }
-#pragma unroll
-    for (int nb = 0; nb < 8; ++nb) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float pv = exp2f(fmaf(sc[nb][e], p.scale_log2, -lse_r[e >> 1]));
-        sc[nb][e] = pv * (dp[nb][e] - del_r[e >> 1]);  // dS
-      }
-    }
+    if (p.has_drop) drop_tile(ds, drow0, kv0, t4, dp);  // dP = dropout'(dO V^T)
+    scores_to_ds(p, sc, dp, lse_r, del_r);
     wg_pv<D>(dq_acc, sc, smem_u32(Ks));
     __syncthreads();
   }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int qi = q0 + warp * 16 + g + r * 8;
-    if (qi >= sq) continue;
-    __nv_bfloat16* dqrow = p.dq + rrow(mdq, qi) * p.lddq + h * p.hsdq;
-#pragma unroll
-    for (int nb = 0; nb < DIO / 8; ++nb)
-      *reinterpret_cast<uint32_t*>(dqrow + nb * 8 + t4 * 2) = pack_bf16(dq_acc[nb][2 * r] * p.scale, dq_acc[nb][2 * r + 1] * p.scale);
-  }
+  store_dq<D, DIO>(p, dq_acc, q0 + warp * 16, sq, h, mdq, g, t4);
 }
 
 // dK, dV: CTA = 64 key rows, streams Q / dO tiles; everything in the transposed frame (rows = keys, columns = queries)
@@ -1061,18 +1014,13 @@ __global__ void __launch_bounds__(128) attn_wg_bwd_dkdv_kernel(const AttnKParams
 
   auto load_stage = [&](int stage, int qi0) {
     uint8_t* Qn = QDs + stage * 2 * TB;
-    wg_load_tile<D, DIO>(Qn, Mq, qi0, sq);
-    wg_load_tile<D, DIO>(Qn + TB, Mdo, qi0, sq);
-    if (threadIdx.x < 64) {
-      const int qi = qi0 + threadIdx.x;
-      float* st = stat + stage * 128;
-      st[threadIdx.x] = (qi < sq) ? p.lse[stat_base + qi] * 1.4426950408889634f : CUDART_INF_F;
-      st[64 + threadIdx.x] = (qi < sq) ? p.delta[stat_base + qi] : 0.f;
-    }
+    load_tile<SWIZZLE_128B, D, DIO>(Qn, Mq, qi0, sq);
+    load_tile<SWIZZLE_128B, D, DIO>(Qn + TB, Mdo, qi0, sq);
+    stage_dkdv_stats(p, stat_base, qi0, sq, stat + stage * 128);
   };
 
-  wg_load_tile<D, DIO>(Ks, Mk, kv0, skv);
-  wg_load_tile<D, DIO>(Vs, Mv, kv0, skv);
+  load_tile<SWIZZLE_128B, D, DIO>(Ks, Mk, kv0, skv);
+  load_tile<SWIZZLE_128B, D, DIO>(Vs, Mv, kv0, skv);
   load_stage(0, q_begin);
   cp_async_commit();
 
@@ -1085,7 +1033,6 @@ __global__ void __launch_bounds__(128) attn_wg_bwd_dkdv_kernel(const AttnKParams
   DropState ds;  // only read when has_drop
   if (p.has_drop) ds = drop_state(p.drop);
   const uint32_t dbase = (uint32_t)stat_base;
-  const int k0 = kv0 + warp * 16 + g, k1 = k0 + 8;  // this thread's two key rows (elements 0, 1 and 2, 3)
 
   for (int t = 0; t < ntiles; ++t) {
     const int qi0 = q_begin + t * 64;
@@ -1104,74 +1051,13 @@ __global__ void __launch_bounds__(128) attn_wg_bwd_dkdv_kernel(const AttnKParams
     float st_[8][4], dpt[8][4];
     wg_scores<D>(st_, smem_u32(Ks), smem_u32(Qs));   // S^T = K Q^T
     wg_scores<D>(dpt, smem_u32(Vs), smem_u32(dOs));  // dZ^T = V dO^T
-    {
-      const int k_lo = kv0 + warp * 16;
-      const bool need = (k_lo + 16 > skv) || (p.mask == MASK_CAUSAL && k_lo + 15 > qi0);
-      if (need) {
-#pragma unroll
-        for (int nb = 0; nb < 8; ++nb) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int qc = qi0 + nb * 8 + t4 * 2 + e;
-            bool m0 = k0 >= skv, m1 = k1 >= skv;
-            if (p.mask == MASK_CAUSAL) { m0 |= k0 > qc; m1 |= k1 > qc; }
-            if (m0) st_[nb][e] = -CUDART_INF_F;
-            if (m1) st_[nb][2 + e] = -CUDART_INF_F;
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int nb = 0; nb < 8; ++nb) {
-      // dropout keep bits of the four (query, key) pairs this thread holds, bit e for element e: queries q, q + 1 and keys
-      // k0, k1 = k0 + 8.  The four lanes g = 4a .. 4a+3 (same t4) need the same four Philox calls (rows q / q + 1, key
-      // groups of k0 / k1), each a different word of them: lane j = g & 3 makes call j and the words are exchanged.
-      uint32_t keep = 0xFu;
-      if (p.has_drop) {
-        const int j = g & 3;
-        const uint32_t qr = dbase + (uint32_t)(qi0 + nb * 8 + t4 * 2 + (j & 1));
-        const uint4 w = drop_words(ds, qr, (uint32_t)(kv0 + warp * 16 + (g & ~3) + (j >> 1) * 8) >> 2);
-        keep = 0;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int comp = (j + r) & 3, c = (j - r) & 3;  // send word comp, receive call c's word j
-          const uint32_t v = comp == 0 ? w.x : comp == 1 ? w.y : comp == 2 ? w.z : w.w;
-          const uint32_t got = __shfl_sync(0xffffffffu, v, (lane & ~0xC) | (c << 2));
-          keep |= (got >= ds.thresh ? 1u : 0u) << c;
-        }
-      }
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int ql = nb * 8 + t4 * 2 + (e & 1);
-        const float pv = exp2f(fmaf(st_[nb][e], p.scale_log2, -st[ql]));  // lse=+inf for absent queries -> 0
-        float dz = dpt[nb][e];
-        if (p.has_drop) {  // Z = dropout(P): dV += Z^T dO, dP = dropout'(dZ)
-          const float kf = (keep >> e) & 1u ? ds.scale : 0.f;
-          dz *= kf;
-          st_[nb][e] = pv * kf;  // Z^T
-        } else {
-          st_[nb][e] = pv;       // P^T
-        }
-        dpt[nb][e] = pv * (dz - st[64 + ql]);  // dS^T
-      }
-    }
+    apply_mask_t<false>(p, st_, kv0 + warp * 16, qi0, skv, g, t4);
+    probs_t<true>(p, ds, st_, dpt, st, dbase + (uint32_t)qi0, kv0 + warp * 16, lane);
     wg_pv<D>(dv_acc, st_, smem_u32(dOs));
     wg_pv<D>(dk_acc, dpt, smem_u32(Qs));
     __syncthreads();
   }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int kvr = kv0 + warp * 16 + g + r * 8;
-    if (kvr >= skv) continue;
-    const long row = rrow(mdkv, kvr);
-    __nv_bfloat16* dkrow = p.dk + row * p.lddk + h * p.hsdk;
-    __nv_bfloat16* dvrow = p.dv + row * p.lddv + h * p.hsdv;
-#pragma unroll
-    for (int nb = 0; nb < DIO / 8; ++nb) {
-      *reinterpret_cast<uint32_t*>(dkrow + nb * 8 + t4 * 2) = pack_bf16(dk_acc[nb][2 * r] * p.scale, dk_acc[nb][2 * r + 1] * p.scale);
-      *reinterpret_cast<uint32_t*>(dvrow + nb * 8 + t4 * 2) = pack_bf16(dv_acc[nb][2 * r], dv_acc[nb][2 * r + 1]);
-    }
-  }
+  store_dkdv<D, DIO>(p, dk_acc, dv_acc, kv0 + warp * 16, skv, h, mdkv, g, t4);
 }
 
 // ------------------------------------------------------------------------------ single-query forward (decoding)
@@ -1288,41 +1174,6 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
   }
   if (p.lse && threadIdx.x == 0) p.lse[((long)s * p.n_heads + h) * p.s_q] = (m_all + log2f(l_all)) * 0.6931471805599453f;
 }
-template <int D>
-static int launch_decode(const AttnKParams& p, cudaStream_t st) {
-  constexpr int smem = (128 * (D + 1) + 128 + 4) * 4;
-  static DeviceOnce once;
-  if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(attn_decode_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
-  launch_k(attn_decode_kernel<D>, dim3(p.n_heads, p.n_seq), dim3(128), smem, st, p);
-  YMP_LAUNCH_CHECK();
-  return YMP_OK;
-}
-
-template <int D, int DIO = D>
-static int launch_wg_fwd(const AttnKParams& p, cudaStream_t st) {
-  const int smem = 5 * WgTile<D>::BYTES + 1024;
-  static DeviceOnce once;
-  if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(attn_wg_fwd_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
-  const int lead = p.mask == MASK_CAUSAL ? (p.s_kv - p.s_q) & 63 : 0;  // padding rows before query 0 (offset causal)
-  launch_k(attn_wg_fwd_kernel<D, DIO>, dim3((p.s_q + lead + 63) / 64, p.n_heads, p.n_seq), dim3(128), smem, st, p);
-  YMP_LAUNCH_CHECK();
-  return YMP_OK;
-}
-template <int D, int DIO = D>
-static int launch_wg_bwd(const AttnKParams& p, cudaStream_t st) {
-  const int smem = 6 * WgTile<D>::BYTES + 1024 + 1024;
-  static DeviceOnce once;
-  if (once.first()) {
-    YMP_CUDA(cudaFuncSetAttribute(attn_wg_bwd_dq_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    YMP_CUDA(cudaFuncSetAttribute(attn_wg_bwd_dkdv_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  }
-  attn_wg_bwd_dq_kernel<D, DIO><<<dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
-  YMP_LAUNCH_CHECK();
-  attn_wg_bwd_dkdv_kernel<D, DIO><<<dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
-  YMP_LAUNCH_CHECK();
-  return YMP_OK;
-}
-
 static int fill_params(const ymp_attn_args* a, AttnKParams& p, const char* who) {
   YMP_CHECK_ARG(a && a->q && a->k && a->v, "%s: null q/k/v", who);
   YMP_CHECK_ARG(a->head_dim == 64 || a->head_dim == 80 || a->head_dim == 88 || a->head_dim == 96 || a->head_dim == 128,
@@ -1344,7 +1195,7 @@ static int fill_params(const ymp_attn_args* a, AttnKParams& p, const char* who) 
   p.mq = to_map(a->map_q); p.mkv = to_map(a->map_kv); p.mo = to_map(a->map_o);
   p.n_seq = a->n_seq; p.n_heads = a->n_heads; p.s_q = a->s_q; p.s_kv = a->s_kv;
   p.mask = a->mask; p.mask_block = a->mask_block > 0 ? a->mask_block : 1; p.total_rows = a->total_rows;
-  p.scale = a->scale; p.scale_log2 = a->scale * 1.4426950408889634f;
+  p.scale = a->scale; p.scale_log2 = a->scale * LOG2E;
   p.skv_dev = a->s_kv_dev;
   p.kv_rows = a->kv_rows; p.kv_rows_ld = a->kv_rows_ld;
   p.has_drop = (a->drop.rng && a->drop.p > 0.f) ? 1 : 0;
@@ -1352,29 +1203,74 @@ static int fill_params(const ymp_attn_args* a, AttnKParams& p, const char* who) 
   return YMP_OK;
 }
 
-template <int D, int DIO = D>
-static int launch_fwd(const AttnKParams& p, cudaStream_t st) {
-  const int smem = 5 * 64 * (D + 8) * 2;
+// The <D, DIO> instantiation that serves a head_dim: 88 is computed as 96 with zero-filled tail columns.
+template <int D_, int DIO_ = D_>
+struct HeadDim {
+  static constexpr int D = D_, DIO = DIO_;
+};
+// launch(HeadDim<D, DIO>{}) for a head_dim that fill_params accepted.  WITH_128: the family has head_dim-128 kernels
+// (only the mma.sync one; the routing never sends head_dim 128 to the others).
+template <bool WITH_128, class F>
+static int for_head_dim(int head_dim, F&& launch) {
+  switch (head_dim) {
+    case 64: return launch(HeadDim<64>{});
+    case 80: return launch(HeadDim<80>{});
+    case 88: return launch(HeadDim<96, 88>{});
+    case 96: return launch(HeadDim<96>{});
+  }
+  if constexpr (WITH_128) return launch(HeadDim<128>{});
+  else return set_error(YMP_EINVAL, "attention: no kernel of this family for head_dim %d", head_dim);
+}
+// One launch of 128 threads with `smem` bytes of dynamic shared memory (opted in once per device and kernel).  PDL: the
+// kernel calls griddep_wait before it reads its inputs, so it goes through launch_k, which honours ymp_set_pdl.  The
+// backward kernels never wait on the previous grid and must take an ordinary launch.
+template <void (*K)(AttnKParams), bool PDL>
+static int launch_attn(dim3 grid, int smem, cudaStream_t st, const AttnKParams& p) {
   static DeviceOnce once;
-  if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
-  dim3 grid((p.s_q + 63) / 64, p.n_heads, p.n_seq);
-  launch_k(attn_fwd_kernel<D, DIO>, grid, dim3(128), smem, st, p);
+  if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
+  if constexpr (PDL) launch_k(K, grid, dim3(128), smem, st, p);
+  else K<<<grid, 128, smem, st>>>(p);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }
-template <int D, int DIO = D>
-static int launch_bwd(const AttnKParams& p, cudaStream_t st) {
-  const int smem = 6 * 64 * (D + 8) * 2 + 1024;
-  static DeviceOnce once;
-  if (once.first()) {
-    YMP_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    YMP_CUDA(cudaFuncSetAttribute(attn_bwd_dkdv_kernel<D, DIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  }
-  attn_bwd_dq_kernel<D, DIO><<<dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
-  YMP_LAUNCH_CHECK();
-  attn_bwd_dkdv_kernel<D, DIO><<<dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), 128, smem, st>>>(p);
-  YMP_LAUNCH_CHECK();
-  return YMP_OK;
+
+static int launch_decode(const AttnKParams& p, int head_dim, cudaStream_t st) {
+  return for_head_dim<false>(head_dim, [&](auto hd) {
+    constexpr int D = decltype(hd)::D;
+    return launch_attn<attn_decode_kernel<D>, true>(dim3(p.n_heads, p.n_seq), (128 * (D + 1) + 128 + 4) * 4, st, p);
+  });
+}
+static int launch_wg_fwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
+  const int lead = p.mask == MASK_CAUSAL ? (p.s_kv - p.s_q) & 63 : 0;  // padding rows before query 0 (offset causal)
+  const dim3 grid((p.s_q + lead + 63) / 64, p.n_heads, p.n_seq);
+  return for_head_dim<false>(head_dim, [&](auto hd) {
+    using H = decltype(hd);
+    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO>, true>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
+  });
+}
+static int launch_wg_bwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
+  return for_head_dim<false>(head_dim, [&](auto hd) {
+    using H = decltype(hd);
+    const int smem = 6 * WgTile<H::D>::BYTES + 1024 + 1024;
+    const int rc = launch_attn<attn_wg_bwd_dq_kernel<H::D, H::DIO>, false>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
+    if (rc) return rc;
+    return launch_attn<attn_wg_bwd_dkdv_kernel<H::D, H::DIO>, false>(dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
+  });
+}
+static int launch_fwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
+  return for_head_dim<true>(head_dim, [&](auto hd) {
+    using H = decltype(hd);
+    return launch_attn<attn_fwd_kernel<H::D, H::DIO>, true>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), 5 * 64 * (H::D + 8) * 2, st, p);
+  });
+}
+static int launch_bwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
+  return for_head_dim<true>(head_dim, [&](auto hd) {
+    using H = decltype(hd);
+    const int smem = 6 * 64 * (H::D + 8) * 2 + 1024;
+    const int rc = launch_attn<attn_bwd_dq_kernel<H::D, H::DIO>, false>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
+    if (rc) return rc;
+    return launch_attn<attn_bwd_dkdv_kernel<H::D, H::DIO>, false>(dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
+  });
 }
 
 }  // namespace ymp
@@ -1408,20 +1304,11 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
     YMP_CHECK_ARG(!dropped, "ymp_attn_fwd: causal with s_q < s_kv takes no dropout");
     YMP_CHECK_ARG(!a->s_kv_dev, "ymp_attn_fwd: causal with s_q < s_kv takes no s_kv_dev");
     g_attn_path = YMP_ATTN_PATH_WGMMA;
-    switch (a->head_dim) {
-      case 64: return launch_wg_fwd<64>(p, st);
-      case 80: return launch_wg_fwd<80>(p, st);
-      case 88: return launch_wg_fwd<96, 88>(p, st);
-      default: return launch_wg_fwd<96>(p, st);
-    }
+    return launch_wg_fwd(p, a->head_dim, st);
   }
   if (a->s_q == 1 && a->mask == YMP_MASK_NONE && a->total_rows == 0 && !dropped && a->head_dim != 88 && a->head_dim != 128) {
     g_attn_path = YMP_ATTN_PATH_DECODE;   // one query row per sequence: the streaming kernel (also follows s_kv_dev)
-    switch (a->head_dim) {
-      case 64: return launch_decode<64>(p, st);
-      case 80: return launch_decode<80>(p, st);
-      default: return launch_decode<96>(p, st);
-    }
+    return launch_decode(p, a->head_dim, st);
   }
   const bool dev_len = a->s_kv_dev != nullptr;  // key count read on the device: the mma.sync kernels bound their KV loop by it
   YMP_CHECK_ARG(!dev_len || (!dropped && a->mask == YMP_MASK_NONE && a->total_rows == 0 && a->head_dim != 88),
@@ -1434,21 +1321,10 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   // skip the masked chunks warp by warp), the device-side key count, a row table and a few query rows against a long cache
   if (a->head_dim != 128 && a->mask != YMP_MASK_BLOCK && !dev_len && !a->kv_rows && !(a->s_q < 16 && a->s_kv > 256)) {
     g_attn_path = YMP_ATTN_PATH_WGMMA;
-    switch (a->head_dim) {
-      case 64: return launch_wg_fwd<64>(p, st);
-      case 80: return launch_wg_fwd<80>(p, st);
-      case 88: return launch_wg_fwd<96, 88>(p, st);
-      default: return launch_wg_fwd<96>(p, st);
-    }
+    return launch_wg_fwd(p, a->head_dim, st);
   }
   g_attn_path = YMP_ATTN_PATH_MMA_SYNC;
-  switch (a->head_dim) {
-    case 64: return launch_fwd<64>(p, st);
-    case 80: return launch_fwd<80>(p, st);
-    case 88: return launch_fwd<96, 88>(p, st);
-    case 96: return launch_fwd<96>(p, st);
-    default: return launch_fwd<128>(p, st);
-  }
+  return launch_fwd(p, a->head_dim, st);
 }
 
 extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {
@@ -1477,19 +1353,8 @@ extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {
   }
   if (a->head_dim != 128 && a->mask != YMP_MASK_BLOCK) {
     g_attn_path = YMP_ATTN_PATH_WGMMA;
-    switch (a->head_dim) {
-      case 64: return launch_wg_bwd<64>(p, st);
-      case 80: return launch_wg_bwd<80>(p, st);
-      case 88: return launch_wg_bwd<96, 88>(p, st);
-      default: return launch_wg_bwd<96>(p, st);
-    }
+    return launch_wg_bwd(p, a->head_dim, st);
   }
   g_attn_path = YMP_ATTN_PATH_MMA_SYNC;
-  switch (a->head_dim) {
-    case 64: return launch_bwd<64>(p, st);
-    case 80: return launch_bwd<80>(p, st);
-    case 88: return launch_bwd<96, 88>(p, st);
-    case 96: return launch_bwd<96>(p, st);
-    default: return launch_bwd<128>(p, st);
-  }
+  return launch_bwd(p, a->head_dim, st);
 }

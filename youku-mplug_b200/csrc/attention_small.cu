@@ -28,24 +28,6 @@ struct SmallParams {
 };
 
 namespace {
-__device__ __forceinline__ void sm_cp16(void* smem, const void* gmem) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void sm_ldsm(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void sm_ldsm_t(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void sm_mma(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-      "{%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ uint32_t sm_movt(uint32_t a) {
   uint32_t d;
   asm volatile("movmatrix.sync.aligned.m8n8.trans.b16 %0, %1;" : "=r"(d) : "r"(a));
@@ -66,7 +48,7 @@ __device__ __forceinline__ void load16(uint8_t* tile, const __nv_bfloat16* base,
     const int c = lane + 32 * j;
     if (c < 16 * CPR) {
       const int r = c / CPR, cc = c - r * CPR;
-      if (r < nrows) sm_cp16(tile + r * PITCH + cc * 16, base + (long)r * ld + cc * 8);
+      if (r < nrows) cp_async16(tile + r * PITCH + cc * 16, base + (long)r * ld + cc * 8);
       else *reinterpret_cast<uint4*>(tile + r * PITCH + cc * 16) = make_uint4(0, 0, 0, 0);
     }
   }
@@ -101,10 +83,10 @@ __device__ __forceinline__ void mma_abt(float (&c)[2][4], const uint8_t* A, cons
 #pragma unroll
   for (int kk = 0; kk < HD / 16; ++kk) {
     uint32_t a[4], b[4];
-    sm_ldsm(a, smem_u32(A + (lane & 15) * PITCH + kk * 32 + (lane >> 4) * 16));
-    sm_ldsm(b, smem_u32(B + ((lane & 7) + (lane >> 4) * 8) * PITCH + kk * 32 + ((lane >> 3) & 1) * 16));
-    sm_mma(c[0], a, b[0], b[1]);
-    sm_mma(c[1], a, b[2], b[3]);
+    ldsm_x4(a, smem_u32(A + (lane & 15) * PITCH + kk * 32 + (lane >> 4) * 16));
+    ldsm_x4(b, smem_u32(B + ((lane & 7) + (lane >> 4) * 8) * PITCH + kk * 32 + ((lane >> 3) & 1) * 16));
+    mma16816(c[0], a, b[0], b[1]);
+    mma16816(c[1], a, b[2], b[3]);
   }
 }
 // C[16 x HD] = A[16 x 16] (register fragments) * B[16 x HD] (smem tile, rows = contraction index)
@@ -116,9 +98,9 @@ __device__ __forceinline__ void mma_ab(float (&c)[HD / 8][4], const uint32_t (&a
 #pragma unroll
   for (int dbp = 0; dbp < HD / 16; ++dbp) {
     uint32_t b[4];
-    sm_ldsm_t(b, smem_u32(B + ((lane & 7) + ((lane >> 3) & 1) * 8) * PITCH + dbp * 32 + (lane >> 4) * 16));
-    sm_mma(c[2 * dbp], a, b[0], b[1]);
-    sm_mma(c[2 * dbp + 1], a, b[2], b[3]);
+    ldsm_x4_t(b, smem_u32(B + ((lane & 7) + ((lane >> 3) & 1) * 8) * PITCH + dbp * 32 + (lane >> 4) * 16));
+    mma16816(c[2 * dbp], a, b[0], b[1]);
+    mma16816(c[2 * dbp + 1], a, b[2], b[3]);
   }
 }
 }  // namespace

@@ -232,14 +232,6 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (LN ? 2 : 1)) gemm_skinny_kerne
   }
 }
 
-__device__ __forceinline__ void mma16816_bf16_rows16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
-                                                     uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
 // 9 <= M <= 64: gemm_skinny_kernel's grid, warp roles, K slices, weight stream and k-block loop (SK_UNROLL = 4, the same
 // zero-padded tail), with one accumulator set per group of 16 rows.  Group j's lane (g, t) holds rows 16j + g (acc[j][0..1])
 // and 16j + 8 + g (acc[j][2..3]).  The activation chunks of the k-block being consumed are loaded from global memory
@@ -286,8 +278,9 @@ __global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(cons
         for (int j = 0; j < SK_WIDE_GROUPS; ++j) {
           if (j < groups) {
             const uint4 lo = fetch_x(16 * j + g, b + u, c), hi = fetch_x(16 * j + 8 + g, b + u, c);
-            mma16816_bf16_rows16(acc[j], lo.x, hi.x, lo.y, hi.y, wv[u].x, wv[u].y);
-            mma16816_bf16_rows16(acc[j], lo.z, hi.z, lo.w, hi.w, wv[u].z, wv[u].w);
+            const uint32_t a0[4] = {lo.x, hi.x, lo.y, hi.y}, a1[4] = {lo.z, hi.z, lo.w, hi.w};
+            mma16816(acc[j], a0, wv[u].x, wv[u].y);
+            mma16816(acc[j], a1, wv[u].z, wv[u].w);
           }
         }
       }
