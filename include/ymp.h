@@ -88,6 +88,8 @@ typedef struct ymp_dropout_spec {
  *   if drop:    v = dropout(v)           (row = m, column = n; bias-dropout-add: residual + dropout(x + bias))
  *   v += residual[m,n]                   (bf16 or fp32 [M,N], row stride ldr, optional)
  *   D[m,n] = v  (bf16 or fp32) ; or atomically D[m,n] += v (fp32, accumulate=1, used by split-K)
+ *   accumulate=1 allows alpha only: no bias, act, aux_out, aux_in or residual (each K-split adds its own partial
+ *   product to D, so a bias would be counted once per split; the library picks the split when split_k = 0)
  * ------------------------------------------------------------------------------------------ */
 #define YMP_ACT_NONE 0
 #define YMP_ACT_GELU_ERF 1  /* nn.GELU() exact: ViT / abstractor MLP (vision_transformer.py:94) */
@@ -110,7 +112,7 @@ typedef struct ymp_gemm_args {
   void* aux_out;        /* bf16 [M,N] (ld = ldd) or NULL: act'(pre-activation) (or the value if act=NONE) */
   const void* aux_in;   /* bf16 [M,N] (ld = ldd) or NULL: element-wise multiplier */
   int32_t out_dtype;    /* YMP_DT_BF16 | YMP_DT_F32 */
-  int32_t accumulate;   /* 1: D (fp32) += result using atomics */
+  int32_t accumulate;   /* 1: D (fp32) += alpha * op(A) . op(B)^T using atomics; bias, act, aux, residual must be unset */
   int32_t split_k;      /* >=1; >1 requires accumulate=1 and out_dtype=F32; 0 = library picks */
   float alpha;
   int32_t tile_n;       /* 0 = auto, else 128 or 256 (512 is accepted and means 256) */

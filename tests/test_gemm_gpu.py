@@ -128,9 +128,10 @@ def test_gemm_large_persistent(cuda):
 
 @pytest.mark.parametrize("M", [1000, 2560 + 37])
 def test_gemm_pair_tile_tma_epilogue_variants(cuda, M):
-    """CTA-pair kernel, epilogue staged through swizzled smem and written with bulk tensor stores / reduce-adds:
-    ragged M (rows clipped by the tensor map), fp32 residual stream in and out, bf16 + act' pairs, row-strided
-    outputs, split-K accumulation into a non-zero buffer, several tiles per CTA pair (staging-buffer reuse)."""
+    """The widest tile (128 x 256) with its epilogue variants: ragged M (rows past M skipped by the epilogue), fp32
+    residual stream in and out (also in place), bf16 + act' pairs into column slices of wider buffers, the activation
+    backward's multiplier, split-K accumulation (fp32 vector atomics) into a non-zero buffer, and many more tiles than
+    SMs (the staging tile reuses the operand ring)."""
     from ymp import ops
     torch.manual_seed(5)
     N, K = 768, 320

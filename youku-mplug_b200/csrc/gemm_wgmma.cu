@@ -510,7 +510,8 @@ extern "C" int ymp_gemm(const ymp_gemm_args* a, void* stream) {
   YMP_CHECK_ARG(!a->aux_out || aligned16(a->aux_out), "ymp_gemm: aux_out alignment");
   YMP_CHECK_ARG(!a->aux_in || aligned16(a->aux_in), "ymp_gemm: aux_in alignment");
   YMP_CHECK_ARG(!(a->accumulate && a->out_dtype != YMP_DT_F32), "ymp_gemm: accumulate needs fp32 output");
-  YMP_CHECK_ARG(!(a->accumulate && (a->aux_out || a->aux_in || a->act || a->residual)),
+  // every K-split's epilogue adds its partial to D, so a bias would be added once per split
+  YMP_CHECK_ARG(!(a->accumulate && (a->bias || a->aux_out || a->aux_in || a->act || a->residual)),
                 "ymp_gemm: accumulate mode supports only alpha and bias-free linear epilogue");
   YMP_CHECK_ARG(a->res_row_mod >= 0 && a->d_row_block >= 0 && (a->d_row_block == 0 || a->d_row_stride >= a->d_row_block),
                 "ymp_gemm: bad res_row_mod / d_row_block / d_row_stride");
