@@ -209,6 +209,8 @@ typedef struct ymp_layernorm_bwd_args {
                          the A operand of the dgrad GEMM below that bias-dropout-add */
   ymp_dropout_spec drop;
 } ymp_layernorm_bwd_args;
+/* Rows are read and written in 16-byte vectors: dy, x, gamma, dx, add, dx_drop, dgamma and dbeta must be 16-byte
+ * aligned, and ldx, lddy, ldadd must be multiples of 8 and >= D (YMP_EINVAL otherwise). */
 int ymp_layernorm_bwd(const ymp_layernorm_bwd_args* a, void* stream);
 
 /* ------------------------------------------------------------------------------------------
@@ -313,6 +315,9 @@ typedef struct ymp_im2col_args {
   void* out;
   int32_t B, C, T, H, W, P, ldo;
 } ymp_im2col_args;
+/* ldo >= C*P*P, a multiple of 8, out 16-byte aligned.  P % 8 == 0 and W % 8 == 0 (video also 16-byte aligned) take the
+ * vector kernel, which writes columns [0, C*P*P) of each row and leaves [C*P*P, ldo) alone.  Any other P or W takes the
+ * element kernel, which also writes zeros to columns [C*P*P, ldo) of each row (the zero K padding of a GEMM operand). */
 int ymp_im2col(const ymp_im2col_args* a, void* stream);
 
 /* ------------------------------------------------------------------------------------------
@@ -357,6 +362,8 @@ typedef struct ymp_embed_args {
   int32_t B, L, S, row_offset, hidden, vocab, ldo;
   int32_t out_dtype;   /* YMP_DT_BF16 | YMP_DT_F32 */
 } ymp_embed_args;
+/* hidden and ldo multiples of 8, ldo >= hidden, vocab > 0 (ids are clamped to [0, vocab)), and table, pos, out 16-byte
+ * aligned (YMP_EINVAL otherwise).  Only the rows b*S + row_offset + l, l < L, are written. */
 int ymp_embed_gather(const ymp_embed_args* a, void* stream);
 
 /* Softmax cross entropy over the vocabulary, per-token (unreduced) losses.  Replaces
@@ -390,6 +397,7 @@ typedef struct ymp_group_args {
   int32_t G, T, C, ld_in, ld_out, broadcast;
   float scale;
 } ymp_group_args;
+/* C, ld_in, ld_out multiples of 8, ld_in and ld_out >= C, in and out 16-byte aligned (YMP_EINVAL otherwise). */
 int ymp_group_reduce(const ymp_group_args* a, void* stream);
 
 /* ------------------------------------------------------------------------------------------

@@ -45,7 +45,8 @@ covers results that underflow.
     e_out = C [e + u32 |out| [residual] + split u32 (|D0| + |alpha||A||B|) [accumulate] + u |out| [bf16]] + 2^-100
 
 LayerNorm of the skinny kernel (fp32 y, two-pass statistics over n = N columns, rsqrt.approx):
-    e_mean = (n + 1) u32 mean|y|,   relative variance error e_var = (n + 4) u32 + (e_mean / sigma)^2,
+    e_mean = (n + 1) u32 mean|y|,   relative error of var + eps: e_var = ((n + 4) u32 var + e_mean^2) / (var + eps)
+    (the sum of squares of the deviations from the computed mean is off by n e_mean^2 at most),
     e_rstd = 0.5 e_var + 2^-22 (rsqrt.approx) + 2 u32,
     e_ln   = C [|gamma| (e_mean rstd + |z| (e_rstd + 2 u32)) + u32 |gamma z| + u |ln|] + 2^-100,  z = (y - mean) rstd.
 """
@@ -247,15 +248,24 @@ def layernorm_reference(y, gamma, beta, eps):
     return z * gamma.double() + beta.double(), z, rstd, y.abs().mean(-1, keepdim=True), var.sqrt()
 
 
-def layernorm_bound(y, gamma, beta, eps):
-    """Per-element bound on |ln_out - LN(y)| (module docstring, LayerNorm of the skinny kernel)."""
+def layernorm_stat_errors(y, eps):
+    """(e_mean, e_rstd) per row, before the safety factor: the absolute error of the fp32 mean and the relative error of
+    the fp32 rstd (module docstring).  The variance error is taken relative to var + eps, which is what rstd sees."""
     n = y.shape[-1]
-    ln, z, rstd, mabs, sigma = layernorm_reference(y, gamma, beta, eps)
-    e_mean = (n + 1) * U32 * mabs
-    e_var = (n + 4) * U32 + (e_mean / sigma.clamp(min=1e-30)) ** 2
-    e_rstd = 0.5 * e_var + 2.0 ** -22 + 2 * U32
+    y = y.double()
+    var = y.var(-1, unbiased=False, keepdim=True)
+    e_mean = (n + 1) * U32 * y.abs().mean(-1, keepdim=True)
+    e_var = ((n + 4) * U32 * var + e_mean ** 2) / (var + eps)
+    return e_mean, 0.5 * e_var + 2.0 ** -22 + 2 * U32
+
+
+def layernorm_bound(y, gamma, beta, eps, out_bf16=True):
+    """Per-element bound on |ln_out - LN(y)| (module docstring, LayerNorm of the skinny kernel; an fp32 output rounds
+    once, u32 |ln|, instead of u |ln|)."""
+    ln, z, rstd, _, _ = layernorm_reference(y, gamma, beta, eps)
+    e_mean, e_rstd = layernorm_stat_errors(y, eps)
     g = gamma.double().abs()
-    e = g * (e_mean * rstd + z.abs() * (e_rstd + 2 * U32)) + U32 * (g * z).abs() + U * ln.abs()
+    e = g * (e_mean * rstd + z.abs() * (e_rstd + 2 * U32)) + U32 * (g * z).abs() + (U if out_bf16 else U32) * ln.abs()
     return C * e + TINY
 
 

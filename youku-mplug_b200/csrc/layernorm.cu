@@ -265,7 +265,10 @@ extern "C" int ymp_layernorm_bwd(const ymp_layernorm_bwd_args* a, void* stream) 
   YMP_CHECK_ARG(a->rows > 0 && a->D > 0 && a->D % 8 == 0 && a->D <= 4096, "ymp_layernorm_bwd: bad D=%d", a->D);
   YMP_CHECK_ARG((a->dgamma == nullptr) == (a->dbeta == nullptr), "ymp_layernorm_bwd: dgamma/dbeta must both be set or both NULL");
   YMP_CHECK_ARG(!a->dgamma || (aligned16(a->dgamma) && aligned16(a->dbeta)), "ymp_layernorm_bwd: dgamma/dbeta must be 16-byte aligned");
-  YMP_CHECK_ARG(a->ldx % 8 == 0 && a->lddy % 8 == 0 && (!a->add || a->ldadd % 8 == 0), "ymp_layernorm_bwd: bad ld");
+  YMP_CHECK_ARG(a->ldx % 8 == 0 && a->lddy % 8 == 0 && (!a->add || a->ldadd % 8 == 0) && a->ldx >= a->D && a->lddy >= a->D &&
+                (!a->add || a->ldadd >= a->D), "ymp_layernorm_bwd: bad ld");
+  YMP_CHECK_ARG(aligned16(a->dy) && aligned16(a->x) && aligned16(a->gamma) && aligned16(a->dx) && (!a->add || aligned16(a->add)),
+                "ymp_layernorm_bwd: 16-byte alignment required");
   LnBwdParams p;
   p.dy = (const __nv_bfloat16*)a->dy; p.x = a->x; p.gamma = (const __nv_bfloat16*)a->gamma;
   p.mean = a->mean; p.rstd = a->rstd; p.add = (const __nv_bfloat16*)a->add; p.dx = (__nv_bfloat16*)a->dx;

@@ -410,6 +410,8 @@ extern "C" int ymp_embed_gather(const ymp_embed_args* a, void* stream) {
   YMP_CHECK_ARG(a && a->ids && a->table && a->out, "ymp_embed_gather: null pointer");
   YMP_CHECK_ARG(a->hidden % 8 == 0 && a->ldo % 8 == 0 && a->ldo >= a->hidden, "ymp_embed_gather: hidden/ldo must be multiples of 8");
   YMP_CHECK_ARG(a->B > 0 && a->L > 0 && a->S >= a->row_offset + a->L, "ymp_embed_gather: bad B/L/S/offset");
+  YMP_CHECK_ARG(a->vocab > 0, "ymp_embed_gather: vocab must be positive");
+  YMP_CHECK_ARG(aligned16(a->table) && (!a->pos || aligned16(a->pos)) && aligned16(a->out), "ymp_embed_gather: 16-byte alignment required");
   const int rows = a->B * a->L;
   const int blocks = min((rows + 7) / 8, num_sms() * 8);
   embed_gather_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
@@ -455,6 +457,8 @@ extern "C" int ymp_colsum(const ymp_colsum_args* a, void* stream) {
 extern "C" int ymp_group_reduce(const ymp_group_args* a, void* stream) {
   YMP_CHECK_ARG(a && a->in && a->out, "ymp_group_reduce: null pointer");
   YMP_CHECK_ARG(a->G > 0 && a->T > 0 && a->C > 0 && a->C % 8 == 0 && a->ld_in % 8 == 0 && a->ld_out % 8 == 0, "ymp_group_reduce: bad shape");
+  YMP_CHECK_ARG(a->ld_in >= a->C && a->ld_out >= a->C, "ymp_group_reduce: bad ld");
+  YMP_CHECK_ARG(aligned16(a->in) && aligned16(a->out), "ymp_group_reduce: 16-byte alignment required");
   const long total = (long)a->G * (a->C / 8) * (a->broadcast ? a->T : 1);
   const int blocks = (int)min((total + 255) / 256, (long)num_sms() * 8);
   if (!a->broadcast)
