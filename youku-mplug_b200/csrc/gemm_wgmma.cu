@@ -69,25 +69,65 @@ __device__ __forceinline__ void st_bf16x4(__nv_bfloat16* p, const float* f) {
   *reinterpret_cast<uint2*>(p) = make_uint2(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]));
 }
 
+// The epilogue's flags are uniform over a launch, but tested per row they are some fifty branches, most of them taken,
+// and with two warps per scheduler nothing hides them: the row loop of a plain bf16 tile took 10 500 cycles, with or
+// without its stores.  So the row loop is compiled once per flag combination the training step launches (KIND >= 0:
+// the flags below are constants and the untaken code is gone) and once with every flag read at run time (EPI_ANY),
+// which serves everything else (dropout, an activation without act', bf16 residual, ...).  Same statements, same
+// order: the results are bit-identical whichever copy runs.
+constexpr int EPI_ANY = -1;
+enum { EPI_AUX_NONE = 0, EPI_AUX_MUL = 1, EPI_AUX_GELU_ERF = 2, EPI_AUX_GELU_TANH = 3 };  // 2, 3: act' stored in aux_out
+enum { EPI_OUT_BF16 = 0, EPI_OUT_F32 = 1, EPI_OUT_ATOMIC = 2 };
+constexpr int epi_kind(int aux, int res_f32, int out) { return aux * 16 + res_f32 * 4 + out; }
+template <int KIND>
+struct EpiFlags {
+  bool aux_in, aux_out, residual, res_f32, out_f32, accumulate;
+  int act;
+  __device__ __forceinline__ explicit EpiFlags(const GemmKParams& p) {
+    if constexpr (KIND == EPI_ANY) {
+      aux_in = p.aux_in != nullptr; aux_out = p.aux_out != nullptr; act = p.act;
+      residual = p.residual != nullptr; res_f32 = p.res_f32 != 0;
+      out_f32 = p.out_f32 != 0; accumulate = p.accumulate != 0;
+    } else {
+      constexpr int aux = KIND / 16, out = KIND % 4;
+      aux_in = aux == EPI_AUX_MUL; aux_out = aux >= EPI_AUX_GELU_ERF;
+      act = aux == EPI_AUX_GELU_ERF ? YMP_ACT_GELU_ERF : aux == EPI_AUX_GELU_TANH ? YMP_ACT_GELU_TANH : YMP_ACT_NONE;
+      residual = res_f32 = (KIND / 4) % 4 != 0;
+      out_f32 = out != EPI_OUT_BF16; accumulate = out == EPI_OUT_ATOMIC;
+    }
+  }
+};
+// The combination of a launch, or EPI_ANY when no specialised copy exists for it.
+__device__ __forceinline__ int epi_kind_of(const GemmKParams& p) {
+  const int aux = p.aux_in ? EPI_AUX_MUL
+                  : (p.act == YMP_ACT_NONE && !p.aux_out) ? EPI_AUX_NONE
+                  : (p.act == YMP_ACT_GELU_ERF && p.aux_out) ? EPI_AUX_GELU_ERF
+                  : (p.act == YMP_ACT_GELU_TANH && p.aux_out) ? EPI_AUX_GELU_TANH : -1;
+  if (aux < 0 || p.has_drop || (p.residual && !p.res_f32)) return EPI_ANY;
+  return epi_kind(aux, p.residual ? 1 : 0, !p.out_f32 ? EPI_OUT_BF16 : p.accumulate ? EPI_OUT_ATOMIC : EPI_OUT_F32);
+}
+
 // Global operands of one row of a thread's two quads, fetched for a group of rows before any of them is stored.
 struct EpiIn {
   uint32_t res[8];  // 8 fp32, or 8 bf16 in the first 4 words
   uint32_t aux[4];  // 8 bf16 (aux_in)
 };
+template <int KIND>
 __device__ __forceinline__ void epilogue_fetch(const GemmKParams& p, int row, const int (&col)[2], bool full, EpiIn& in) {
+  const EpiFlags<KIND> f(p);
   if (row >= p.M || !full) return;
-  if (p.aux_in) {
+  if (f.aux_in) {
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
       const uint2 a = ld_bf16x4(p.aux_in + (size_t)row * p.ldd + col[q]);
       in.aux[2 * q] = a.x; in.aux[2 * q + 1] = a.y;
     }
   }
-  if (p.residual) {
+  if (f.residual) {
     const int rrow = p.res_row_mod ? row % p.res_row_mod : row;
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
-      if (p.res_f32) {
+      if (f.res_f32) {
         const float4 a = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.residual) + (size_t)rrow * p.ldr + col[q]));
         in.res[4 * q] = __float_as_uint(a.x); in.res[4 * q + 1] = __float_as_uint(a.y);
         in.res[4 * q + 2] = __float_as_uint(a.z); in.res[4 * q + 3] = __float_as_uint(a.w);
@@ -100,10 +140,11 @@ __device__ __forceinline__ void epilogue_fetch(const GemmKParams& p, int row, co
 }
 
 // Epilogue of one row of a thread's two quads: v[4q + e] is column col[q] + e.  `full`: both quads lie inside N.
-template <bool DROP>
+template <bool DROP, int KIND>
 __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8], int row, const int (&col)[2], bool full,
                                              const uint32_t (&bias)[4], const EpiIn& in, const DropState& ds) {
   if (row >= p.M) return;
+  const EpiFlags<KIND> f(p);
   const int drow = p.d_row_block ? (row / p.d_row_block) * p.d_row_stride + row % p.d_row_block : row;
   const int rrow = p.res_row_mod ? row % p.res_row_mod : row;
   if (p.alpha != 1.0f) {
@@ -120,11 +161,11 @@ __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8]
     const size_t doff[2] = {(size_t)drow * p.ldd + col[0], (size_t)drow * p.ldd + col[1]};   // D: optionally re-blocked
     // aux_out: with an activation it receives act'(v) (what the backward epilogue multiplies by),
     // without one the value itself.  aux_in: a plain multiplier.  Switches are warp-uniform.
-    if (p.aux_in) {
+    if (f.aux_in) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) { v[2 * i] *= bf16_lo(in.aux[i]); v[2 * i + 1] *= bf16_hi(in.aux[i]); }
-    } else if (p.act == YMP_ACT_GELU_ERF) {
-      if (p.aux_out) {
+    } else if (f.act == YMP_ACT_GELU_ERF) {
+      if (f.aux_out) {
         float x[8], d[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) x[i] = v[i];
@@ -137,8 +178,8 @@ __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8]
         for (int i = 0; i < 8; ++i) x[i] = v[i];
         gelu_erf_x8(x, v);
       }
-    } else if (p.act == YMP_ACT_GELU_TANH) {
-      if (p.aux_out) {
+    } else if (f.act == YMP_ACT_GELU_TANH) {
+      if (f.aux_out) {
         float d[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) v[i] = gelu_tanh_both(v[i], d[i]);
@@ -148,7 +189,7 @@ __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8]
 #pragma unroll
         for (int i = 0; i < 8; ++i) v[i] = gelu_tanh(v[i]);
       }
-    } else if (p.aux_out) {
+    } else if (f.aux_out) {
       st_bf16x4(p.aux_out + off[0], v);
       st_bf16x4(p.aux_out + off[1], v + 4);
     }
@@ -156,8 +197,8 @@ __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8]
 #pragma unroll
       for (int q = 0; q < 2; ++q) drop4(ds, (uint32_t)row, (uint32_t)col[q], v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
     }
-    if (p.residual) {
-      if (p.res_f32) {  // fp32 residual stream
+    if (f.residual) {
+      if (f.res_f32) {  // fp32 residual stream
 #pragma unroll
         for (int i = 0; i < 8; ++i) v[i] += __uint_as_float(in.res[i]);
       } else {
@@ -167,9 +208,9 @@ __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8]
     }
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
-      if (!p.out_f32) {
+      if (!f.out_f32) {
         st_bf16x4(reinterpret_cast<__nv_bfloat16*>(p.D) + doff[q], v + 4 * q);
-      } else if (!p.accumulate) {
+      } else if (!f.accumulate) {
         *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.D) + doff[q]) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
       } else {
         asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(reinterpret_cast<float*>(p.D) + doff[q]),
@@ -186,15 +227,15 @@ __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8]
         float x = v[i];
         if (p.bias) x += __bfloat162float(p.bias[c]);
         const size_t off = (size_t)row * p.ldd + c, doff = (size_t)drow * p.ldd + c;
-        if (p.aux_in) {
+        if (f.aux_in) {
           x *= __bfloat162float(p.aux_in[off]);
-        } else if (p.act == YMP_ACT_GELU_ERF) {
+        } else if (f.act == YMP_ACT_GELU_ERF) {
           float d; x = gelu_erf_both(x, d);
-          if (p.aux_out) p.aux_out[off] = __float2bfloat16(d);
-        } else if (p.act == YMP_ACT_GELU_TANH) {
+          if (f.aux_out) p.aux_out[off] = __float2bfloat16(d);
+        } else if (f.act == YMP_ACT_GELU_TANH) {
           float d; x = gelu_tanh_both(x, d);
-          if (p.aux_out) p.aux_out[off] = __float2bfloat16(d);
-        } else if (p.aux_out) {
+          if (f.aux_out) p.aux_out[off] = __float2bfloat16(d);
+        } else if (f.aux_out) {
           p.aux_out[off] = __float2bfloat16(x);
         }
         if constexpr (DROP) {
@@ -202,11 +243,11 @@ __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8]
           const uint32_t wc = (c & 3) == 0 ? w.x : (c & 3) == 1 ? w.y : (c & 3) == 2 ? w.z : w.w;
           x = wc >= ds.thresh ? x * ds.scale : 0.f;
         }
-        if (p.residual)
-          x += p.res_f32 ? reinterpret_cast<const float*>(p.residual)[(size_t)rrow * p.ldr + c]
+        if (f.residual)
+          x += f.res_f32 ? reinterpret_cast<const float*>(p.residual)[(size_t)rrow * p.ldr + c]
                          : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[(size_t)rrow * p.ldr + c]);
-        if (!p.out_f32) reinterpret_cast<__nv_bfloat16*>(p.D)[doff] = __float2bfloat16(x);
-        else if (!p.accumulate) reinterpret_cast<float*>(p.D)[doff] = x;
+        if (!f.out_f32) reinterpret_cast<__nv_bfloat16*>(p.D)[doff] = __float2bfloat16(x);
+        else if (!f.accumulate) reinterpret_cast<float*>(p.D)[doff] = x;
         else atomicAdd(reinterpret_cast<float*>(p.D) + doff, x);
       }
     }
@@ -239,6 +280,41 @@ __device__ __forceinline__ void load_a_im2col(uint8_t* sa, const CUtensorMap* tm
 // Accumulator fragment of wgmma m64nBN (thread t of a consumer warpgroup): acc[4j + e] holds row 16 (t / 32) + (t % 32) / 4
 // (+8 for e >= 2), column 8 j + 2 (t % 4) + (e & 1) of the warpgroup's 64-row slice.
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// The row loop of the epilogue over the staged tile, for one flag combination (see EpiFlags).
+template <int BN, int KIND>
+__device__ __forceinline__ void epilogue_rows(const GemmKParams& p, const float* stg, int m_blk, int n_blk) {
+  using Cfg = GemmCfg<BN>;
+  using Epi = EpiCfg<BN>;
+  DropState ds;  // only read when has_drop
+  if (KIND == EPI_ANY && p.has_drop) ds = drop_state(p.drop);
+  const int et = threadIdx.x - 128, tj = et % Epi::TPR, tr = et / Epi::TPR;
+  const int col[2] = {n_blk * BN + 4 * tj, n_blk * BN + BN / 2 + 4 * tj};
+  const bool full = col[1] + 4 <= p.N;
+  uint32_t bias[4];
+  if (p.bias && full) {
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const uint2 b = ld_bf16x4(p.bias + col[q]);
+      bias[2 * q] = b.x; bias[2 * q + 1] = b.y;
+    }
+  }
+#pragma unroll 1
+  for (int lr0 = tr; lr0 < BM; lr0 += Epi::RPP * Epi::GROUP) {
+    EpiIn in[Epi::GROUP];
+#pragma unroll
+    for (int u = 0; u < Epi::GROUP; ++u) epilogue_fetch<KIND>(p, m_blk * BM + lr0 + u * Epi::RPP, col, full, in[u]);
+#pragma unroll
+    for (int u = 0; u < Epi::GROUP; ++u) {
+      const int lr = lr0 + u * Epi::RPP;
+      const float4 a = *reinterpret_cast<const float4*>(stg + lr * Cfg::STG_LD + 4 * tj);
+      const float4 b = *reinterpret_cast<const float4*>(stg + lr * Cfg::STG_LD + BN / 2 + 4 * tj);
+      float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+      if (KIND == EPI_ANY && p.has_drop) epilogue_row<true, KIND>(p, v, m_blk * BM + lr, col, full, bias, in[u], ds);
+      else epilogue_row<false, KIND>(p, v, m_blk * BM + lr, col, full, bias, in[u], ds);
+    }
+  }
+}
 
 template <int BN, int AMN, int BMN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -361,34 +437,17 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
     }
   }
   named_sync(1, 256);
-  DropState ds;  // only read when has_drop
-  if (p.has_drop) ds = drop_state(p.drop);
-  using Epi = EpiCfg<BN>;
-  const int et = threadIdx.x - 128, tj = et % Epi::TPR, tr = et / Epi::TPR;
-  const int col[2] = {n_blk * BN + 4 * tj, n_blk * BN + BN / 2 + 4 * tj};
-  const bool full = col[1] + 4 <= p.N;
-  uint32_t bias[4];
-  if (p.bias && full) {
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const uint2 b = ld_bf16x4(p.bias + col[q]);
-      bias[2 * q] = b.x; bias[2 * q + 1] = b.y;
-    }
-  }
-#pragma unroll 1
-  for (int lr0 = tr; lr0 < BM; lr0 += Epi::RPP * Epi::GROUP) {
-    EpiIn in[Epi::GROUP];
-#pragma unroll
-    for (int u = 0; u < Epi::GROUP; ++u) epilogue_fetch(p, m_blk * BM + lr0 + u * Epi::RPP, col, full, in[u]);
-#pragma unroll
-    for (int u = 0; u < Epi::GROUP; ++u) {
-      const int lr = lr0 + u * Epi::RPP;
-      const float4 a = *reinterpret_cast<const float4*>(stg + lr * Cfg::STG_LD + 4 * tj);
-      const float4 b = *reinterpret_cast<const float4*>(stg + lr * Cfg::STG_LD + BN / 2 + 4 * tj);
-      float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-      if (p.has_drop) epilogue_row<true>(p, v, m_blk * BM + lr, col, full, bias, in[u], ds);
-      else epilogue_row<false>(p, v, m_blk * BM + lr, col, full, bias, in[u], ds);
-    }
+  switch (epi_kind_of(p)) {  // uniform over the launch
+#define YMP_EPI_CASE(aux, res, out) \
+    case epi_kind(aux, res, out): epilogue_rows<BN, epi_kind(aux, res, out)>(p, stg, m_blk, n_blk); break;
+    YMP_EPI_CASE(EPI_AUX_NONE, 0, EPI_OUT_BF16)        // qkv, dgrads, LM head
+    YMP_EPI_CASE(EPI_AUX_NONE, 1, EPI_OUT_F32)         // projections onto the fp32 residual stream
+    YMP_EPI_CASE(EPI_AUX_NONE, 0, EPI_OUT_ATOMIC)      // wgrad
+    YMP_EPI_CASE(EPI_AUX_GELU_ERF, 0, EPI_OUT_BF16)    // ViT fc1
+    YMP_EPI_CASE(EPI_AUX_GELU_TANH, 0, EPI_OUT_BF16)   // GPT h->4h
+    YMP_EPI_CASE(EPI_AUX_MUL, 0, EPI_OUT_BF16)         // their dgrads
+#undef YMP_EPI_CASE
+    default: epilogue_rows<BN, EPI_ANY>(p, stg, m_blk, n_blk);
   }
 }
 
