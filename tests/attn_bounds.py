@@ -42,6 +42,11 @@ Backward (the kernels recompute P = exp(S - lse) in fp32 from the given lse).
     dQ      = scale dS K, fp32 accumulation over the keys (u, as above), rounded to bf16:
               E_dQ = C [scale (E_dS |K| + u |dS| |K|) + u |dQ_ref|] + 2^-24
     dK      = the same with dS^T and |Q|.
+
+Dropout on the probabilities (mult M = keep / (1 - p), exact in float64; lse stays that of the undropped P):
+O = (P o M) V, dP = M o (dO V^T), dV = (P o M)^T dO, and delta = rowsum(dO o O) = sum_j P_ij dP_ij still.  The kernels
+scale each kept P_ij by one fp32 product (one more u32, inside the 2^-20 term), so every bound above holds with P o M
+in place of P in (P|V|) and in E_dV, and E_dP multiplied by M.
 """
 import math
 
@@ -103,8 +108,9 @@ def visible(n_seq, s_q, s_kv, mask, mask_block=0, total_rows=0, kv_count=None):
 
 
 # ---------------------------------------------------------------------------------- reference
-def reference(q, k, v, vis, scale, dout=None):
-    """Explicit-formula float64 attention.  q [n,H,sq,hd], k/v [n,H,skv,hd], vis [n,sq,skv] bool, dout like q.
+def reference(q, k, v, vis, scale, dout=None, mult=None):
+    """Explicit-formula float64 attention.  q [n,H,sq,hd], k/v [n,H,skv,hd], vis [n,sq,skv] bool, dout like q, mult
+    [n,H,sq,skv] the dropout multiplier keep / (1 - p) or None.
     Returns a dict with O, lse, P, S (scaled scores, 0 where masked) and, with dout, dP, delta, dS, dQ, dK, dV.
     Rows that see no key get O = 0, lse = -inf, P = 0."""
     q, k, v = q.double(), k.double(), v.double()
@@ -113,14 +119,17 @@ def reference(q, k, v, vis, scale, dout=None):
     Sm = S.masked_fill(~vm, -math.inf)
     lse = torch.logsumexp(Sm, -1)
     P = torch.exp(Sm - lse[..., None]).nan_to_num(0.0)
-    r = dict(S=S.masked_fill(~vm, 0.0), P=P, O=P @ v, lse=lse, vis=vm)
+    Pm = P if mult is None else P * mult.double()
+    r = dict(S=S.masked_fill(~vm, 0.0), P=P, Pm=Pm, mult=mult, O=Pm @ v, lse=lse, vis=vm)
     if dout is not None:
         do = dout.double()
         dP = do @ v.transpose(-1, -2)
+        if mult is not None:
+            dP = dP * mult.double()
         delta = (do * r["O"]).sum(-1)
         dS = P * (dP - delta[..., None])
         r.update(dP=dP, delta=delta, dS=dS, dQ=scale * dS @ k, dK=scale * dS.transpose(-1, -2) @ q,
-                 dV=P.transpose(-1, -2) @ do)
+                 dV=Pm.transpose(-1, -2) @ do)
     return r
 
 
@@ -134,7 +143,7 @@ def fwd_bounds(q, k, v, scale, ref):
     vm = ref["vis"]
     ds = _score_err(q, k, scale, vm)
     ds_i = ds.amax(-1)
-    pv = ref["P"] @ v.double().abs()
+    pv = ref.get("Pm", ref["P"]) @ v.double().abs()
     e_o = C * ((2 * U + 2 * ds_i[..., None] + EXP) * pv + U * ref["O"].abs()) + TINY
     n_i = vm.sum(-1).double()
     s_max = ref["S"].abs().amax(-1)
@@ -152,8 +161,10 @@ def bwd_bounds(q, k, v, dout, scale, ref, e_o=None, e_lse=None):
     eP = (_score_err(q, k, scale, vm) + EXP * (1 + lse.abs()[..., None] + ref["S"].abs())) * vm
     if e_lse is not None:
         eP = eP + e_lse.masked_fill(~vm.any(-1), 0.0)[..., None] * vm
-    e_dv = C * ((((2 * U + eP) * P).transpose(-1, -2) @ do.abs()) + U * ref["dV"].abs()) + TINY
+    e_dv = C * ((((2 * U + eP) * ref.get("Pm", P)).transpose(-1, -2) @ do.abs()) + U * ref["dV"].abs()) + TINY
     e_dp = hd * G32 * (do.abs() @ v.abs().transpose(-1, -2))
+    if ref.get("mult") is not None:
+        e_dp = e_dp * ref["mult"].double()
     dP, delta = ref["dP"], ref["delta"]
     n_i = vm.sum(-1).double()
     pdp = (P * dP.abs()).sum(-1)
@@ -174,7 +185,7 @@ def _bf16(x):
     return x.to(torch.bfloat16).float()
 
 
-def simulate_fwd(q, k, v, vis, scale, defect=None):
+def simulate_fwd(q, k, v, vis, scale, defect=None, mult=None):
     """The forward kernels' arithmetic in fp32: raw scores accumulated in fp32, the scale folded into the exponent
     (exp2 of s * scale * log2e - m * scale * log2e), P rounded to bf16 before P V, the normaliser summed from the
     fp32 P, O rounded to bf16, lse = m * scale + log(l).
@@ -193,17 +204,19 @@ def simulate_fwd(q, k, v, vis, scale, defect=None):
     ms = torch.where(torch.isinf(m), torch.zeros_like(m), m * sl2)
     p = torch.exp2(s * sl2 - ms)
     l = p.sum(-1, keepdim=True)
-    o = _bf16((_bf16(p) @ v) / torch.where(l > 0, l, torch.ones_like(l)))
+    pd = p if mult is None else p * mult.float()          # dropout: each kept probability scaled by 1 / (1 - p)
+    o = _bf16((_bf16(pd) @ v) / torch.where(l > 0, l, torch.ones_like(l)))
     lse = (m * torch.tensor(scale, dtype=torch.float32) + torch.log(l)).squeeze(-1)
     if defect == "lse_shift":
         lse = lse + math.log(2) / 64
     return o, lse
 
 
-def simulate_bwd(q, k, v, o, lse, dout, vis, scale):
+def simulate_bwd(q, k, v, o, lse, dout, vis, scale, mult=None):
     """The tensor-core backward's arithmetic in fp32 from the given bf16 O and fp32 lse: P = exp2(s * scale * log2e -
     lse * log2e), dP = dO V^T, delta = rowsum(dO o O), dS = P o (dP - delta) rounded to bf16, dQ = scale dS K,
-    dK = scale dS^T Q, dV = bf16(P)^T dO, each rounded to bf16."""
+    dK = scale dS^T Q, dV = bf16(P)^T dO, each rounded to bf16.  With a dropout multiplier M, dP is M o dO V^T and
+    dV = bf16(P o M)^T dO."""
     q, k, v, o, do = q.float(), k.float(), v.float(), o.float(), dout.float()
     vm = vis[:, None]
     sl2 = torch.tensor(scale * 1.4426950408889634, dtype=torch.float32)
@@ -211,12 +224,15 @@ def simulate_bwd(q, k, v, o, lse, dout, vis, scale):
     s = (q @ k.transpose(-1, -2)).masked_fill(~vm, -math.inf)
     p = torch.exp2(s * sl2 - lse2[..., None])
     dp = do @ v.transpose(-1, -2)
+    pd = p
+    if mult is not None:
+        dp, pd = dp * mult.float(), p * mult.float()
     delta = (do * o).sum(-1, keepdim=True)
     ds = _bf16(p * (dp - delta))
     sc = torch.tensor(scale, dtype=torch.float32)
     dq = _bf16((ds @ k) * sc)
     dk = _bf16((ds.transpose(-1, -2) @ q) * sc)
-    dv = _bf16(_bf16(p).transpose(-1, -2) @ do)
+    dv = _bf16(_bf16(pd).transpose(-1, -2) @ do)
     return dq, dk, dv
 
 

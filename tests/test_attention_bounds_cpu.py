@@ -137,3 +137,41 @@ def test_geometric_values_expose_a_late_causal_leak():
     assert AB.worst_ratio(o_ok, ref["O"], e_o) <= 1
     late = (torch.arange(S) >= 64)[None, None, :, None]
     assert AB.worst_ratio(o, ref["O"], e_o, late) > 1
+
+
+def _mult(n, H, sq, skv, p, seed):
+    g = torch.Generator().manual_seed(seed)
+    keep = torch.rand(n, H, sq, skv, generator=g) >= p
+    return keep.double() * float(torch.tensor(1.0 / (1.0 - p), dtype=torch.float32))
+
+
+@pytest.mark.parametrize("mask,sq,skv", [(AB.MASK_CAUSAL, 70, 70), (AB.MASK_NONE, 33, 97)])
+@pytest.mark.parametrize("p", [0.1, 0.5])
+def test_dropout_simulation_inside_bounds(mask, sq, skv, p):
+    """Dropout on the probabilities (O = (P o M) V, lse of the undropped P): the simulated kernel arithmetic with a
+    keep mask stays inside the forward and backward bounds taken with the same multiplier, isolated and chained."""
+    hd, n, H = 32, 2, 2
+    q, k, v, do = _inputs(n, sq, skv, hd=hd, seed=4)
+    scale = hd ** -0.5
+    vis = AB.visible(n, sq, skv, mask)
+    m = _mult(n, H, sq, skv, p, 5)
+    ref = AB.reference(q, k, v, vis, scale, do, mult=m)
+    e_o, e_lse = AB.fwd_bounds(q, k, v, scale, ref)
+    o, lse = AB.simulate_fwd(q, k, v, vis, scale, mult=m)
+    assert AB.worst_ratio(o, ref["O"], e_o) <= 1 and AB.worst_ratio(lse, ref["lse"], e_lse) <= 1
+    for o_in, l_in, e in ((_bf(ref["O"]), ref["lse"].float(), (None, None)), (o, lse, (e_o, e_lse))):
+        dq, dk, dv = AB.simulate_bwd(q, k, v, o_in, l_in, do, vis, scale, mult=m)
+        e_dq, e_dk, e_dv = AB.bwd_bounds(q, k, v, do, scale, ref, *e)
+        for got, want, b in ((dq, ref["dQ"], e_dq), (dk, ref["dK"], e_dk), (dv, ref["dV"], e_dv)):
+            assert AB.worst_ratio(got, want, b) <= 1
+
+
+def test_dropout_wrong_mask_exceeds_bounds():
+    """The forward with another draw of the same keep probability is far outside the bounds of the right mask."""
+    hd, n, H, sq = 32, 2, 2, 70
+    q, k, v, do = _inputs(n, sq, sq, hd=hd, seed=4)
+    vis = AB.visible(n, sq, sq, AB.MASK_CAUSAL)
+    ref = AB.reference(q, k, v, vis, hd ** -0.5, do, mult=_mult(n, H, sq, sq, 0.1, 5))
+    e_o, _ = AB.fwd_bounds(q, k, v, hd ** -0.5, ref)
+    o, _ = AB.simulate_fwd(q, k, v, vis, hd ** -0.5, mult=_mult(n, H, sq, sq, 0.1, 6))
+    assert AB.worst_ratio(o, ref["O"], e_o) > 1
