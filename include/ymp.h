@@ -132,6 +132,9 @@ typedef struct ymp_gemm_args {
 } ymp_gemm_args;
 
 int ymp_gemm(const ymp_gemm_args* a, void* stream);
+/* ymp_gemm with the tile height chosen by the caller: tile_m = 0 (auto: what ymp_gemm does), 128 or 192.  192-row tiles
+ * need the 256-column tile (tile_n = 0, 256 or 512) and no fused im2col operand; other combinations are rejected. */
+int ymp_gemm_tiled(const ymp_gemm_args* a, int tile_m, void* stream);
 
 /* Skinny GEMM for single-token decoding (KV-cache steps of sample() / beam_search(),
  * models/modeling_distributed_gpt3.py:1620-1886): y[M, N] = epilogue(x[M, K] . w[N, K]^T).  One pass over the weights on

@@ -4,9 +4,9 @@
 
 The distinct launches (shape, operand layouts, epilogue flags) come from `bench.py --gemm-report` of each config:
 DIR/gemm_<config>.json is read when it exists, otherwise bench.py is run once (1 step) to write it.  Every launch is
-then rebuilt on seeded random operands and timed through `ops.gemm` with CUDA events, once per `tile_n` value in
---arms (the arms alternate, three rounds each) and once as `torch.matmul` on the same bf16 operands (cuBLAS, a
-reference for what a plain GEMM of that shape reaches on the card).  Operands and outputs are allocated once per
+then rebuilt on seeded random operands and timed through `ops.gemm` with CUDA events, once per arm in --arms (an arm
+is `tile_n` or `tile_n:tile_m`, e.g. `0,256:128,256:192`; the arms alternate, three rounds each) and once as
+`torch.matmul` on the same bf16 operands (cuBLAS, a reference for what a plain GEMM of that shape reaches on the card).  Operands and outputs are allocated once per
 launch, so a timed window is the kernel alone.
 
 Not reproduced from the report (it does not record them): bias, row-mod residual broadcast, row re-blocking of D,
@@ -94,7 +94,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", nargs="+", default=["pretrain", "caption27b", "retrieval"])
     ap.add_argument("--reports-dir", default=None, help="where gemm_<config>.json live (written by bench.py if missing)")
-    ap.add_argument("--arms", default="0", help="comma-separated tile_n values timed alternately through ops.gemm")
+    ap.add_argument("--arms", default="0", help="comma-separated tile_n or tile_n:tile_m arms timed alternately")
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--window-ms", type=float, default=20.0, help="target length of one timed window")
     ap.add_argument("--root", default=HERE, help="repository tree whose ymp package is imported")
@@ -108,19 +108,20 @@ def main():
     from ymp import ops
     if not torch.cuda.is_available():
         sys.exit("gemm_ab.py needs a GPU")
-    arms = [int(x) for x in args.arms.split(",")]
+    arms = args.arms.split(",")
+    tiles = {arm: dict(tile_n=int(arm.split(":")[0]), tile_m=int(arm.split(":")[1]) if ":" in arm else 0) for arm in arms}
     rdir = args.reports_dir or tempfile.mkdtemp(prefix="gemm_ab_")
     os.makedirs(rdir, exist_ok=True)
     info = card_info()
     print(f"# {info['name']}, power limit {info['power_limit']}, max SM clock {info['max_sm_clock']}; "
-          f"ymp from {root}; arms tile_n={arms}", flush=True)
+          f"ymp from {root}; arms tile_n[:tile_m]={arms}", flush=True)
 
     result = dict(card=info, root=root, arms=arms, configs={})
     for cfg in args.configs:
         rows = load_report(root, cfg, rdir)
         print(f"\n## {cfg}: {len(rows)} distinct launches, {sum(r['n'] for r in rows)} per step")
         hdr = "   M     N     K at bt acc act ax ai res r32 o32   n  step_us " + \
-              " ".join(f"  t{a:<3}us   TF/s" for a in arms) + "  cublas_us   TF/s  same"
+              " ".join(f" {a:>8}us   TF/s" for a in arms) + "  cublas_us   TF/s  same"
         print(hdr)
         out_rows = []
         tot = {a: 0.0 for a in arms}
@@ -129,7 +130,7 @@ def main():
             a, b, kw = build_case(row, 1000 + i)
             flop = 2.0 * row["M"] * row["N"] * row["K"]
             reps = max(5, min(500, int(args.window_ms * 1e-3 / (flop / 4e14 + 4e-6))))
-            fns = {arm: (lambda arm=arm: ops.gemm(a, b, tile_n=arm, **kw)) for arm in arms}
+            fns = {arm: (lambda arm=arm: ops.gemm(a, b, **tiles[arm], **kw)) for arm in arms}
             am = a.t() if row["a_t"] else a
             bm = b if row["b_t"] else b.t()
             cb_out = torch.empty(row["M"], row["N"], device=a.device, dtype=torch.bfloat16)
@@ -144,7 +145,7 @@ def main():
                 outs = {}
                 for arm in arms:
                     kw["out"].zero_()
-                    ops.gemm(a, b, tile_n=arm, **kw)
+                    ops.gemm(a, b, **tiles[arm], **kw)
                     outs[arm] = kw["out"].clone()
                     fps[arm] = fingerprint(outs[arm])
                 same = all(torch.equal(outs[arms[0]], outs[x]) for x in arms[1:])
@@ -155,7 +156,7 @@ def main():
             print(f"{row['M']:5d} {row['N']:5d} {row['K']:5d} {row['a_t']:2d} {row['b_t']:2d} {row['acc']:3d} {row['act']:3d} "
                   f"{row['aux_out']:2d} {row['aux_in']:2d} {row['res']:3d} {row['res_f32']:3d} {row['out_f32']:3d} "
                   f"{row['n']:3d} {row['ms'] * 1e3 / row['n']:8.1f} "
-                  + " ".join(f"{us[arm]:8.1f} {flop / us[arm] / 1e6:6.1f}" for arm in arms)
+                  + " ".join(f"{us[arm]:10.1f} {flop / us[arm] / 1e6:6.1f}" for arm in arms)
                   + f" {us['cublas']:10.1f} {flop / us['cublas'] / 1e6:6.1f}  {'-' if same is None else 'yes' if same else 'NO'}",
                   flush=True)
             out_rows.append(dict(row, step_us=row["ms"] * 1e3 / row["n"], us={str(k): v for k, v in us.items()},
@@ -165,7 +166,7 @@ def main():
             del a, b, kw, cb_out, fns
             torch.cuda.empty_cache()
         print(f"# {cfg}: sum over one step's launches (ms): "
-              + ", ".join(f"tile_n={a}: {tot[a] / 1e3:.2f}" for a in arms) + f", cuBLAS: {tot_cb / 1e3:.2f}")
+              + ", ".join(f"{a}: {tot[a] / 1e3:.2f}" for a in arms) + f", cuBLAS: {tot_cb / 1e3:.2f}")
         result["configs"][cfg] = dict(rows=out_rows, step_ms={str(a): tot[a] / 1e3 for a in arms}, cublas_step_ms=tot_cb / 1e3)
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)

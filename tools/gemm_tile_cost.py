@@ -1,12 +1,14 @@
 """Fixed cost per output tile of the wgmma GEMM: µs per wave = k_blocks x t + f, fitted per launch class.
 
-    python tools/gemm_tile_cost.py [--root TREE [TREE ...]] [--rounds 3] [--json OUT]
+    python tools/gemm_tile_cost.py [--root TREE [TREE ...]] [--tile-n 256 [128]] [--tile-m 128 [192]] [--rounds 3]
+                                   [--json OUT]
 
-A launch runs ceil(units / SMs) waves of 128 x 256 tiles, one CTA per SM.  For each launch class (M, N, operand
+A launch runs ceil(units / SMs) waves of tile_m x tile_n tiles, one CTA per SM.  For each launch class (M, N, operand
 layouts and epilogue of a launch of the training step, DESIGN.md §5) `ops.gemm` is timed at K = 64, 256, 768, 2048 and
 8192 (1 to 128 k-blocks of 64), warm, with CUDA events over enough repeats for at least 0.2 s per point, and
-time / waves is fitted by least squares to k_blocks x t + f: t is the cost of one k-block of MMAs, f what a tile costs
-whatever its K (pipeline fill, epilogue, turnover between tiles).  The classes:
+time / waves is fitted by least squares to k_blocks x t + f: t is the cost of one tile's k-block of MMAs, f what a tile
+costs whatever its K (pipeline fill, epilogue, turnover between tiles).  Every tile shape of --tile-n x --tile-m (192
+rows only with 256 columns) is an arm; the arms alternate at every point.  The classes:
 
     the ViT's fc1 (GELU, act' stored), its dgrad (B MN-major, x act'), qkv (plain bf16), proj / fc2 (fp32 residual; one
     class, they differ in K only), GPT h->4h (GELU, act' stored), 4h->h (fp32 residual), its dgrad (B MN-major), the LM
@@ -29,7 +31,7 @@ sys.path.insert(0, os.path.join(HERE, "tools"))
 from gemm_ab import card_info, time_fn  # noqa: E402
 
 KS = (64, 256, 768, 2048, 8192)
-BM, BN, BK = 128, 256, 64
+BK = 64
 # name, M, N, a_t, b_t, epilogue
 CLASSES = [
     ("vit fc1: GELU, act' stored", 50208, 3072, 0, 0, "gelu_aux"),
@@ -44,8 +46,8 @@ CLASSES = [
 ]
 
 
-def waves(M, N, sms):
-    return -(-(-(-M // BM) * -(-N // BN)) // sms)
+def waves(M, N, sms, bm, bn):
+    return -(-(-(-M // bm) * -(-N // bn)) // sms)
 
 
 def fit(kbs, ys):
@@ -57,7 +59,7 @@ def fit(kbs, ys):
     return t, f, math.sqrt(sum((y - (x * t + f)) ** 2 for x, y in zip(kbs, ys)) / n)
 
 
-def worker(root, out_path, min_s):
+def worker(root, out_path, min_s, arms):
     for p in (root, os.path.join(root, "youku-mplug_b200")):
         sys.path.insert(0, p)
     import torch
@@ -69,12 +71,12 @@ def worker(root, out_path, min_s):
     g = torch.Generator(device=dev).manual_seed(5)
     res = []
     for name, M, N, a_t, b_t, epi in CLASSES:
-        us = []
+        us = {arm: [] for arm in arms}
         for K in KS:
             rnd = lambda *s: (torch.randn(*s, device=dev, generator=g) / K ** 0.25).to(torch.bfloat16)  # noqa: E731
             a = rnd(K, M) if a_t else rnd(M, K)
             b = rnd(K, N) if b_t else rnd(N, K)
-            kw = dict(a_t=bool(a_t), b_t=bool(b_t), tile_n=256)
+            kw = dict(a_t=bool(a_t), b_t=bool(b_t))
             f32 = epi in ("res32", "acc")
             kw["out"] = torch.zeros(M, N, device=dev, dtype=torch.float32 if f32 else torch.bfloat16)
             if epi == "gelu_aux":
@@ -85,12 +87,14 @@ def worker(root, out_path, min_s):
                 kw["residual"] = torch.randn(M, N, device=dev, generator=g)
             elif epi == "acc":
                 kw.update(accumulate=True, split_k=1)
-            fn = lambda: ops.gemm(a, b, **kw)  # noqa: E731
-            est = time_fn(fn, 3) * 1e-6
-            us.append(time_fn(fn, max(5, int(min_s / est) + 1)))
+            for bm, bn in arms:
+                fn = lambda: ops.gemm(a, b, tile_m=bm, tile_n=bn, **kw)  # noqa: E731
+                est = time_fn(fn, 3) * 1e-6
+                us[(bm, bn)].append(time_fn(fn, max(5, int(min_s / est) + 1)))
             del a, b, kw, fn
             torch.cuda.empty_cache()
-        res.append(dict(name=name, M=M, N=N, waves=waves(M, N, sms), us=us))
+        res.append(dict(name=name, M=M, N=N, arms={f"{bm}x{bn}": dict(waves=waves(M, N, sms, bm, bn), us=us[(bm, bn)])
+                                                  for bm, bn in arms}))
     with open(out_path, "w") as fh:
         json.dump(dict(root=root, sms=sms, classes=res), fh)
 
@@ -98,13 +102,16 @@ def worker(root, out_path, min_s):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--root", nargs="+", default=[HERE], help="built repository trees to measure, alternated")
+    ap.add_argument("--tile-n", type=int, nargs="+", default=[256], choices=(128, 256))
+    ap.add_argument("--tile-m", type=int, nargs="+", default=[128], choices=(128, 192))
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--min-seconds", type=float, default=0.2, help="timed window per (class, K) point")
     ap.add_argument("--json", default=None, help="also write the samples and fits as json")
     ap.add_argument("--worker", default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
+    arms = [(bm, bn) for bn in args.tile_n for bm in args.tile_m if bm == 128 or bn == 256]
     if args.worker:
-        return worker(os.path.abspath(args.root[0]), args.worker, args.min_seconds)
+        return worker(os.path.abspath(args.root[0]), args.worker, args.min_seconds, arms)
 
     import tempfile
     import torch
@@ -118,7 +125,8 @@ def main():
             for r in roots:
                 out = os.path.join(td, f"r{rnd}.json")
                 subprocess.run([sys.executable, os.path.abspath(__file__), "--worker", out, "--root", r,
-                                "--min-seconds", str(args.min_seconds)], check=True)
+                                "--min-seconds", str(args.min_seconds), "--tile-n", *map(str, args.tile_n),
+                                "--tile-m", *map(str, args.tile_m)], check=True)
                 with open(out) as fh:
                     samples[r].append(json.load(fh))
     print(f"# {info['name']}, power limit {info['power_limit']}, max SM clock {info['max_sm_clock']}; "
@@ -127,15 +135,20 @@ def main():
     result = dict(card=info, ks=KS, roots={})
     for r in roots:
         print(f"\n## {r}")
-        print(f"{'class':40s} {'M':>6s} {'N':>6s} waves " + " ".join(f"K={K:<5d}us" for K in KS) + "   t_us    f_us  resid_us")
+        print(f"{'class':40s} {'M':>6s} {'N':>6s} tile    waves " + " ".join(f"K={K:<5d}us" for K in KS)
+              + "   t_us    f_us  resid_us")
         rows = []
         for i, (name, M, N, *_rest) in enumerate(CLASSES):
-            w = samples[r][0]["classes"][i]["waves"]
-            us = [statistics.median(s["classes"][i]["us"][j] for s in samples[r]) for j in range(len(KS))]
-            t, f, resid = fit(kbs, [u / w for u in us])
-            print(f"{name:40s} {M:6d} {N:6d} {w:5d} " + " ".join(f"{u:9.1f}" for u in us) + f" {t:6.3f} {f:7.2f} {resid:9.2f}")
-            rows.append(dict(name=name, M=M, N=N, waves=w, us=us, t_us=t, f_us=f, resid_us=resid,
-                             samples_us=[s["classes"][i]["us"] for s in samples[r]]))
+            for bm, bn in arms:
+                arm = f"{bm}x{bn}"
+                got = [s["classes"][i]["arms"][arm] for s in samples[r]]
+                w = got[0]["waves"]
+                us = [statistics.median(g["us"][j] for g in got) for j in range(len(KS))]
+                t, f, resid = fit(kbs, [u / w for u in us])
+                print(f"{name:40s} {M:6d} {N:6d} {arm:7s} {w:5d} " + " ".join(f"{u:9.1f}" for u in us)
+                      + f" {t:6.3f} {f:7.2f} {resid:9.2f}")
+                rows.append(dict(name=name, M=M, N=N, tile=arm, waves=w, us=us, t_us=t, f_us=f, resid_us=resid,
+                                 samples_us=[g["us"] for g in got]))
         result["roots"][r] = rows
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)

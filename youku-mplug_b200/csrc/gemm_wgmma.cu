@@ -1,11 +1,13 @@
-// Warp-specialised bf16 GEMM for sm_90a (one 128 x BN output tile per CTA, BN = 128 or 256).
-//   warpgroup 0   : TMA producer   (cp.async.bulk.tensor 2D / 5D, SWIZZLE_128B, NSTAGE-deep mbarrier ring)
-//   warpgroups 1-2: consumers      (wgmma.mma_async m64 x BN x 16 each, fp32 accumulators in registers), then the
+// Warp-specialised bf16 GEMM for sm_90a (one BM x BN output tile per CTA: 128 x 128, 128 x 256 or 192 x 256).
+//   warpgroup 0      : TMA producer (cp.async.bulk.tensor 2D / 5D, SWIZZLE_128B, NSTAGE-deep mbarrier ring)
+//   warpgroups 1-BM/64: consumers   (wgmma.mma_async m64 x BN x 16 each, fp32 accumulators in registers), then the
 //                   epilogue: accumulators staged through shared memory -> each warp along one row, two 4-column quads a thread ->
 //                   bias / GELU / GELU' / dropout / residual -> bf16 | fp32 | atomic fp32
 // Operands may be K-major or MN-major (the transpose bits of wgmma), so the same kernel serves forward (x.W^T),
 // dgrad (dy.W) and wgrad (dy^T.x, split-K with fp32 atomics).
 #include <cuda.h>
+
+#include <algorithm>
 
 #include "common.h"
 #include "philox.cuh"
@@ -14,11 +16,9 @@
 
 namespace ymp {
 
-constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle row
 constexpr int WGMMA_K = 16;
-constexpr int GEMM_THREADS = 3 * 128;
-constexpr int A_STAGE_BYTES = BM * BK * 2;
+constexpr int SMEM_OPTIN_MAX = 232448;  // dynamic shared memory a CTA may opt in to on sm_90
 
 struct GemmKParams {
   void* D;
@@ -41,24 +41,37 @@ struct GemmKParams {
   int has_drop;
 };
 
-template <int BN>
+// BM = 192 exists for BN = 256 only: it brings (192 + 256) operand bytes per 192 x 256 k-block product against
+// (128 + 256) per 128 x 256, 22 % fewer L2 bytes per FLOP, and its epilogue runs on 384 threads instead of 256.  It has
+// no producer warpgroup: ptxas compiles every instruction within the register count the launch bounds leave (128 at
+// 512 threads, whatever setmaxnreg does at run time), and one m64n256 wgmma alone needs 154.  So its three consumer
+// warpgroups are the whole CTA (384 threads, 168 registers, as for BM = 128), and thread 0 refills the ring.
+template <int BM, int BN>
 struct GemmCfg {
-  static constexpr int NSTAGE = (BN == 256) ? 4 : 6;    // 192 KB operand ring either way
+  static_assert((BM == 128 && (BN == 128 || BN == 256)) || (BM == 192 && BN == 256), "tile shapes");
+  static constexpr int CONSUMERS = BM / 64;             // consumer warpgroups, 64 rows each
+  static constexpr bool PRODUCER_WG = CONSUMERS == 2;   // warpgroup 0 is a TMA producer
+  static constexpr int THREADS = 128 * (CONSUMERS + PRODUCER_WG);
+  static constexpr int FIRST_CONSUMER = THREADS - 128 * CONSUMERS;
+  static constexpr int NSTAGE = (BN == 256) ? 4 : 6;    // 192 KB operand ring for BM = 128, 224 KB for 192
+  static constexpr int A_STAGE_BYTES = BM * BK * 2;
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int STG_LD = BN + 4;                 // fp32 staging row (+4: conflict-free row-per-thread reads)
   static_assert(BM * STG_LD * 4 <= NSTAGE * STAGE_BYTES, "epilogue staging reuses the operand ring");
   static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + 256 + 1024;
+  static_assert(SMEM_BYTES <= SMEM_OPTIN_MAX, "ring, barriers and alignment pad fit the opt-in shared memory");
 };
 
 // Epilogue thread layout: the threads of a warp cover consecutive columns of one output row (two rows for BN = 128), so
 // every global access of the epilogue is coalesced along the row and every staging read is a contiguous run of shared
 // memory.  A thread owns two 4-column quads of the tile, columns 4j .. 4j+3 and BN/2 + 4j .. +3, in every RPP-th row;
 // its bias is loaded once.
-template <int BN>
+template <int BM, int BN>
 struct EpiCfg {
+  static constexpr int THREADS = 2 * BM;    // the consumer warpgroups
   static constexpr int TPR = BN / 8;        // threads per row
-  static constexpr int RPP = 256 / TPR;     // rows per pass of the 256 epilogue threads
+  static constexpr int RPP = THREADS / TPR; // rows per pass of the epilogue threads
   static constexpr int GROUP = 4;           // rows whose global operands are fetched together
   static_assert(BM % (RPP * GROUP) == 0, "row groups tile BM");
 };
@@ -261,12 +274,14 @@ __device__ __forceinline__ void epilogue_row(const GemmKParams& p, float (&v)[8]
 // SWIZZLE_32B is exactly T/8 shared-memory atoms of 8 rows x 32 bytes, dense (a 128-byte-swizzled box would give every
 // 32-byte line its own 128-byte row).  Each sub-tile is the A operand of one wgmma K-step
 // (K = 16) through a SWIZZLE_32B descriptor; rows past the last sample are out of range and arrive as zeros.
-constexpr int IM2COL_SUB_BYTES = BM * 32;  // one 128-row x 16-column sub-tile
+// Only the 128-row tiles take it.
+constexpr int IM2COL_BM = 128;
+constexpr int IM2COL_SUB_BYTES = IM2COL_BM * 32;  // one 128-row x 16-column sub-tile
 __device__ __forceinline__ void load_a_im2col(uint8_t* sa, const CUtensorMap* tma, uint64_t* bar, int m0, int kb,
                                               const GemmKParams& p) {
   const int T = p.im2col_T, c = kb >> 2, y0 = (kb & 3) * 4;
   const int pt = m0 / T;  // first patch (global index b*N + n) of the tile
-  for (int i = 0; i < BM / T; ++i) {
+  for (int i = 0; i < IM2COL_BM / T; ++i) {
     const int g = pt + i, b = g / p.im2col_N, n = g - b * p.im2col_N;
     const int ny = n / p.im2col_Wp, nx = n - ny * p.im2col_Wp;
 #pragma unroll
@@ -282,13 +297,13 @@ __device__ __forceinline__ void load_a_im2col(uint8_t* sa, const CUtensorMap* tm
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // The row loop of the epilogue over the staged tile, for one flag combination (see EpiFlags).
-template <int BN, int KIND>
+template <int BM, int BN, int KIND>
 __device__ __forceinline__ void epilogue_rows(const GemmKParams& p, const float* stg, int m_blk, int n_blk) {
-  using Cfg = GemmCfg<BN>;
-  using Epi = EpiCfg<BN>;
+  using Cfg = GemmCfg<BM, BN>;
+  using Epi = EpiCfg<BM, BN>;
   DropState ds;  // only read when has_drop
   if (KIND == EPI_ANY && p.has_drop) ds = drop_state(p.drop);
-  const int et = threadIdx.x - 128, tj = et % Epi::TPR, tr = et / Epi::TPR;
+  const int et = threadIdx.x - Cfg::FIRST_CONSUMER, tj = et % Epi::TPR, tr = et / Epi::TPR;
   const int col[2] = {n_blk * BN + 4 * tj, n_blk * BN + BN / 2 + 4 * tj};
   const bool full = col[1] + 4 <= p.N;
   uint32_t bias[4];
@@ -316,12 +331,14 @@ __device__ __forceinline__ void epilogue_rows(const GemmKParams& p, const float*
   }
 }
 
-template <int BN, int AMN, int BMN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+template <int BM, int BN, int AMN, int BMN>
+__global__ void __launch_bounds__(GemmCfg<BM, BN>::THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                        const GemmKParams p) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BM, BN>;
   constexpr int NSTAGE = Cfg::NSTAGE;
+  constexpr int A_STAGE_BYTES = Cfg::A_STAGE_BYTES;
+  constexpr bool IM2COL = BM == IM2COL_BM;  // the fused im2col operand can occur (p.im2col_T decides)
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment in the shared address space
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -347,46 +364,56 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
     tma_prefetch_desc(&tma_b);
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[i], Cfg::CONSUMERS);  // one arrival per consumer warpgroup
     }
     fence_mbar_init();
   }
   __syncthreads();
 
-  if (wg == 0) {
-    // ===================================================================== TMA producer
-    if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-        uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
-        uint8_t* sb = smem_b + stage * Cfg::B_STAGE_BYTES;
-        if (p.im2col_T) {
-          load_a_im2col(sa, &tma_a, &full_bar[stage], m_blk * BM, kb, p);
-        } else if (!AMN) {
-          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * BK, m_blk * BM);
-        } else {
+  // k-block kb into ring slot `stage`, completion on its full barrier
+  auto load_stage = [&](int kb, int stage) {
+    mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+    uint8_t* sa = smem_a + stage * A_STAGE_BYTES;
+    uint8_t* sb = smem_b + stage * Cfg::B_STAGE_BYTES;
+    if (IM2COL && p.im2col_T) {
+      load_a_im2col(sa, &tma_a, &full_bar[stage], m_blk * BM, kb, p);
+    } else if (!AMN) {
+      tma_load_2d(sa, &tma_a, &full_bar[stage], kb * BK, m_blk * BM);
+    } else {
 #pragma unroll
-          for (int c = 0; c < BM / 64; ++c)
-            tma_load_2d(sa + c * (64 * BK * 2), &tma_a, &full_bar[stage], m_blk * BM + c * 64, kb * BK);
-        }
-        if (!BMN) {
-          tma_load_2d(sb, &tma_b, &full_bar[stage], kb * BK, n_blk * BN);
-        } else {
-#pragma unroll
-          for (int c = 0; c < BN / 64; ++c)
-            tma_load_2d(sb + c * (64 * BK * 2), &tma_b, &full_bar[stage], n_blk * BN + c * 64, kb * BK);
-        }
-        if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-      }
+      for (int c = 0; c < BM / 64; ++c)
+        tma_load_2d(sa + c * (64 * BK * 2), &tma_a, &full_bar[stage], m_blk * BM + c * 64, kb * BK);
     }
-    return;
+    if (!BMN) {
+      tma_load_2d(sb, &tma_b, &full_bar[stage], kb * BK, n_blk * BN);
+    } else {
+#pragma unroll
+      for (int c = 0; c < BN / 64; ++c)
+        tma_load_2d(sb + c * (64 * BK * 2), &tma_b, &full_bar[stage], n_blk * BN + c * 64, kb * BK);
+    }
+  };
+
+  if constexpr (Cfg::PRODUCER_WG) {
+    if (wg == 0) {
+      // =================================================================== TMA producer
+      if (threadIdx.x == 0) {
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          load_stage(kb, stage);
+          if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+        }
+      }
+      return;
+    }
+  } else if (threadIdx.x == 0) {
+    // no producer warpgroup: the empty ring is filled here, and refilled slot by slot in the main loop
+    for (int i = 0; i < NSTAGE && kb0 + i < kb1; ++i) load_stage(kb0 + i, i);
   }
 
-  // ======================================================================= consumers: rows 64 (wg - 1) .. +63
-  const int cw = wg - 1;
+  // ======================================================================= consumers: rows 64 cw .. +63
+  const int cw = wg - Cfg::PRODUCER_WG;
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -406,7 +433,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < BK / WGMMA_K; ++k) {
-        const uint64_t da = p.im2col_T ? make_smem_desc(sa + k * IM2COL_SUB_BYTES + cw * 64 * 32, 16, 256, 3)
+        const uint64_t da = IM2COL && p.im2col_T ? make_smem_desc(sa + k * IM2COL_SUB_BYTES + cw * 64 * 32, 16, 256, 3)
                             : AMN ? make_smem_desc(sa + cw * 8192 + k * WGMMA_K * 128, 64 * BK * 2, 1024, 1)
                                   : make_smem_desc(sa + cw * 8192 + k * WGMMA_K * 2, 16, 1024, 1);
         const uint64_t db = BMN ? make_smem_desc(sb + k * WGMMA_K * 128, 64 * BK * 2, 1024, 1)
@@ -417,6 +444,14 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
       wgmma_commit();
       wgmma_wait<1>();  // the previous k-block's MMAs have retired: its slot may be refilled
       if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      if constexpr (!Cfg::PRODUCER_WG) {
+        // k-block kb - 1 + NSTAGE takes the previous k-block's slot once every warpgroup has released it (release
+        // number (kb - 1 - kb0) / NSTAGE of that slot)
+        if (threadIdx.x == 0 && prev >= 0 && kb - 1 + NSTAGE < kb1) {
+          mbar_wait(&empty_bar[prev], ((kb - 1 - kb0) / NSTAGE) & 1);
+          load_stage(kb - 1 + NSTAGE, prev);
+        }
+      }
       prev = stage;
       if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
     }
@@ -426,7 +461,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
 
   // ======================================================================= epilogue
   // Every operand byte has been consumed (the ring holds this tile only), so the ring becomes the fp32 staging tile.
-  named_sync(1, 256);
+  named_sync(1, 128 * Cfg::CONSUMERS);
   float* stg = reinterpret_cast<float*>(smem);
   {
     const int lt = threadIdx.x & 127, r0 = cw * 64 + (lt >> 5) * 16 + ((lt & 31) >> 2), c0 = 2 * (lt & 3);
@@ -436,10 +471,10 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
       *reinterpret_cast<float2*>(stg + (r0 + 8) * Cfg::STG_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
   }
-  named_sync(1, 256);
+  named_sync(1, 128 * Cfg::CONSUMERS);
   switch (epi_kind_of(p)) {  // uniform over the launch
 #define YMP_EPI_CASE(aux, res, out) \
-    case epi_kind(aux, res, out): epilogue_rows<BN, epi_kind(aux, res, out)>(p, stg, m_blk, n_blk); break;
+    case epi_kind(aux, res, out): epilogue_rows<BM, BN, epi_kind(aux, res, out)>(p, stg, m_blk, n_blk); break;
     YMP_EPI_CASE(EPI_AUX_NONE, 0, EPI_OUT_BF16)        // qkv, dgrads, LM head
     YMP_EPI_CASE(EPI_AUX_NONE, 1, EPI_OUT_F32)         // projections onto the fp32 residual stream
     YMP_EPI_CASE(EPI_AUX_NONE, 0, EPI_OUT_ATOMIC)      // wgrad
@@ -447,7 +482,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
     YMP_EPI_CASE(EPI_AUX_GELU_TANH, 0, EPI_OUT_BF16)   // GPT h->4h
     YMP_EPI_CASE(EPI_AUX_MUL, 0, EPI_OUT_BF16)         // their dgrads
 #undef YMP_EPI_CASE
-    default: epilogue_rows<BN, EPI_ANY>(p, stg, m_blk, n_blk);
+    default: epilogue_rows<BM, BN, EPI_ANY>(p, stg, m_blk, n_blk);
   }
 }
 
@@ -508,19 +543,19 @@ static int make_video_map(CUtensorMap* m, const ymp_gemm_args* a) {
   return YMP_OK;
 }
 
-template <int BN, int AMN, int BMN>
+template <int BM, int BN, int AMN, int BMN>
 static int launch_gemm_t(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& kp, int grid, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BM, BN>;
   static DeviceOnce once;
   if (once.first())
-    YMP_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN, AMN, BMN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    YMP_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BM, BN, AMN, BMN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   Cfg::SMEM_BYTES));
-  gemm_bf16_wgmma_kernel<BN, AMN, BMN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, kp);
+  gemm_bf16_wgmma_kernel<BM, BN, AMN, BMN><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, kp);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }
 
-template <int BN>
+template <int BM, int BN>
 static int launch_gemm(const ymp_gemm_args* a, const GemmKParams& kp, cudaStream_t stream) {
   CUtensorMap ta, tb;
   int rc;
@@ -534,16 +569,44 @@ static int launch_gemm(const ymp_gemm_args* a, const GemmKParams& kp, cudaStream
   const int num_m = (a->M + BM - 1) / BM, num_n = (a->N + BN - 1) / BN;
   const int grid = num_m * num_n * kp.split_k;
   switch (kp.a_mn * 2 + kp.b_mn) {
-    case 0: return launch_gemm_t<BN, 0, 0>(ta, tb, kp, grid, stream);
-    case 1: return launch_gemm_t<BN, 0, 1>(ta, tb, kp, grid, stream);
-    case 2: return launch_gemm_t<BN, 1, 0>(ta, tb, kp, grid, stream);
-    default: return launch_gemm_t<BN, 1, 1>(ta, tb, kp, grid, stream);
+    case 0: return launch_gemm_t<BM, BN, 0, 0>(ta, tb, kp, grid, stream);
+    case 1: return launch_gemm_t<BM, BN, 0, 1>(ta, tb, kp, grid, stream);
+    case 2: return launch_gemm_t<BM, BN, 1, 0>(ta, tb, kp, grid, stream);
+    default: return launch_gemm_t<BM, BN, 1, 1>(ta, tb, kp, grid, stream);
   }
+}
+
+// What one CTA per SM spends on a tile, in µs: t per 64-deep k-block of MMAs, f whatever the tile's K (ring fill,
+// epilogue, turnover), f_acc the same with the fp32-atomic epilogue of split-K.  Fitted by tools/gemm_tile_cost.py
+// (DESIGN.md §5) on an H100 80GB HBM3 at 700 W; only their ratios matter for the choices below.
+struct TileCost { double t, f, f_acc; };
+constexpr TileCost TILE_COST_128 = {0.78, 5.0, 14.7};   // 128 x 256
+constexpr TileCost TILE_COST_192 = {1.09, 8.0, 20.0};   // 192 x 256
+
+// A launch of `tiles` output tiles, kb_total k-blocks deep, as waves of one tile per SM: µs of a K split count `split`,
+// or with split = 0 the count the cost model picks (1 unless accumulating: the K splits then add into D).
+struct GemmPlan { int split; double us; };
+static GemmPlan plan_gemm(long tiles, int kb_total, int split, bool accumulate, int sms, const TileCost& c) {
+  auto cost = [&](int sp) {
+    const long waves = (tiles * sp + sms - 1) / sms;
+    return waves * (((kb_total + sp - 1) / sp) * c.t + (accumulate ? c.f_acc : c.f));
+  };
+  if (split > 0) return {split, cost(std::min(split, kb_total))};
+  GemmPlan best{1, cost(1)};
+  if (accumulate) {
+    for (int sp = 2; sp <= 64 && sp * 8 <= kb_total; ++sp) {
+      const double us = cost(sp);
+      if (us < best.us) best = {sp, us};
+    }
+  }
+  return best;
 }
 
 }  // namespace ymp
 
-extern "C" int ymp_gemm(const ymp_gemm_args* a, void* stream) {
+extern "C" int ymp_gemm(const ymp_gemm_args* a, void* stream) { return ymp_gemm_tiled(a, 0, stream); }
+
+extern "C" int ymp_gemm_tiled(const ymp_gemm_args* a, int tile_m, void* stream) {
   using namespace ymp;
   YMP_CHECK_ARG(a != nullptr, "ymp_gemm: null args");
   YMP_CHECK_ARG(a->A && a->B && a->D, "ymp_gemm: null A/B/D");
@@ -578,33 +641,32 @@ extern "C" int ymp_gemm(const ymp_gemm_args* a, void* stream) {
                 "ymp_gemm: dropout needs 0 < p < 1 and is not combined with aux_out / accumulate");
   YMP_CHECK_ARG(a->tile_n == 0 || a->tile_n == 128 || a->tile_n == 256 || a->tile_n == 512,
                 "ymp_gemm: tile_n must be 0 (auto), 128, 256 or 512 (the widest tile: 256 columns on sm_90)");
+  YMP_CHECK_ARG(tile_m == 0 || tile_m == 128 || tile_m == 192, "ymp_gemm: tile_m must be 0 (auto), 128 or 192 (tile_m=%d)", tile_m);
+  YMP_CHECK_ARG(tile_m != 192 || (a->tile_n != 128 && !a->im2col_P),
+                "ymp_gemm: tile_m = 192 needs the 256-column tile and no fused im2col operand");
 
   const int kb_total = (a->K + BK - 1) / BK;
   const int sms = num_sms();
   int bn = a->tile_n == 512 ? 256 : a->tile_n;
+  if (tile_m == 192) bn = 256;
   if (a->im2col_P && bn == 0) bn = (a->N <= 128) ? 128 : 256;
   if (bn == 0) {
     // the 128x256 tile when it fills the machine (or for split-K accumulation); 128x128 when N is narrow or the
     // wide tile would leave SMs idle
-    const long t256 = (long)((a->M + BM - 1) / BM) * ((a->N + 255) / 256);
+    const long t256 = (long)((a->M + 127) / 128) * ((a->N + 255) / 256);
     bn = (a->N <= 128 || (t256 < sms && a->split_k <= 1 && !a->accumulate)) ? 128 : 256;
   }
-  int split = a->split_k;
-  if (split <= 0) {
-    split = 1;
-    if (a->accumulate) {
-      const long tiles = (long)((a->M + BM - 1) / BM) * ((a->N + bn - 1) / bn);
-      // cost model (k-blocks of MMA time): waves x (k-blocks per unit + a fixed pipeline-fill / atomic-epilogue
-      // overhead of ~24 k-blocks), one unit per SM at a time
-      const long workers = sms;
-      long best = -1;
-      for (int sp = 1; sp <= 64 && sp * 8 <= kb_total; ++sp) {
-        const long waves = (tiles * sp + workers - 1) / workers;
-        const long cost = waves * ((kb_total + sp - 1) / sp + 24);
-        if (best < 0 || cost < best) { best = cost; split = sp; }
-      }
-    }
+  // 192 rows when the 256-column tile runs and the cost model puts it below 128 rows: fewer operand bytes per FLOP and
+  // epilogue threads per row, against coarser waves and more rows past M
+  const bool acc = a->accumulate != 0;
+  const long tiles128 = (long)((a->M + 127) / 128) * ((a->N + bn - 1) / bn);
+  GemmPlan plan = plan_gemm(tiles128, kb_total, a->split_k, acc, sms, TILE_COST_128);
+  int bm = 128;
+  if (tile_m == 192 || (tile_m == 0 && bn == 256 && !a->im2col_P)) {
+    const GemmPlan p192 = plan_gemm((long)((a->M + 191) / 192) * ((a->N + 255) / 256), kb_total, a->split_k, acc, sms, TILE_COST_192);
+    if (tile_m == 192 || p192.us < plan.us) { plan = p192; bm = 192; }
   }
+  int split = plan.split;
   YMP_CHECK_ARG(split == 1 || (a->accumulate && a->out_dtype == YMP_DT_F32), "ymp_gemm: split_k>1 needs accumulate=1 and fp32 output");
   if (split > kb_total) split = kb_total;
   int per = (kb_total + split - 1) / split;
@@ -632,7 +694,8 @@ extern "C" int ymp_gemm(const ymp_gemm_args* a, void* stream) {
   kp.has_drop = (a->drop.rng && a->drop.p > 0.f) ? 1 : 0;
   kp.drop.rng = a->drop.rng; kp.drop.site = a->drop.site; kp.drop.p = a->drop.p;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (bn == 256) return launch_gemm<256>(a, kp, st);
-  return launch_gemm<128>(a, kp, st);
+  if (bm == 192) return launch_gemm<192, 256>(a, kp, st);
+  if (bn == 256) return launch_gemm<128, 256>(a, kp, st);
+  return launch_gemm<128, 128>(a, kp, st);
 }
 

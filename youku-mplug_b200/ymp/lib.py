@@ -165,6 +165,9 @@ def _declare(name, argstruct):
 
 
 _gemm = _declare("ymp_gemm", GemmArgs)
+_gemm_tiled = lib.ymp_gemm_tiled
+_gemm_tiled.restype = C.c_int
+_gemm_tiled.argtypes = [C.POINTER(GemmArgs), C.c_int, c_vp]
 _gemm_skinny = _declare("ymp_gemm_skinny", GemmSkinnyArgs)
 _gemm_skinny_wide = _declare("ymp_gemm_skinny_wide", GemmSkinnyArgs)
 _ln_fwd = _declare("ymp_layernorm_fwd", LayerNormArgs)

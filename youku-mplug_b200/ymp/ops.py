@@ -61,10 +61,12 @@ def _chk2d(t, name):
 
 def gemm(a, b, *, a_t=False, b_t=False, bias=None, residual=None, act=ACT_NONE, aux_out=None,
          aux_in=None, out=None, out_dtype=bf16, accumulate=False, split_k=0, alpha=1.0, tile_n=0,
-         res_row_mod=0, d_row_block=0, d_row_stride=0, drop=None, _im2col=None):
+         tile_m=0, res_row_mod=0, d_row_block=0, d_row_stride=0, drop=None, _im2col=None):
     """D[M,N] = epilogue(alpha * op(A) @ op(B)^T).
 
     a: [M,K] (or [K,M] when a_t)      b: [N,K] like nn.Linear.weight (or [K,N] when b_t)
+    tile_n / tile_m: output tile width (0: auto, 128, 256) and height (0: auto, 128, 192; 192 needs the 256-wide
+    tile and no fused im2col)
     """
     _chk2d(a, "a"); _chk2d(b, "b")
     assert a.dtype == bf16 and b.dtype == bf16
@@ -110,7 +112,7 @@ def gemm(a, b, *, a_t=False, b_t=False, bias=None, residual=None, act=ACT_NONE, 
     _set_drop(g.drop, drop)
     if _im2col is not None:
         g.im2col_P, g.im2col_B, g.im2col_C, g.im2col_T, g.im2col_H, g.im2col_W = _im2col
-    L.call(L._gemm, g, "ymp_gemm")
+    L.check(L._gemm_tiled(L.C.byref(g), tile_m, L.cur_stream()), "ymp_gemm")
     return out
 
 
