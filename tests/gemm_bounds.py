@@ -238,6 +238,16 @@ def bounds(ref, K, *, split=1, out_bf16=True):
     return C * e_out + TINY, C * e_aux + TINY
 
 
+def skinny_slices(N, K):
+    """K slices per CTA of ymp_gemm_skinny / ymp_gemm_skinny_wide, as the host picks them (gemv.cu): up to 8 (4 for
+    N > 4096), doubled while every slice keeps at least 128 columns.  Each slice is its own accumulation chain (the
+    `split` of bounds())."""
+    ks, ks_max = 1, 8 if N <= 4096 else 4
+    while ks < ks_max and K // (2 * ks) >= 128:
+        ks *= 2
+    return ks
+
+
 def layernorm_reference(y, gamma, beta, eps):
     """float64 LayerNorm of each row of y (the kernel's own fp32 result); returns (ln, z, rstd, mean|y|, sigma)."""
     y = y.double()

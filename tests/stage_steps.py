@@ -44,6 +44,16 @@ Bounds this module adds (C, u, u32, TINY as in gemm_bounds.py; each is one round
 
 Row layouts are those of the kernels' interfaces: ViT tokens row (b N + n) T + t, then B cls rows; decoder row
 b S + s; attention operands are gathered per (sequence, head) through the calls' own sequence maps.
+
+Decoding (decode_session: DistributedGPT3's sample / beam_search over the KV cache).  Host events drive the program:
+decode entries (new token ids, whether query embeddings were fed), KVCache.reindex / reorder / share_prefill, and the
+logits each decode returned, which must be the last step's value bit for bit.  The program keeps each sequence's
+history of cached QKV rows (KVHistory) and applies the events to it; every attention step's K / V operands, gathered
+through the call's row table (kv_rows, min(s_kv, *s_kv_dev) keys), must equal that history bit for bit, and a skinny
+QKV GEMM's cache copy must land in slot b max_len + len and equal its output row bit for bit.  The GPU walks fill each
+new cache store with a finite +-3e4 poison, so a read of a slot no step wrote fails.  The skinny GEMMs use
+gemm_bounds.bounds with split = skinny_slices(N, K) (each K slice is its own chain) and their fused LayerNorm
+gemm_bounds.layernorm_bound of the kernel's own fp32 y; the table gather is exact.  No bound is added.
 """
 import json
 import math
@@ -127,6 +137,20 @@ def _k_gemm(a, kw, sms):
     if kw.get("aux"):
         r["aux"] = (ref["aux"], e_aux)
     return r
+
+
+def _k_skinny(a, kw, sms):
+    # out2 (the KV-cache copy) holds the same bf16 value as D; the walker also checks that bit for bit
+    A, B = a["A"], a["B"]
+    ref = GB.reference(A, B, bias=a.get("bias"), act=kw.get("act", 0), residual=a.get("residual"))
+    e_out, _ = GB.bounds(ref, A.shape[1], split=GB.skinny_slices(B.shape[0], A.shape[1]), out_bf16=kw["out_dtype"] == BF16)
+    return dict(D=(ref["out"], e_out), out2=(ref["out"], e_out))
+
+
+def _skinny_ln(y, a, kw):
+    """The skinny kernel's fused LayerNorm is of its own fp32 result y: (float64 LN(y), bound)."""
+    g, b, eps = a["ln_gamma"], a["ln_beta"], kw["ln_eps"]
+    return GB.layernorm_reference(y, g, b, eps)[0], GB.layernorm_bound(y, g, b, eps)
 
 
 def _k_im2col(a, kw, sms):
@@ -235,7 +259,7 @@ def _k_ce_bwd(a, kw, sms):
 KERNELS = dict(gemm=_k_gemm, patch_embed_gemm=_k_gemm, im2col=_k_im2col, layernorm_fwd=_k_ln_fwd, layernorm_bwd=_k_ln_bwd,
                attn_fwd=_k_attn_fwd, attn_bwd=_k_attn_bwd, attn_temporal_fwd=_k_attn_fwd, attn_temporal_bwd=_k_attn_bwd,
                group_reduce=_k_group_reduce, colsum=_k_colsum, dropout=_k_dropout, embed_gather=_k_embed,
-               ce_fwd=_k_ce_fwd, ce_bwd=_k_ce_bwd)
+               ce_fwd=_k_ce_fwd, ce_bwd=_k_ce_bwd, gemm_skinny=_k_skinny, gemm_skinny_wide=_k_skinny)
 
 
 def patch_rows(video, P):
@@ -307,7 +331,9 @@ class Exec:
             if self.mode == "synth" and name in self.tamper:
                 ins, kw = self.tamper[name](dict(ins), dict(kw), self.vals)
             refs = KERNELS[op](ins, kw, self.sms)
-            res = {o: (refs[o][0] if self.mode == "exact" else self.rnd(refs[o][0], outs[o])) for o in outs}
+            res = {o: (refs[o][0] if self.mode == "exact" else self.rnd(refs[o][0], outs[o])) for o in outs if o != "ln"}
+            if "ln" in outs:
+                res["ln"] = self.rnd(_skinny_ln(res["D"], ins, kw)[0], outs["ln"])
             if self.mode == "synth":
                 targets = {o: (acc[o] if (o in acc and acc[o] is not None) else None) for o in outs}
                 self.out_trace.append(Rec(op, {k: v.clone() for k, v in ins.items()}, kw,
@@ -372,7 +398,9 @@ class Exec:
             if o not in rec.outs:
                 raise StepFailure(name, f"output {o} missing from the trace")
             got = rec.outs[o]
-            want, bound = refs[o]
+            want, bound = _skinny_ln(rec.outs["D"].to(F64), ins, kw) if o == "ln" else refs[o]
+            if o == "out2" and not torch.equal(got, rec.outs["D"].to(got.dtype)):
+                raise StepFailure(name, "value out2: the cache row is not the output row bit for bit")
             if got.dtype != dt:
                 raise StepFailure(name, f"output {o} stored as {got.dtype}, expected {dt}")
             if tuple(got.shape) != tuple(want.shape):
@@ -431,6 +459,47 @@ class Exec:
         if self.mode == "walk" and not _same(got, want):
             raise StepFailure(name, "the returned tensor is not the last step's value")
 
+    # ---- host events (decoding: cache table updates, decode entries, returned logits)
+    def next_host(self, name, script):
+        """The next host event (kind, payload) that drives a program: walk reads it from the trace (None at its end),
+        exact / synth take it from the iterator `script` (synth logs it).  A synth tamper named `name.kind` changes
+        what the program applies, not what is logged (an event the product logs but does not carry out)."""
+        if self.mode == "walk":
+            if self.pos >= len(self.trace):
+                return None
+            rec = self.trace[self.pos]
+            if rec.op != "event":
+                raise StepFailure(f"after {self.pos} calls", f"schedule: expected a host event, the trace has {rec.op}")
+            self.pos += 1
+            return rec.kw["kind"], rec.ins
+        ev = next(script, None)
+        if ev is None:
+            return None
+        kind, payload = ev
+        return kind, self._log_event(f"{name}.{kind}", kind, payload)
+
+    def host(self, name, kind, payload):
+        """A host event the program expects here with this payload (walk: the recorded one must match it)."""
+        if self.mode == "walk":
+            if self.pos >= len(self.trace):
+                raise StepFailure(name, f"schedule: the trace ends before this {kind} event")
+            rec = self.trace[self.pos]
+            self.pos += 1
+            if rec.op != "event" or rec.kw["kind"] != kind:
+                raise StepFailure(name, f"schedule: expected a {kind} event, the trace has {rec.kw.get('kind', rec.op)}")
+            for k in set(payload) | set(rec.ins):
+                if not _same(payload.get(k), rec.ins.get(k)):
+                    raise StepFailure(name, f"event {kind}: {k} is not the value the program names")
+            return payload
+        return self._log_event(name, kind, payload)
+
+    def _log_event(self, name, kind, payload):
+        if self.mode == "synth":
+            self.out_trace.append(Rec("event", dict(payload), dict(kind=kind), {}, {}))
+            if name in self.tamper:
+                return self.tamper[name](dict(payload), None, self.vals)
+        return payload
+
 
 def write_report(ex, stage):
     """Merge the walk's largest err/bound per step into the JSON file named by YMP_STAGE_BOUNDS_REPORT."""
@@ -477,10 +546,10 @@ def colsum(X, name, x, tgt):
     return X.call(name, "colsum", dict(x=x), {}, dict(out=F32), acc=dict(out=tgt))["out"]
 
 
-def ln_fwd(X, name, x, W, pre, eps, y=BF16, in_rows=None, pad=None):
+def ln_fwd(X, name, x, W, pre, eps, y=BF16, in_rows=None, pad=None, stats=True):
     r = X.call(name, "layernorm_fwd", dict(x=x, gamma=W[pre + ".weight"], beta=W[pre + ".bias"]),
-               dict(eps=eps, y_dtype=y, in_rows=in_rows, pad=pad), dict(y=y, mean=F32, rstd=F32))
-    return r["y"], r["mean"], r["rstd"]
+               dict(eps=eps, y_dtype=y, in_rows=in_rows, pad=pad), dict(y=y, mean=F32, rstd=F32) if stats else dict(y=y))
+    return r["y"], r.get("mean"), r.get("rstd")
 
 
 def ln_bwd(X, name, dy, x, W, pre, mean, rstd, T, add=None, drop=None, in_rows=None, xrows=None):
@@ -498,10 +567,29 @@ def ln_bwd(X, name, dy, x, W, pre, mean, rstd, T, add=None, drop=None, in_rows=N
     return r["dx"], r.get("dx_drop", r["dx"])
 
 
-def attn(X, name, q, k, v, *, scale, causal=False, drop=None, temporal=False):
+def attn(X, name, q, k, v, *, scale, causal=False, drop=None, temporal=False, keys=None):
+    """keys: the key count of a call that reads its keys through a row table (kv_rows), as the device held it."""
     r = X.call(name, "attn_temporal_fwd" if temporal else "attn_fwd", dict(q=q, k=k, v=v),
-               dict(mask=AB.MASK_CAUSAL if causal else AB.MASK_NONE, scale=scale, drop=drop), dict(o=BF16, lse=F32))
+               dict(mask=AB.MASK_CAUSAL if causal else AB.MASK_NONE, scale=scale, drop=drop, keys=keys),
+               dict(o=BF16, lse=F32))
     return r["o"], r["lse"]
+
+
+def skinny(X, name, op, A, B, *, bias=None, residual=None, act=ACT_NONE, out=BF16, out2_rows=None, ln=None):
+    """ymp_gemm_skinny(_wide): D = act(A B^T + bias) + residual.  out2_rows: the KV-cache rows the result is also
+    written to (the step names them); ln = (W, prefix, eps): the kernel's last CTA also returns LN(D) (y, ln)."""
+    ins = dict(A=A, B=B, bias=bias, residual=residual)
+    kw = dict(act=act, out_dtype=out, out2_rows=out2_rows, ln_eps=None)
+    outs = dict(D=out)
+    if out2_rows is not None:
+        outs["out2"] = BF16
+    if ln is not None:
+        Wl, pre, eps = ln
+        ins.update(ln_gamma=Wl[pre + ".weight"], ln_beta=Wl[pre + ".bias"])
+        kw["ln_eps"] = eps
+        outs["ln"] = BF16
+    r = X.call(name, op, ins, kw, outs)
+    return (r["D"], r["ln"]) if ln is not None else r["D"]
 
 
 def attn_b(X, name, q, k, v, o, lse, do, *, scale, causal=False, drop=None, temporal=False):
@@ -1104,6 +1192,209 @@ def component_bwd(X, W, T, c, loss_mask):
     return d_img
 
 
+# ---------------------------------------------------------------------------------- GPT-3 decoding
+POISON = 3.0e4
+
+
+def poison_(store):
+    """Fill a bf16 KV-cache store with the finite poison +-3e4 in alternating signs (every row starts with +), so
+    that a read of a slot no step wrote fails its bound."""
+    v = store.view(-1, 2)
+    v[:, 0] = POISON
+    v[:, 1] = -POISON
+    return store
+
+
+def poison_row(width, dev="cpu"):
+    r = torch.full((width,), POISON, dtype=F64, device=dev)
+    r[1::2] = -POISON
+    return r.to(BF16).to(F64)
+
+
+class KVHistory:
+    """The decoder's KV cache as the decoding programs see it: for each sequence, the ids of the cached QKV rows of its
+    positions in order.  Every layer's row of one position has the same id; id 0 is the poison row of a slot that was
+    never written.  reindex / reorder permute the sequences' lists; share_prefill starts every beam of a clip from
+    its clip's prefill rows."""
+
+    def __init__(self, layers, B, width, dev):
+        self.B, self.len = B, 0
+        self.pool = [[poison_row(width, dev)[None]] for _ in range(layers)]
+        self.n = [1] * layers
+        self._cat = [None] * layers
+        self.seq = [[] for _ in range(B)]
+
+    def put(self, i, rows):
+        """Cache the QKV rows [r, 3H] of layer i; returns their ids."""
+        base = self.n[i]
+        self.pool[i].append(rows)
+        self.n[i] += rows.shape[0]
+        self._cat[i] = None
+        return list(range(base, self.n[i]))
+
+    def rows(self, i):
+        """[B, len, 3H] float64: each sequence's cached rows of layer i, in position order."""
+        if self._cat[i] is None:
+            self._cat[i] = torch.cat(self.pool[i])
+        idx = torch.tensor(self.seq, dtype=torch.long, device=self._cat[i].device)
+        return self._cat[i][idx]
+
+    def permute(self, idx):
+        """Sequence b continues old sequence idx[b]."""
+        self.seq = [list(self.seq[int(j)]) for j in idx]
+
+
+def _emb_pos(W, ids, p0, n, qf=None):
+    """[word_embeddings[ids] (after the prefix qf) | positions p0 .. p0 + n - 1] as DistributedGPT3._decode and
+    TokenStep add them: x = fl32(bf16 embedding + bf16 position), [B n, H]."""
+    wemb, pos = W[GPT + "embedding.word_embeddings.weight"], W[GPT + "embedding.position_embeddings.weight"]
+    B = ids.shape[0]
+    emb = wemb[ids.reshape(-1).to(wemb.device)].view(B, -1, wemb.shape[1])
+    if qf is not None:
+        emb = torch.cat([qf.to(F64), emb], 1)
+    return emb + pos[p0:p0 + n][None]
+
+
+def decode_prefill(X, W, qf, ids, gcfg, stride, hist, name="decode.0"):
+    """gpt_decode with an empty cache (off = 0) and the bf16 LM head of DistributedGPT3._decode.  The B / stride
+    sequences [qf | ids] of n positions: x = fl32(emb + pos[0:n]); per layer LN1 -> QKV (GEMM row b n + i is cache
+    row (b stride) max_len + i) -> causal attention -> dense + fp32 residual -> LN2 -> h->4h tanh-GELU -> 4h->h +
+    residual; share_prefill(stride); the final LayerNorm of each sequence's last row b n + n - 1; the LM head.
+    Sequence b's rows become the history of cache sequence b stride; the other beams of its group hold poison until
+    share_prefill points them at it.  Returns the logits [B / stride, V]."""
+    g = dims_gpt(gcfg)
+    nh, hd, H = g["nh"], g["hd"], g["H"]
+    Bp = ids.shape[0]
+    if Bp * stride != hist.B:
+        raise StepFailure(name, f"decode entry: {Bp} prefill sequences at stride {stride} for a cache of {hist.B}")
+    emb = _emb_pos(W, ids, 0, ids.shape[1] + (0 if qf is None else qf.shape[1]), qf)
+    n = emb.shape[1]
+    x = X.rnd(emb, F32).reshape(Bp * n, H)
+    for i in range(g["layers"]):
+        pre, s = f"{GPT}encoder.layers.{i}.", f"{name}.L{i}."
+        ln1, _, _ = ln_fwd(X, s + "input_layernorm", x, W, pre + "input_layernorm", g["eps"], stats=False)
+        qkv = gemm(X, s + "qkv", ln1, W[pre + "self_attention.query_key_value.weight"],
+                   bias=W[pre + "self_attention.query_key_value.bias"])
+        new = hist.put(i, qkv)
+        if i == 0:
+            hist.seq = [new[(b // stride) * n:(b // stride + 1) * n] if b % stride == 0 else [0] * n for b in range(hist.B)]
+        q, k, v = (heads(qkv, Bp, n, nh, hd, col=j * hd, hs=3 * hd) for j in range(3))
+        o, _ = attn(X, s + "attn", q, k, v, scale=g["scale"], causal=True)
+        x1 = gemm(X, s + "dense", unheads(o), W[pre + "self_attention.dense.weight"],
+                  bias=W[pre + "self_attention.dense.bias"], residual=x, out=F32)
+        ln2, _, _ = ln_fwd(X, s + "post_attention_layernorm", x1, W, pre + "post_attention_layernorm", g["eps"], stats=False)
+        h = gemm(X, s + "h_to_4h", ln2, W[pre + "mlp.dense_h_to_4h.weight"], bias=W[pre + "mlp.dense_h_to_4h.bias"],
+                 act=ACT_GELU_TANH)
+        x = gemm(X, s + "4h_to_h", h, W[pre + "mlp.dense_4h_to_h.weight"], bias=W[pre + "mlp.dense_4h_to_h.bias"],
+                 residual=x1, out=F32)
+    hist.len = n
+    if X.host(name + ".share_prefill", "share_prefill", dict(stride=stride)) is not None and stride > 1:
+        hist.seq = [list(hist.seq[b // stride * stride]) for b in range(hist.B)]
+    last = torch.arange(Bp, dtype=torch.int32) * n + (n - 1)
+    hid, _, _ = ln_fwd(X, name + ".final_layernorm", x[last.long().to(x.device)], W, GPT + "encoder.final_layernorm",
+                       g["eps"], in_rows=last, stats=False)
+    return gemm(X, name + ".lm_head", hid, W[GPT + "embedding.word_embeddings.weight"])
+
+
+def decode_token(X, W, tok, hist, gcfg, kind, name, max_len):
+    """One single-token step of all B sequences at position len = hist.len, after which len grows by one.
+    kind "skinny" is TokenStep: x = fl32(bf16 emb(tok) + bf16 pos[len]), every linear a skinny GEMM (the wide entry
+    point above 8 rows); the QKV GEMM writes q to the staging rows and the same row to cache slot b max_len + len;
+    attention reads the len + 1 keys of each sequence's history (the new one last) through the row table; the
+    LayerNorms are separate calls, or with kind "skinny_ln" computed by the last CTA of the GEMM that completes their
+    input; fp32 logits.  kind "gemm" is gpt_decode with n = 1: wgmma GEMMs, the QKV rows stored straight into the
+    cache slots, share_prefill(1), the final LayerNorm through in_rows, bf16 logits.  Returns the logits [B, V]."""
+    g = dims_gpt(gcfg)
+    nh, hd, H, eps = g["nh"], g["hd"], g["H"], g["eps"]
+    B, p = hist.B, hist.len
+    x = X.rnd(_emb_pos(W, tok.reshape(B, 1), p, 1), F32).reshape(B, H)
+    op = "gemm_skinny" if B <= 8 else "gemm_skinny_wide"
+
+    def lin(nm, a, wname, **k):
+        wb = dict(bias=W[wname + ".bias"])
+        if kind == "gemm":
+            k.pop("out2_rows", None)
+            return gemm(X, nm, a, W[wname + ".weight"], **wb, **k)
+        return skinny(X, nm, op, a, W[wname + ".weight"], **wb, **k)
+
+    def lin_ln(nm, a, wname, residual, ln_pre, ln_name):
+        if kind == "skinny_ln":
+            return skinny(X, nm, op, a, W[wname + ".weight"], bias=W[wname + ".bias"], residual=residual, out=F32,
+                          ln=(W, ln_pre, eps))
+        y = lin(nm, a, wname, residual=residual, out=F32)
+        if kind == "gemm":    # gpt_decode normalises at the start of the next layer, the final rows after the loop
+            return y, None
+        return y, ln_fwd(X, ln_name, y, W, ln_pre, eps, stats=False)[0]
+
+    ln1 = ln_fwd(X, f"{name}.L0.input_layernorm", x, W, f"{GPT}encoder.layers.0.input_layernorm", eps, stats=False)[0]
+    for i in range(g["layers"]):
+        pre, s = f"{GPT}encoder.layers.{i}.", f"{name}.L{i}."
+        if kind == "gemm" and i > 0:
+            ln1 = ln_fwd(X, s + "input_layernorm", x, W, pre + "input_layernorm", eps, stats=False)[0]
+        qkv = lin(s + "qkv", ln1, pre + "self_attention.query_key_value",
+                  out2_rows=torch.arange(B, dtype=torch.int64) * max_len + p)
+        new = hist.put(i, qkv)
+        if i == 0:
+            for b in range(B):
+                hist.seq[b].append(new[b])
+        q = heads(qkv, B, 1, nh, hd, hs=3 * hd)
+        rows = hist.rows(i).reshape(B * (p + 1), 3 * H)
+        k, v = (heads(rows, B, p + 1, nh, hd, col=j * hd, hs=3 * hd) for j in (1, 2))
+        o, _ = attn(X, s + "attn", q, k, v, scale=g["scale"], keys=p + 1)
+        x1, ln2 = lin_ln(s + "dense", unheads(o), pre + "self_attention.dense", x, pre + "post_attention_layernorm",
+                         s + "post_attention_layernorm")
+        if kind == "gemm":
+            ln2 = ln_fwd(X, s + "post_attention_layernorm", x1, W, pre + "post_attention_layernorm", eps, stats=False)[0]
+        h = lin(s + "h_to_4h", ln2, pre + "mlp.dense_h_to_4h", act=ACT_GELU_TANH)
+        last = i + 1 == g["layers"]
+        nxt = GPT + "encoder.final_layernorm" if last else f"{GPT}encoder.layers.{i + 1}.input_layernorm"
+        x, ln1 = lin_ln(s + "4h_to_h", h, pre + "mlp.dense_4h_to_h", x1, nxt,
+                        f"{name}.final_layernorm" if last else f"{name}.L{i + 1}.input_layernorm")
+    hist.len = p + 1
+    wemb = W[GPT + "embedding.word_embeddings.weight"]
+    if kind != "gemm":
+        return skinny(X, name + ".lm_head", op, ln1, wemb, out=F32)
+    X.host(name + ".share_prefill", "share_prefill", dict(stride=1))
+    hid = ln_fwd(X, name + ".final_layernorm", x, W, GPT + "encoder.final_layernorm", eps,
+                 in_rows=torch.arange(B, dtype=torch.int32), stats=False)[0]
+    return gemm(X, name + ".lm_head", hid, wemb)
+
+
+def decode_session(X, W, gcfg, qf, script=None, *, B, max_len, stride=1, kind="skinny"):
+    """A decoding run of DistributedGPT3 (sample / beam_search / the batched beam search) over one KV cache of B
+    sequences: the host events drive it (exact / synth: `script`, a list of (kind, payload); walk: the trace).
+    ("decode", dict(tokens, query)) is a decode entry: the first is the prefill of [qf | tokens] (query embeddings
+    fed), every later one a single-token step; ("reindex" | "reorder", dict(idx)) permutes the sequences.  After each
+    decode the logits it returned must be the last step's value bit for bit.  Returns every decode's logits."""
+    g = dims_gpt(gcfg)
+    hist = KVHistory(g["layers"], B, 3 * g["H"], W[GPT + "embedding.word_embeddings.weight"].device)
+    it = iter(script or [])
+    out = []
+    while True:
+        name = f"decode.{len(out)}"
+        ev = X.next_host(name, it)
+        if ev is None:
+            return out
+        kind_, p = ev
+        if kind_ in ("reindex", "reorder"):
+            if p is not None:
+                hist.permute(p["idx"].tolist())
+            continue
+        if kind_ != "decode":
+            raise StepFailure(name, f"schedule: unexpected host event {kind_}")
+        first = hist.len == 0
+        if bool(p["query"]) != (first and qf is not None):
+            raise StepFailure(name, f"decode entry: query embeddings fed = {bool(p['query'])}")
+        if first:
+            logits = decode_prefill(X, W, qf, p["tokens"], gcfg, stride, hist, name)
+        else:
+            if tuple(p["tokens"].shape) != (B, 1):
+                raise StepFailure(name, f"decode entry: tokens of shape {tuple(p['tokens'].shape)}, expected ({B}, 1)")
+            logits = decode_token(X, W, p["tokens"][:, 0], hist, gcfg, kind, name, max_len)
+        X.host(name + ".logits", "logits", dict(logits=logits))
+        out.append(logits)
+
+
 # ---------------------------------------------------------------------------------- trace recorder (GPU)
 def _map_dict(m):
     return {f: int(getattr(m, f)) for f in ("seq_div", "n_prefix", "prefix_per_seq", "outer_stride", "inner_stride",
@@ -1116,6 +1407,12 @@ def _gather_view(tv, n, S, H, hd):
     return heads(tv.t[rows].to(F64), n, S, H, hd, col=tv.col, hs=tv.hs)
 
 
+def _table_view(tv, rows, H, hd):
+    """A TView's keys read through a row table: rows [n, cnt] -> [n, H, cnt, hd] float64."""
+    n, cnt = rows.shape
+    return heads(tv.t[rows.reshape(-1).to(tv.t.device)].to(F64), n, cnt, H, hd, col=tv.col, hs=tv.hs)
+
+
 class Recorder:
     """Wraps the ymp.ops entry points that engine.py and functional.py call (installed with monkeypatch.setattr; the
     product is unchanged).  Every outermost call becomes one Rec: operands gathered to their logical layout and copied
@@ -1124,7 +1421,7 @@ class Recorder:
 
     NAMES = ("gemm", "patch_embed_gemm", "im2col", "layernorm_fwd", "layernorm_bwd", "attn_fwd", "attn_bwd",
              "attn_temporal_fwd", "attn_temporal_bwd", "group_reduce", "colsum", "dropout", "embed_gather", "ce_fwd",
-             "ce_bwd")
+             "ce_bwd", "gemm_skinny", "gemm_skinny_wide")
 
     def __init__(self, ops, G=None):
         self.ops, self.G = ops, dict(G or {})
@@ -1134,6 +1431,23 @@ class Recorder:
     def install(self, monkeypatch):
         for n in self.NAMES:
             monkeypatch.setattr(self.ops, n, self._wrap(n))
+
+    def install_decode(self, monkeypatch, cache_cls, model_cls):
+        """Also log the host events of decoding as Recs of op "event": KVCache.reindex / reorder (idx) and
+        share_prefill (stride), and around every model._decode entry its new token ids and whether query embeddings
+        were fed, then the logits [B, V] it returns."""
+        for nm, key in (("reindex", "idx"), ("reorder", "idx"), ("share_prefill", "stride")):
+            def w(cache, arg, _orig=getattr(cache_cls, nm), _nm=nm, _key=key):
+                self._push("event", {_key: arg.detach().cpu().clone() if torch.is_tensor(arg) else arg}, dict(kind=_nm), {})
+                return _orig(cache, arg)
+            monkeypatch.setattr(cache_cls, nm, w)
+
+        def decode(model, tokens, input_embeds, n_query, _orig=model_cls._decode):
+            self._push("event", dict(tokens=tokens.detach().cpu().clone(), query=n_query > 0), dict(kind="decode"), {})
+            out = _orig(model, tokens, input_embeds, n_query)
+            self._push("event", dict(logits=out.logits.reshape(out.logits.shape[0], -1).clone()), dict(kind="logits"), {})
+            return out
+        monkeypatch.setattr(model_cls, "_decode", decode)
 
     def _key_of(self, t):
         p = t.data_ptr()
@@ -1214,6 +1528,40 @@ class Recorder:
         self._push("im2col", ins, dict(P=P, ld=r.shape[1]), dict(out=r.clone()))
         return r
 
+    def _skinny(self, op, fn, x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_dtype=BF16, out2=None,
+                out2_row_stride=0, out2_off=None, ln=None):
+        """out2: the cache rows m out2_row_stride + *out2_off (offset read after the sync) as output out2 and their
+        indices as argument out2_rows; ln: the fused LayerNorm's (gamma, beta) operands, eps and output ln."""
+        ins = dict(A=x.to(F64).clone(), B=w.to(F64).clone())
+        if bias is not None:
+            ins["bias"] = bias.to(F64).clone()
+        if residual is not None:
+            ins["residual"] = residual.to(F64).clone()
+        kw = dict(act=act, out2_rows=None, ln_eps=None)
+        if ln is not None:
+            ins["ln_gamma"], ins["ln_beta"] = ln[0].to(F64).clone(), ln[1].to(F64).clone()
+            kw["ln_eps"] = ln[2]
+        r = fn(x, w, bias=bias, residual=residual, act=act, out=out, out_dtype=out_dtype, out2=out2,
+               out2_row_stride=out2_row_stride, out2_off=out2_off, ln=ln)
+        torch.cuda.synchronize()
+        y = r[0] if ln is not None else r
+        kw["out_dtype"] = y.dtype
+        outs = dict(D=y.clone())
+        if out2 is not None:
+            rows = torch.arange(y.shape[0], dtype=torch.int64) * out2_row_stride + int(out2_off.item())
+            kw["out2_rows"] = rows
+            outs["out2"] = out2[rows.to(out2.device)].clone()
+        if ln is not None:
+            outs["ln"] = r[1].clone()
+        self._push(op, ins, kw, outs)
+        return r
+
+    def _gemm_skinny(self, fn, x, w, **kw):
+        return self._skinny("gemm_skinny", fn, x, w, **kw)
+
+    def _gemm_skinny_wide(self, fn, x, w, **kw):
+        return self._skinny("gemm_skinny_wide", fn, x, w, **kw)
+
     # ---- LayerNorm
     def _rows_of(self, x, in_rows, rows):
         if in_rows is None:
@@ -1286,9 +1634,16 @@ class Recorder:
 
     def _attn_fwd(self, fn, q, k, v, o, **kw):
         n, H, hd, sq, skv = kw["n_seq"], kw["n_heads"], kw["head_dim"], kw["s_q"], kw["s_kv"]
+        extra = {}
         if self.temporal:
             R, T = self.temporal
             ins = {nm: self._temporal(tv.t[:, tv.col:], R, T, H, hd).clone() for nm, tv in (("q", q), ("k", k), ("v", v))}
+        elif kw.get("kv_rows") is not None:
+            # keys through the row table: key j of sequence s is row kv_rows[s, j], and min(s_kv, *s_kv_dev) exist
+            cnt = skv if kw.get("s_kv_dev") is None else min(skv, int(kw["s_kv_dev"].item()))
+            rows = kw["kv_rows"][:, :cnt].long()
+            ins = dict(q=_gather_view(q, n, sq, H, hd), k=_table_view(k, rows, H, hd), v=_table_view(v, rows, H, hd))
+            extra["keys"] = cnt
         else:
             ins = dict(q=_gather_view(q, n, sq, H, hd), k=_gather_view(k, n, skv, H, hd), v=_gather_view(v, n, skv, H, hd))
         lse = fn(q, k, v, o, **kw)
@@ -1297,7 +1652,7 @@ class Recorder:
             outs = dict(o=self._temporal(o.t, R, T, H, hd).to(BF16), lse=self._lse_temporal(lse, R, T, H).clone())
         else:
             outs = dict(o=_gather_view(o, n, sq, H, hd).to(BF16), lse=lse.clone())
-        self._push("attn_temporal_fwd" if self.temporal else "attn_fwd", ins, self._attn_kw(kw), outs)
+        self._push("attn_temporal_fwd" if self.temporal else "attn_fwd", ins, dict(self._attn_kw(kw), **extra), outs)
         return lse
 
     def _attn_bwd(self, fn, q, k, v, o, lse, dout, dq, dk, dv, **kw):

@@ -428,10 +428,7 @@ def test_skinny_gaussian_model_shapes(cuda, kernel, M, N, K, epi):
     out_dtype = epi.get("out", bf16)
     y = getattr(ops, kernel)(x, w, out_dtype=out_dtype, **kw)
     ref = GB.reference(x, w, **rk)
-    ks = 1   # K slices per CTA, as the host picks them (gemv.cu)
-    while ks < (8 if N <= 4096 else 4) and K // (2 * ks) >= 128:
-        ks *= 2
-    e_out, _ = GB.bounds(ref, K, split=ks, out_bf16=out_dtype == bf16)
+    e_out, _ = GB.bounds(ref, K, split=GB.skinny_slices(N, K), out_bf16=out_dtype == bf16)
     epi_name = "+".join(k for k in epi if k != "out") or "plain"
     _check(f"{kernel}.{M}x{N}x{K}({epi_name}).y", y, ref["out"], e_out)
 

@@ -442,3 +442,161 @@ def test_lm_head_steps_compose_to_reference():
     _close(losses, ref.detach().reshape(-1), "losses")
     _close(dhid, ha.grad.reshape(dhid.shape), "d hidden")
     _grads_close(X, sd, T)
+
+
+# ---------------------------------------------------------------------------------- decoding
+DQ, DPLEN, DSTEPS = 4, 3, 4
+GC_HD80 = dict(GC, hidden_size=160, ffn_hidden_size=640, num_attention_heads=2)
+GC_HD128 = dict(GC, hidden_size=256, ffn_hidden_size=1024, num_attention_heads=2)
+# the beam permutations before each token step of a batched beam search of 2 clips x 2 beams (rows c * 2 + b): each
+# keeps a row within its clip; the later ones take two beams from one ancestor after the beams' histories differ
+REINDEX = ([1, 0, 3, 2], [1, 0, 2, 3], [1, 1, 2, 2], [0, 1, 3, 3])
+
+
+def _dec_weights(gcfg, seed=3):
+    sd = port.init_state_dict(VC, gcfg, DQ, seed=seed, randomize=True)
+    return {k: v.bfloat16().to(F64) for k, v in sd.items() if k.startswith(GPT)}
+
+
+def _beam_case(gcfg, C=2, beam=2, seed=21):
+    """A batched beam search's host events: the prefill of C clips [qf | prompt], then DSTEPS x (reindex, one token per
+    row).  Returns (qf [C, Q, H], script, the token history of every row the logits of each decode belong to)."""
+    g = torch.Generator().manual_seed(seed)
+    V, H = gcfg["vocab_size"], gcfg["hidden_size"]
+    qf = (0.5 * torch.randn(C, DQ, H, generator=g)).bfloat16().to(F64)
+    prompts = torch.randint(0, V, (C, DPLEN), generator=g)
+    script = [("decode", dict(tokens=prompts, query=True))]
+    hist = [prompts[b // beam].tolist() for b in range(C * beam)]
+    hists = [[prompts[c].tolist() for c in range(C)]]
+    for t in range(DSTEPS):
+        idx = torch.tensor(REINDEX[t])
+        tok = torch.randint(0, V, (C * beam, 1), generator=g)
+        script += [("reindex", dict(idx=idx)), ("decode", dict(tokens=tok, query=False))]
+        hist = [hist[j] + [int(tok[b])] for b, j in enumerate(idx.tolist())]
+        hists.append([list(h) for h in hist])
+    return qf, script, hists
+
+
+def _session(X, W, gcfg, qf, script, kind="skinny", beam=2):
+    B = qf.shape[0] * beam
+    return SS.decode_session(X, W, gcfg, qf, script, B=B, max_len=DQ + DPLEN + DSTEPS, stride=beam, kind=kind)
+
+
+def _port_f64(monkeypatch):
+    """port computes its LayerNorm statistics and attention scores in fp32 (.float()): keep float64 tensors float64,
+    so that port.next_token_logits is the float64 reference."""
+    orig = torch.Tensor.float
+    monkeypatch.setattr(torch.Tensor, "float", lambda t, *a, **k: t if t.dtype == F64 else orig(t, *a, **k))
+
+
+@pytest.mark.parametrize("cfg", ["tiny", "hd80", "hd128"])
+@pytest.mark.parametrize("kind", ["skinny", "skinny_ln", "gemm"])
+def test_decode_steps_compose_to_reference(monkeypatch, cfg, kind):
+    """The prefill and single-token step programs, in exact mode over a batched beam history (shared prefill,
+    permutations with repeated ancestors): every decode's logits are port.next_token_logits in float64 of that row's
+    [prefix | token history] within 1e-9 of their maximum."""
+    _port_f64(monkeypatch)
+    gcfg = dict(tiny=GC, hd80=GC_HD80, hd128=GC_HD128)[cfg]
+    W = _dec_weights(gcfg)
+    qf, script, hists = _beam_case(gcfg)
+    logits = _session(SS.Exec("exact"), W, gcfg, qf, script, kind)
+    assert len(logits) == len(hists) == DSTEPS + 1
+    for t, (got, hs) in enumerate(zip(logits, hists)):
+        rows = qf if t == 0 else qf.repeat_interleave(2, 0)
+        want = port.next_token_logits(rows, torch.tensor(hs), W, gcfg)
+        _close(got, want, f"decode {t} logits", tol=1e-9)
+
+
+@pytest.mark.parametrize("kind", ["skinny", "skinny_ln", "gemm"])
+def test_clean_decode_trace_passes(kind):
+    W = _dec_weights(GC)
+    qf, script, _ = _beam_case(GC)
+    Xs = SS.Exec("synth")
+    want = _session(Xs, W, GC, qf, script, kind)
+    Xw = SS.Exec("walk", trace=Xs.out_trace)
+    got = _session(Xw, W, GC, qf, None, kind)
+    Xw.finish()
+    assert len(got) == DSTEPS + 1 and all(torch.equal(a, b) for a, b in zip(got, want))
+    assert Xw.report and max(Xw.report.values()) <= 1.0
+
+
+def _decode_defects(W, qf, script):
+    """(tamper, step that must fail) of each wiring defect of the decoding path, on _beam_case's tiny trace."""
+    pos = W[GPT + "embedding.position_embeddings.weight"]
+    n = DQ + DPLEN
+    prompts, tok2 = script[0][1]["tokens"], script[4][1]["tokens"]
+
+    def x_of(emb):
+        return emb.to(torch.float32).to(F64).reshape(-1, GC["hidden_size"])
+
+    def token_pos_minus_1(ins, kw, vals):            # decode 2 runs at position n + 1
+        ins["x"] = x_of(SS._emb_pos(W, tok2, n, 1))
+        return ins, kw
+
+    def prefill_pos_plus_1(ins, kw, vals):
+        ins["x"] = x_of(SS._emb_pos(W, prompts, 0, n, qf) - pos[:n] + pos[1:n + 1])
+        return ins, kw
+
+    def keys_len(ins, kw, vals):
+        ins["k"], ins["v"], kw["keys"] = ins["k"][:, :, :-1], ins["v"][:, :, :-1], kw["keys"] - 1
+        return ins, kw
+
+    def rows(f):
+        def t(ins, kw, vals):
+            kw["out2_rows"] = f(kw["out2_rows"])
+            return ins, kw
+        return t
+
+    def residual_x(ins, kw, vals):
+        ins["residual"] = vals["decode.2.L0.4h_to_h"]["D"]
+        return ins, kw
+
+    def wrong_ln(ins, kw, vals):
+        pre = GPT + "encoder.layers.1.input_layernorm"
+        ins["gamma"], ins["beta"] = W[pre + ".weight"], W[pre + ".bias"]
+        return ins, kw
+
+    def first_row(ins, kw, vals):
+        r = torch.arange(qf.shape[0], dtype=torch.int32) * n
+        ins["x"], kw["in_rows"] = vals["decode.0.L1.4h_to_h"]["D"][r.long()], r
+        return ins, kw
+
+    def wrong_clip(ins, kw, vals):
+        ins["x"] = ins["x"].roll(n, 0)
+        return ins, kw
+
+    return {
+        "a_token_position_len_minus_1": ({"decode.2.L0.input_layernorm": token_pos_minus_1}, "decode.2.L0.input_layernorm"),
+        "b_prefill_positions_shifted": ({"decode.0.L0.input_layernorm": prefill_pos_plus_1}, "decode.0.L0.input_layernorm"),
+        "c_attention_count_len": ({"decode.2.L0.attn": keys_len}, "decode.2.L0.attn"),
+        "d_kv_row_at_len_plus_1": ({"decode.2.L0.qkv": rows(lambda r: r + 1)}, "decode.2.L0.qkv"),
+        "d_kv_row_other_sequence": ({"decode.2.L0.qkv": rows(lambda r: r.roll(1))}, "decode.2.L0.qkv"),
+        "e_reindex_not_applied": ({"decode.3.reindex": lambda p, _, v: None}, "decode.3.L0.attn"),
+        "f_share_prefill_not_applied": ({"decode.0.share_prefill": lambda p, _, v: None}, "decode.1.L0.attn"),
+        "g_mlp_residual_from_x": ({"decode.2.L1.4h_to_h": residual_x}, "decode.2.L1.4h_to_h"),
+        "h_final_layernorm_params": ({"decode.2.final_layernorm": wrong_ln}, "decode.2.final_layernorm"),
+        "i_prefill_final_ln_first_row": ({"decode.0.final_layernorm": first_row}, "decode.0.final_layernorm"),
+        "j_prefill_wrong_clip": ({"decode.0.L0.input_layernorm": wrong_clip}, "decode.0.L0.input_layernorm"),
+    }
+
+
+DECODE_DEFECTS = ("a_token_position_len_minus_1", "b_prefill_positions_shifted", "c_attention_count_len",
+                  "d_kv_row_at_len_plus_1", "d_kv_row_other_sequence", "e_reindex_not_applied",
+                  "f_share_prefill_not_applied", "g_mlp_residual_from_x", "h_final_layernorm_params",
+                  "i_prefill_final_ln_first_row", "j_prefill_wrong_clip")
+
+
+@pytest.mark.parametrize("defect", DECODE_DEFECTS)
+def test_decode_wiring_defect_fails_at_its_step(defect):
+    W = _dec_weights(GC)
+    qf, script, _ = _beam_case(GC)
+    defects = _decode_defects(W, qf, script)
+    assert set(defects) == set(DECODE_DEFECTS)
+    tamper, step = defects[defect]
+    Xs = SS.Exec("synth", tamper=tamper)
+    _session(Xs, W, GC, qf, script)
+    Xw = SS.Exec("walk", trace=Xs.out_trace)
+    with pytest.raises(SS.StepFailure) as e:
+        _session(Xw, W, GC, qf, None)
+        Xw.finish()
+    assert e.value.step == step, str(e.value)

@@ -223,3 +223,86 @@ def test_component_path_walks(cuda, monkeypatch):
 
     X, _ = _walk("component.vitb_1p3b_p0.1", rec.trace, G0, run, G, cuda)
     assert max(X.report.values()) <= 1.0
+
+
+# ---------------------------------------------------------------------------------- decoding
+GPT_HD128 = dict(port.GCFG_TINY, hidden_size=256, ffn_hidden_size=1024, num_attention_heads=2, max_position_embeddings=256)
+# case: (decoder config, clips, beam (0: sample), TokenStep's fused LayerNorms, step program kind)
+DECODE_CASES = {
+    "1p3b_beam5": (GPT_1P3B, 1, 5, False, "skinny"),
+    "1p3b_beam5_fused_ln": (GPT_1P3B, 1, 5, True, "skinny_ln"),
+    "2p7b_12clips_beam5": (GPT_2P7B, 12, 5, False, "skinny"),
+    "1p3b_sample12": (GPT_1P3B, 12, 0, False, "gemm"),
+    "hd128_2clips_beam3": (GPT_HD128, 2, 3, False, "skinny"),
+}
+
+
+def _decoder(cuda, gcfg, Q, n_new):
+    """A 2-layer DistributedGPT3 in eval mode with random LayerNorm parameters and biases (the defaults are 1 and 0)."""
+    from helpers import build_pretrain
+    vcfg = port.VCFG_TINY
+    dec = build_pretrain(vcfg, gcfg, Q, device=cuda, dtype=BF16, cls_name="DistributedGPT3_Caption",
+                         num_frames=vcfg["num_frames"]).eval().text_decoder
+    dec.config.tokens_to_generate, dec.config.top_k, dec.config.top_p = n_new, 1, 0.0
+    g = torch.Generator().manual_seed(4)
+    with torch.no_grad():
+        for k, p in dec.named_parameters():
+            if k.endswith("layernorm.weight"):
+                p.copy_(1.0 + 0.1 * torch.randn(p.shape, generator=g))
+            elif k.endswith("bias"):
+                p.copy_(0.02 * torch.randn(p.shape, generator=g))
+    return dec
+
+
+@pytest.mark.parametrize("case", sorted(DECODE_CASES))
+def test_decode_walks(cuda, monkeypatch, case):
+    """Caption decoding through the public entry points (beam_search of one clip, the batched beam search, sample()),
+    recorded eagerly (YMP_DECODE_GRAPH=0: the recorder synchronises inside every call) with every new cache store
+    poisoned, and walked against decode_session: the prefill into the KV cache, 7 single-token steps (TokenStep's
+    skinny GEMMs, 60 rows on the wide entry point, or gpt_decode's n = 1 step for 12 sampled rows of two prompt
+    lengths), the row table under reindex and share_prefill, and the logits every decode returned.  2-layer decoders
+    at the 1.3B (32 x 64) and 2.7B (32 x 80) widths and at head_dim 128, Q = 128 prefix rows."""
+    import models.modeling_distributed_gpt3 as M
+    from ymp import engine, ops
+    gcfg, C, beam, fused_ln, kind = DECODE_CASES[case]
+    Q, L, n_new = 128, 8, 7
+    H, V = gcfg["hidden_size"], gcfg["vocab_size"]
+    dec = _decoder(cuda, gcfg, Q, n_new)
+    g = torch.Generator().manual_seed(7)
+    qf = (0.5 * torch.randn(C, Q, H, generator=g)).to(cuda, BF16)
+    ids = torch.randint(0, V, (C, L), generator=g).to(cuda)
+    monkeypatch.setenv("YMP_DECODE_GRAPH", "0")
+    monkeypatch.setenv("YMP_DECODE_FUSED_LN", "1" if fused_ln else "0")
+    init = engine.KVCache.__init__
+
+    def poisoned(cache, *a, **k):
+        init(cache, *a, **k)
+        SS.poison_(cache.store)
+    monkeypatch.setattr(engine.KVCache, "__init__", poisoned)
+    rec = SS.Recorder(ops)
+    rec.install(monkeypatch)
+    rec.install_decode(monkeypatch, engine.KVCache, M.DistributedGPT3)
+    with torch.no_grad():
+        if beam == 0:
+            dec.sample(ids, query_embeds=qf, prompt_length=torch.tensor([5, 8] * (C // 2)))
+        else:
+            dec.beam_search(ids, query_embeds=qf, beam_size=beam, stop_token=dec.config.eod_id)
+    torch.cuda.synchronize()
+    monkeypatch.undo()
+    keys, params = dec._param_list()
+    W = {k: pp.detach().to(F64) for k, pp in zip(keys, params)}
+    rows, stride = (C, 1) if beam == 0 else (C * beam, beam if C > 1 else 1)
+    qf_rows = qf if beam == 0 or C > 1 else qf.repeat(beam, 1, 1)
+
+    def run(X):
+        return SS.decode_session(X, W, gcfg, qf_rows.to(F64), B=rows, max_len=L + n_new + Q, stride=stride, kind=kind)
+
+    X, logits = _walk(f"decode.{case}", rec.trace, {}, run, None, cuda)
+    assert len(logits) >= 7 and max(X.report.values()) <= 1.0
+    ops_seen = {r.op for r in rec.trace}
+    assert ("gemm_skinny_wide" if rows > 8 and kind != "gemm" else "gemm_skinny") in ops_seen or kind == "gemm"
+    if beam:
+        reidx = [r.ins["idx"].tolist() for r in rec.trace if r.op == "event" and r.kw["kind"] == "reindex"]
+        assert len(reidx) >= 6
+        # after the first step (every beam continues its clip's first) some step takes two beams from one ancestor
+        assert any(len(set(ix[c * beam:(c + 1) * beam])) < beam for ix in reidx[1:] for c in range(C)), reidx
