@@ -285,6 +285,20 @@ typedef struct ymp_attn_args {
 } ymp_attn_args;
 int ymp_attn_fwd(const ymp_attn_args* a, void* stream);
 
+/* Causal attention with a key prefix per sequence: many texts behind prefixes of different lengths in one launch
+ * (the scoring evaluations share each video's [visual queries | title] rows among its texts).  Sequence s has
+ * n_prefix[s / map_kv.seq_div] keys before its s_q queries, read through map_kv's prefix rows (map_kv.n_prefix is
+ * ignored); its key count is that prefix plus s_q, and query i sits at key position n_prefix[...] + i (causal, bottom-
+ * right aligned per sequence).  Each row is bit-identical to the same row of the square causal call over that
+ * sequence's keys.  attn.mask must be YMP_MASK_CAUSAL; attn.s_kv is an upper bound on every key count (preconditions,
+ * not checked: 0 <= n_prefix[...] <= s_kv - s_q).  Forward only, head_dim 64 / 80 / 88 / 96, no dropout, total_rows,
+ * s_kv_dev or kv_rows; served by the wgmma tiles. */
+typedef struct ymp_attn_prefix_table_args {
+  ymp_attn_args attn;
+  const int32_t* n_prefix;  /* DEVICE table, one key count per prefix: n_seq / map_kv.seq_div entries */
+} ymp_attn_prefix_table_args;
+int ymp_attn_fwd_prefix_table(const ymp_attn_prefix_table_args* a, void* stream);
+
 typedef struct ymp_attn_bwd_args {
   ymp_attn_args fwd;      /* the forward call's arguments (q,k,v,o,lse and maps) */
   const void* dout;       /* bf16, addressed by map_do / lddo / do_head_stride */

@@ -4,14 +4,19 @@ eval calls at the shipped yamls' shapes.
     python tools/eval_prefix.py [--shapes cls_1.3B itm_2.7B ...] [--rounds 3] [--counts]
 
 Each shape builds the yaml's model class with random bf16 weights (eval mode, 128 queries, the yaml's frame count) and
-times one eval model(...) call per arm, the two arms alternating in one process after a warm-up call of each, every
+times one eval model(...) call per arm, the arms alternating in one process after a warm-up call of each, every
 call ending in a device synchronise:
-  repeated - today's composition: every video's query features copied once per text, then _gen_pass / _cls_pass;
-  shared   - model(..., train=False), which scores every text against one copy of its video's prefix.
-Text lengths are set two ways: all 80 tokens, and uniform in [16, 80].  One JSON line per (shape, lengths): card name,
-power limit and max SM clock, median ms per call, peak allocated memory of each arm (of the whole call, and of its
-decoder passes: from the end of the visual prefix, which both arms compute alike), and whether the two arms' outputs
-are bit-equal.  --counts prints the decoder rows and GEMM work counted from shapes, without a GPU.
+  repeated    - every video's query features copied once per text, then _gen_pass / _cls_pass;
+  prefix_only - every text against one copy of its video's prefix, each text's own columns all computed
+                (forward_shared_prefix without shared_cols);
+  shared      - model(..., train=False): one copy of the prefix and of the text columns a video's texts have in common.
+Text shapes: all 80 tokens; uniform lengths in [16, 80]; and (Cls shapes) `titles`: per video a title prompt of
+U[12, 60] tokens, its t class labels of 1-4 tokens and eos, padded to 80, laid out as
+DistributedGPT3Tokenizer._fit_prompt does.  One JSON line per (shape, text shape): card name, power limit and max SM
+clock, median ms per call, peak allocated memory of each arm (of the whole call, and of its decoder passes: from the
+end of the visual prefix, which every arm computes alike), the decoder rows of each arm's generation pass, and whether
+the arms' outputs are bit-equal.  --counts prints the decoder rows and GEMM work counted from shapes, and the rows of
+each arm per text shape, without a GPU.
 """
 import argparse
 import json
@@ -94,6 +99,83 @@ def make_text(n, vocab, lo, seed, prompt):
     return d
 
 
+def make_titles(V, t, vocab, seed, cls):
+    """The `titles` text shape: (text, prompt_text) dicts.  Video v's texts are [bos | title prompt | label | eos] for the
+    t class labels (one class list for every video), prompt_lengths as _fit_prompt sets them; prompt_text is
+    [bos | title prompt | eos], one row per video (Cls) or per pair (ITM)."""
+    import torch
+    g = torch.Generator().manual_seed(seed)
+    labels = [torch.randint(3, vocab, (int(torch.randint(1, 5, (1,), generator=g)),), generator=g).tolist() for _ in range(t)]
+    ids, plen, pids = [], [], []
+    for _ in range(V):
+        prompt = torch.randint(3, vocab, (int(torch.randint(12, 61, (1,), generator=g)),), generator=g).tolist()
+        for lab in labels:
+            pr = prompt[:L - len(lab) - 2] if 2 + len(prompt) + len(lab) > L else prompt
+            ids.append([1] + pr + lab + [2])
+            plen.append(len(pr))
+        pids += [([1] + prompt + [2])[:L]] * (1 if cls == "DistributedGPT3_Cls" else t)
+
+    def pad(rows):
+        return dict(input_ids=torch.tensor([r + [0] * (L - len(r)) for r in rows]),
+                    attention_mask=torch.tensor([[1] * len(r) + [0] * (L - len(r)) for r in rows]))
+    return dict(pad(ids), prompt_lengths=torch.tensor(plen)), pad(pids)
+
+
+def make_texts(name, lengths):
+    """(text, prompt_text) dicts of one text shape (CPU tensors)."""
+    cls, _, _, V, t = SHAPES[name]
+    vocab = gpt_cfg(name)["vocab_size"]
+    if lengths == "titles":
+        return make_titles(V, t, vocab, 2, cls)
+    lo = L if lengths == "all80" else 16
+    n_prompt = V if cls == "DistributedGPT3_Cls" else V * t   # Cls: one cls prompt per video; ITM: one per pair
+    return make_text(V * t, vocab, lo, 2, True), make_text(n_prompt, vocab, lo, 3, False)
+
+
+def text_shapes(name):
+    return ("all80", "uniform16_80") + (("titles",) if SHAPES[name][0] == "DistributedGPT3_Cls" else ())
+
+
+def arm_rows(name, lengths):
+    """Decoder rows of each arm's generation pass at one text shape (the same host arithmetic as the model)."""
+    from models.distributed_gpt3 import build_targets, mask_prompt, shared_text_columns
+    from ymp import functional as YF
+    import torch
+    _, _, _, V, t = SHAPES[name]
+    text, _ = make_texts(name, lengths)
+    _, loss_mask = build_targets(text["input_ids"], mask_prompt(text["attention_mask"][:, 1:].clone(), text["prompt_lengths"]), Q)
+    shared, used = shared_text_columns(text["input_ids"], text["attention_mask"], torch.nn.functional.pad(loss_mask[:, Q:], (0, 1)), V)
+    _, Ls, Pmax = YF.shared_title_layout(V, max(used), shared, used)
+    N = V * t
+    return dict(rows_repeated=N * (Q + L), rows_prefix_only=N * max(used) + V * Q, rows_shared=N * Ls + V * (Q + Pmax),
+                shared_cols_min=min(shared), shared_cols_max=Pmax)
+
+
+def prefix_only_call(model, video, text, prompt_text):
+    """The eval branch with every text against one copy of its video's prefix and all of its own columns computed:
+    forward_shared_prefix without shared_cols, composed as the model's shared passes are."""
+    import torch
+    from models.distributed_gpt3 import build_targets, mask_prompt, used_columns
+    _, _, _, qf = model.visual_prefix(video)
+    V, Q_ = qf.shape[:2]
+    N, Lt = text.input_ids.shape
+    t = N // V
+    dec, wemb = model.text_decoder, model._word_embedding()
+    targets, loss_mask = build_targets(text.input_ids, mask_prompt(text.attention_mask[:, 1:].clone(), text.prompt_lengths), Q_)
+    Le = used_columns(text.attention_mask)
+    out = dec.forward_shared_prefix(qf, wemb(text.input_ids[:, :Le]).to(qf.dtype), labels=targets[:, Q_:Q_ + Le])
+    losses = torch.zeros((N, Q_ + Lt), device=qf.device, dtype=torch.float32)
+    losses[:, Q_:Q_ + Le] = out.losses
+    gen = (-(losses[:, :-1] * loss_mask).sum(dim=-1)).view(V, t)
+    att = prompt_text.attention_mask
+    Lp = used_columns(att)
+    rows = torch.arange(att.shape[0], device=att.device) * Lp + att.sum(dim=-1) - 1
+    cls = model.cls_head(dec.forward_shared_prefix(qf, wemb(prompt_text.input_ids[:, :Lp]).to(qf.dtype), hidden_rows=rows).hidden)
+    if type(model).__name__ == "DistributedGPT3_Cls":
+        return gen.softmax(dim=-1), cls
+    return gen, cls.float().softmax(dim=-1)[:, 1].view(V, t)
+
+
 def repeated_call(model, video, text, prompt_text):
     """The eval branch with every video's query features copied once per text (the composition before the shared pass)."""
     _, _, _, qf = model.visual_prefix(video)
@@ -112,16 +194,14 @@ def run(model, vis, name, rounds, lengths):
     import models.modeling_distributed_gpt3 as G
     dev = torch.device("cuda:0")
     cls, gjson, frames, V, t = SHAPES[name]
-    vocab = gpt_cfg(name)["vocab_size"]
 
     def enc(d):
         return G.BatchEncoding({k: v.to(dev) for k, v in d.items()})
 
     video = torch.randn(V, 3, frames, vis["img_size"], vis["img_size"], generator=torch.Generator().manual_seed(1)).to(dev).bfloat16()
-    lo = L if lengths == "all80" else 16
-    n_prompt = V if cls == "DistributedGPT3_Cls" else V * t   # Cls: one cls prompt per video; ITM: one per pair
-    text, prompt_text = enc(make_text(V * t, vocab, lo, 2, True)), enc(make_text(n_prompt, vocab, lo, 3, False))
+    text, prompt_text = (enc(d) for d in make_texts(name, lengths))
     arms = dict(repeated=lambda: repeated_call(model, video, text, prompt_text),
+                prefix_only=lambda: prefix_only_call(model, video, text, prompt_text),
                 shared=lambda: model(video, text, prompt_text, train=False))
     ms = {a: [] for a in arms}
     peak = {a: 0 for a in arms}
@@ -157,7 +237,7 @@ def run(model, vis, name, rounds, lengths):
                     peak[a] = max(peak[a], vis["peak"] - base, dec - base)
                     dec_peak[a] = max(dec_peak[a], dec - base)
     del model.visual_prefix
-    equal = all(torch.equal(x, y) for x, y in zip(outs["repeated"], outs["shared"]))
+    equal = all(torch.equal(x, y) for a in ("prefix_only", "shared") for x, y in zip(outs["repeated"], outs[a]))
     res = dict(shape=name, lengths=lengths, videos=V, texts_per_video=t, frames=frames, decoder=gjson, **card_info())
     for a in arms:
         res[f"{a}_ms"] = round(statistics.median(ms[a]), 2)
@@ -165,8 +245,10 @@ def run(model, vis, name, rounds, lengths):
         res[f"{a}_peak_gb"] = round(peak[a] / 1e9, 3)
         res[f"{a}_decoder_peak_gb"] = round(dec_peak[a] / 1e9, 3)
     res["speedup"] = round(res["repeated_ms"] / res["shared_ms"], 3)
+    res["speedup_vs_prefix_only"] = round(res["prefix_only_ms"] / res["shared_ms"], 3)
     res["bit_equal"] = bool(equal)
     res["counts"] = counts(name)
+    res["rows"] = arm_rows(name, lengths)
     print(json.dumps(res), flush=True)
     return res
 
@@ -180,13 +262,15 @@ def main():
     if args.counts:
         for s in args.shapes:
             print(json.dumps(dict(shape=s, **counts(s))))
+            for lengths in text_shapes(s):
+                print(json.dumps(dict(shape=s, lengths=lengths, **arm_rows(s, lengths))))
         return
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("eval_prefix.py times the H100 kernels: no CUDA device found")
     for s in args.shapes:
         model, vis = build(s, torch.device("cuda:0"))
-        for lengths in ("all80", "uniform16_80"):
+        for lengths in text_shapes(s):
             run(model, vis, s, args.rounds, lengths)
         del model
         torch.cuda.empty_cache()

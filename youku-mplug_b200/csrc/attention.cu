@@ -10,7 +10,8 @@
 // Optional dropout of the probabilities (Philox, philox.cuh): the forward drops P after the softmax normaliser, the
 // backward regenerates the same bits.  ymp_attn_fwd / ymp_attn_bwd (bottom of the file) dispatch first to
 // attention_small.cu (block-diagonal sequences of <= 16 rows: TimeSformer temporal attention) and to the
-// single-query decoding kernel, and run everything else here.
+// single-query decoding kernel, and run everything else here.  ymp_attn_fwd_prefix_table runs the wgmma forward's
+// TABLE variant: causal with a key prefix per sequence read from a device table.
 //   forward   : CTA = 64 query rows x (seq, head); K/V tiles streamed with cp.async double buffering
 //   backward  : two kernels, no atomics, deterministic -
 //               dQ   kernel: CTA = 64 query rows, streams K/V   (also emits delta = rowsum(dO*O))
@@ -103,6 +104,8 @@ struct AttnKParams {
   long kv_rows_ld;
   DropSpec drop;       // dropout of the probabilities (has_drop): row = (seq*heads + head)*s_q + query, column = key
   int has_drop;
+  const int* n_prefix; // per-prefix key counts (the wgmma forward's TABLE variant): sequence s has n_prefix[s / mkv.seq_div]
+                       // keys before its s_q queries
 };
 
 // keep-or-drop of the two adjacent key columns col, col+1 (col even) of `row`: scale or zero in place
@@ -855,7 +858,9 @@ __device__ __forceinline__ void wg_pv(float (&acc)[D / 8][4], const float (&pm)[
   wgmma_fence_acc(f);
 }
 
-template <int D, int DIO>
+// TABLE: causal with a key prefix per sequence (ymp_attn_fwd_prefix_table): sequence s has qoff = n_prefix[s / seq_div]
+// keys before its s_q queries, the first qoff taken from map_kv's prefix rows; s_kv only bounds the grid.
+template <int D, int DIO, bool TABLE = false>
 __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   constexpr int TB = WgTile<D>::BYTES;
   extern __shared__ uint8_t smem_wg[];
@@ -869,14 +874,22 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   // Query tiles are aligned to the key tiles (the first starts qoff % 64 rows before query 0, those rows are padding),
   // so each row meets the same key tiles, masks and arithmetic as the same row of the square causal call over the
   // whole key range: bit-identical O and lse, and no key tile that is fully masked for a row.
-  const int qoff = p.mask == MASK_CAUSAL ? p.s_kv - p.s_q : 0;
-  const int q0 = blockIdx.x * 64 - (qoff & 63), a0 = q0 + qoff;  // first query row of the tile and its key position
+  int qoff = p.mask == MASK_CAUSAL ? p.s_kv - p.s_q : 0;
+  int q0 = blockIdx.x * 64 - (qoff & 63), a0 = q0 + qoff;  // first query row of the tile and its key position
   griddep_launch();   // (programmatic dependent launch; no-ops for an ordinary launch)
   griddep_wait();
+  if constexpr (TABLE) {  // (read after the wait: the table is an input like q / k / v)
+    qoff = __ldg(p.n_prefix + s / p.mkv.seq_div);
+    q0 = blockIdx.x * 64 - (qoff & 63);
+    a0 = q0 + qoff;
+  }
   int sq, skv;
   eff_len(p, s, sq, skv);
-  if (q0 >= sq) return;
-  const RSeq mkv = resolve(p.mkv, s), mo = resolve(p.mo, s);
+  if constexpr (TABLE) skv = qoff + sq;
+  if (q0 >= sq) return;  // (TABLE: the grid has a tile for every alignment; the surplus ones end here)
+  RSeq mkv = resolve(p.mkv, s);
+  const RSeq mo = resolve(p.mo, s);
+  if constexpr (TABLE) mkv.n_prefix = qoff;
   const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq);
   const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
   int kv_begin;
@@ -1248,6 +1261,15 @@ static int launch_wg_fwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
     return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO>, true>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
   });
 }
+// The per-sequence prefix is only known on the device, so the grid has (s_q + 63 + 63) / 64 query tiles: enough for
+// any lead of 0 .. 63 padding rows.
+static int launch_wg_fwd_table(const AttnKParams& p, int head_dim, cudaStream_t st) {
+  const dim3 grid((p.s_q + 126) / 64, p.n_heads, p.n_seq);
+  return for_head_dim<false>(head_dim, [&](auto hd) {
+    using H = decltype(hd);
+    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO, true>, true>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
+  });
+}
 static int launch_wg_bwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
   return for_head_dim<false>(head_dim, [&](auto hd) {
     using H = decltype(hd);
@@ -1325,6 +1347,25 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   }
   g_attn_path = YMP_ATTN_PATH_MMA_SYNC;
   return launch_fwd(p, a->head_dim, st);
+}
+
+extern "C" int ymp_attn_fwd_prefix_table(const ymp_attn_prefix_table_args* t, void* stream) {
+  using namespace ymp;
+  YMP_CHECK_ARG(t != nullptr, "ymp_attn_fwd_prefix_table: null args");
+  YMP_CHECK_ARG(t->n_prefix != nullptr, "ymp_attn_fwd_prefix_table: null n_prefix table");
+  const ymp_attn_args* a = &t->attn;
+  AttnKParams p = {};
+  int rc = fill_params(a, p, "ymp_attn_fwd_prefix_table");
+  if (rc) return rc;
+  YMP_CHECK_ARG(a->o && aligned16(a->o), "ymp_attn_fwd_prefix_table: bad o");
+  YMP_CHECK_ARG(a->mask == YMP_MASK_CAUSAL, "ymp_attn_fwd_prefix_table: the mask must be causal");
+  YMP_CHECK_ARG(a->head_dim != 128, "ymp_attn_fwd_prefix_table: needs head_dim 64, 80, 88 or 96");
+  YMP_CHECK_ARG(!p.has_drop, "ymp_attn_fwd_prefix_table: takes no dropout");
+  YMP_CHECK_ARG(a->total_rows == 0 && !a->s_kv_dev && !a->kv_rows,
+                "ymp_attn_fwd_prefix_table: takes no total_rows, s_kv_dev or kv_rows");
+  p.n_prefix = t->n_prefix;
+  g_attn_path = YMP_ATTN_PATH_WGMMA;
+  return launch_wg_fwd_table(p, a->head_dim, (cudaStream_t)stream);
 }
 
 extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {

@@ -331,8 +331,10 @@ class _PromptClsBase(_PrefixModelBase):
 
     # The evaluations score t texts per video.  When nothing can need a backward through the decoder and its dropout
     # is off, every video's prefix is computed once for all its texts (DistributedGPT3.forward_shared_prefix) instead
-    # of once per text, and columns past the last one any text attends to are not computed.  The outputs are
-    # bit-identical to the passes above on the repeated prefixes.
+    # of once per text, and columns past the last one any text attends to are not computed.  The leading text columns
+    # that a video's texts have in common up to the first column read (bos and the title prompt of the Cls texts) are
+    # computed once per video too (shared_text_columns).  The outputs are bit-identical to the passes above on the
+    # repeated prefixes.
     def _shared_prefix_ok(self, query_features):
         """True when the eval passes may share the prefixes: no backward can be needed (grad mode off, or neither the
         query features nor any decoder parameter requires grad) and the decoder's dropout is inactive."""
@@ -343,13 +345,15 @@ class _PromptClsBase(_PrefixModelBase):
     def _gen_pass_shared(self, query_features, text):
         """_gen_pass with text n after prefix n // t, prefixes not repeated: (losses [N, Q+L-1] fp32 with +0 in the prefix
         and untouched columns, loss_mask [N, Q+L-1]) - the same values as (out.losses, loss_mask) of _gen_pass."""
-        Q = query_features.shape[1]
+        V, Q = query_features.shape[:2]
         N, L = text.input_ids.shape
         text_loss_atts = mask_prompt(text.attention_mask[:, 1:].clone(), text.prompt_lengths)
         targets, loss_mask = build_targets(text.input_ids, text_loss_atts, Q)
-        Le = used_columns(text.attention_mask)
+        shared, used = shared_text_columns(text.input_ids, text.attention_mask, F.pad(loss_mask[:, Q:], (0, 1)), V)
+        Le = max(used)
         emb = self._word_embedding()(text.input_ids[:, :Le]).to(query_features.dtype)
-        out = self.text_decoder.forward_shared_prefix(query_features, emb, labels=targets[:, Q:Q + Le])
+        out = self.text_decoder.forward_shared_prefix(query_features, emb, labels=targets[:, Q:Q + Le], shared_cols=shared,
+                                                      used_cols=used)
         losses = torch.zeros((N, Q + L), device=out.losses.device, dtype=torch.float32)
         losses[:, Q:Q + Le] = out.losses
         return losses[:, :-1].contiguous(), loss_mask
@@ -357,10 +361,35 @@ class _PromptClsBase(_PrefixModelBase):
     def _cls_pass_shared(self, query_features, prompt_text):
         """_cls_pass (eval) with prompt n after prefix n // t, prefixes not repeated; the LM head is not run."""
         att = prompt_text.attention_mask
-        Le = used_columns(att)
+        last = att.sum(dim=-1) - 1   # the column whose hidden state is read
+        read = torch.arange(att.shape[1], device=att.device)[None, :] == last[:, None]
+        shared, used = shared_text_columns(prompt_text.input_ids, att, read, query_features.shape[0])
+        Le = max(used)
         emb = self._word_embedding()(prompt_text.input_ids[:, :Le]).to(query_features.dtype)
-        rows = torch.arange(att.shape[0], device=att.device) * Le + att.sum(dim=-1) - 1
-        return self.cls_head(self.text_decoder.forward_shared_prefix(query_features, emb, hidden_rows=rows).hidden)
+        rows = torch.arange(att.shape[0], device=att.device) * Le + last
+        return self.cls_head(self.text_decoder.forward_shared_prefix(query_features, emb, hidden_rows=rows,
+                                                                     shared_cols=shared, used_cols=used).hidden)
+
+
+def shared_text_columns(input_ids, attention_mask, read, V):
+    """Per-video text columns of a scoring pass, from one host read: (shared, used), two lists of V ints.
+    input_ids / attention_mask / read [N, L] hold t = N // V texts per video (rows v*t .. v*t + t - 1); read marks the
+    columns whose loss or hidden state the caller reads.
+    used[v]: 1 + the last column any of video v's texts attends to (at least 1), as used_columns.
+    shared[v]: the leading columns all t texts of video v compute identically, so they can be computed once: the
+    smallest of their longest common id prefix, the first column read in any of them and used[v] - 1.  0 when t == 1
+    (one text has nothing to share)."""
+    N, L = input_ids.shape
+    t = N // V
+    ids, att, rd = torch.stack([input_ids, attention_mask.ne(0).long(), read.ne(0).long()]).cpu().view(3, V, t, L).unbind(0)
+    used = (att.any(1) * torch.arange(1, L + 1)).max(-1).values.clamp(min=1)
+    if t == 1:
+        return [0] * V, used.tolist()
+    common = (ids == ids[:, :1]).all(1).long().cumprod(-1).sum(-1)      # longest common prefix of the t rows
+    r = rd.any(1)
+    first_read = torch.where(r.any(-1), r.long().argmax(-1), L)
+    shared = torch.minimum(torch.minimum(common, first_read), used - 1)
+    return shared.tolist(), used.tolist()
 
 
 def used_columns(attention_mask):

@@ -647,10 +647,14 @@ class DistributedGPT3(nn.Module):
         """Does a pass in the current mode draw dropout masks (train() mode and a non-zero probability)?"""
         return YF.gpt_dropout_active(self.config.engine_cfg(self.training))
 
-    def forward_shared_prefix(self, query_embeds, input_embeds, labels=None, hidden_rows=None):
+    def forward_shared_prefix(self, query_embeds, input_embeds, labels=None, hidden_rows=None, shared_cols=None,
+                              used_cols=None):
         """Score N = V*t texts against V visual prefixes without repeating them: text n follows prefix n // t under the
         same plain causal mask as forward() on torch.cat([query_embeds.repeat_interleave(t, 0), input_embeds], 1).
         query_embeds [V,Q,H], input_embeds [N,L,H]; labels [N,L] are the targets of the text positions.
+        shared_cols: per-video count of leading text columns all t texts of the video have in common (a title prompt),
+        computed once per video; used_cols: per-video count of text columns its texts use (default L).  See
+        ymp.functional.gpt_shared_prefix for which columns are then computed; the others read +0.
         Forward only and without dropout (evaluation): returns Dict(losses [N,L] fp32 per-token CE of the text
         positions or None, hidden [len(hidden_rows), H] final hidden states of text rows n*L + j or None), each value
         bit-identical to the matching position of forward() on the repeated layout."""
@@ -658,7 +662,8 @@ class DistributedGPT3(nn.Module):
             raise ValueError("forward_shared_prefix: the decoder's dropout is active (train() mode with p > 0)")
         keys, params = self._param_list()
         losses, hidden = YF.gpt_shared_prefix(query_embeds, input_embeds.to(query_embeds.dtype), labels, hidden_rows,
-                                              self.config.engine_cfg(self.training), keys, params)
+                                              self.config.engine_cfg(self.training), keys, params, shared=shared_cols,
+                                              used=used_cols)
         return AttrDict(losses=losses, hidden=hidden)
 
     # ------------------------------------------------------------------------------------------ generation

@@ -658,28 +658,50 @@ def shared_prefix_maps(V, t, Q, L):
     return ops.dense_map(L), keys, ops.dense_map(Q)
 
 
-def gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, L, out_rows=None):
+def shared_title_maps(V, t, Q, Ls, Pmax):
+    """Sequence maps of gpt_fwd_shared_prefix's attention with shared text columns, over rows [N*Ls suffix rows |
+    V*(Q + Pmax) block rows] (N = V*t, text n in video n // t): (suffix rows of a text, keys of a text = the first
+    Q + P_v rows of its video's block then its own suffix rows, block rows).  The key map's prefix length is not used:
+    the attention call reads it per video from its n_prefix table (Q + P_v)."""
+    N = V * t
+    keys = ops.seqmap(seq_div=t, outer_stride=t * Ls, inner_stride=Ls, pos_stride=1, prefix_base=N * Ls,
+                      prefix_stride=Q + Pmax, prefix_per_seq=0)
+    return ops.dense_map(Ls), keys, ops.dense_map(Q + Pmax)
+
+
+def gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, L, out_rows=None, shared=None):
     """Forward-only decoder pass over V prefixes of Q rows, each followed by t texts of L rows (the scoring evaluations:
     N = V*t sequences [prefix v | text n], v = n // t), without repeating the prefixes.
     x [N*L + V*Q, H] fp32: rows n*L + j are the text embeddings + positions Q + j, rows N*L + v*Q + i the prefix
     embeddings + positions i.  Causal attention lets no prefix row see a text row, so each layer runs its LayerNorms
     and GEMMs once over all rows and attends twice over its packed QKV: square causal over the prefixes, then the text
-    rows causally after their video's prefix (s_q = L < s_kv = Q + L).  Every kernel computes each row on its own, so
-    the text rows are bit-identical to the same rows of gpt_fwd on the repeated [N, Q + L] layout.
+    rows causally after their video's prefix (s_q = L, per-video key prefix Q).  Every kernel computes each row on its
+    own, so the text rows are bit-identical to the same rows of gpt_fwd on the repeated [N, Q + L] layout.
+    shared: per-video counts P_v of leading text columns that all t texts of video v have in common (the title prompt
+    of the Cls evaluation; None: all 0).  Those columns are computed once per video as part of its block, and L is the
+    number of suffix columns per text (Ls).  x [N*L + V*(Q + Pmax), H], Pmax = max P_v:
+      row n*L + j:                    text column P_v + j of text n (position Q + P_v + j);
+      row N*L + v*(Q + Pmax) + i:     prefix row i (i < Q), text column i - Q of video v's texts (position i) up to
+                                      Q + P_v; the Pmax - P_v rows after them are padding that no kept row attends to.
+    The text rows attend to Q + P_v block rows of their video through the per-video prefix table.
     Returns the final-LayerNorm hidden states of out_rows (int32 indices into x's rows; default: all text rows)."""
     g = GptDims(gcfg)
     N, hd = V * t, g.hd
     T = N * L
-    assert x.shape == (T + V * Q, g.H) and x.dtype == torch.float32
-    m_txt, m_keys, m_pre = shared_prefix_maps(V, t, Q, L)
+    shared = [0] * V if shared is None else [int(p) for p in shared]
+    assert len(shared) == V and min(shared) >= 0, shared
+    B = Q + max(shared)   # rows of a video's block
+    assert x.shape == (T + V * B, g.H) and x.dtype == torch.float32
+    m_txt, m_keys, m_blk = shared_title_maps(V, t, Q, L, B - Q)
+    n_prefix = torch.tensor([Q + p for p in shared], dtype=torch.int32, device=x.device)
 
     def attend(qkv, att):
         pq, pa = qkv[T:], att[T:]
-        ops.attn_fwd(*(TView(pq, i * hd, 3 * hd, m_pre) for i in range(3)), TView(pa, 0, hd, m_pre), n_seq=V,
-                     n_heads=g.heads, head_dim=hd, s_q=Q, s_kv=Q, causal=True, scale=g.scale)
+        ops.attn_fwd(*(TView(pq, i * hd, 3 * hd, m_blk) for i in range(3)), TView(pa, 0, hd, m_blk), n_seq=V,
+                     n_heads=g.heads, head_dim=hd, s_q=B, s_kv=B, causal=True, scale=g.scale)
         ops.attn_fwd(TView(qkv, 0, 3 * hd, m_txt), TView(qkv, hd, 3 * hd, m_keys), TView(qkv, 2 * hd, 3 * hd, m_keys),
-                     TView(att, 0, hd, m_txt), n_seq=N, n_heads=g.heads, head_dim=hd, s_q=L, s_kv=Q + L, causal=True,
-                     scale=g.scale)
+                     TView(att, 0, hd, m_txt), n_seq=N, n_heads=g.heads, head_dim=hd, s_q=L, s_kv=B + L, causal=True,
+                     scale=g.scale, n_prefix=n_prefix)
 
     for i in range(g.layers):
         x, _ = gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", x, g, None, None, attend=attend)

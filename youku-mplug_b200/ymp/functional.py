@@ -473,11 +473,37 @@ class GptFn(torch.autograd.Function):
         return (dx.view(B, S, H).to(ctx.in_dtype), None, None, None, None) + store.grads(keys, params)
 
 
-def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, keys, params):
+def shared_title_layout(V, L, shared=None, used=None):
+    """Host-side sizes of gpt_shared_prefix's rows: (P list, Ls, Pmax).  shared: P_v per video (None: all 0), used:
+    Le_v per video, the text columns video v's texts use (None: all L).  Ls = max_v (Le_v - P_v) suffix columns per
+    text."""
+    P = [0] * V if shared is None else [int(p) for p in shared]
+    Le = [L] * V if used is None else [int(u) for u in used]
+    if len(P) != V or len(Le) != V or any(not (0 <= p < u <= L) for p, u in zip(P, Le)):
+        raise ValueError(f"gpt_shared_prefix: need 0 <= shared[v] < used[v] <= {L} for each of {V} videos, "
+                         f"got shared={P} used={Le}")
+    return P, max(u - p for p, u in zip(P, Le)), max(P)
+
+
+def shared_title_rows(p_n, t, Q, L, Ls, Pmax, want):
+    """Rows of engine.gpt_fwd_shared_prefix's x that hold the caller's text rows want = n*L + j (int64 tensor), and
+    whether column j of text n is computed at all (j < P_v + Ls).  p_n: P_v of each text [N]."""
+    n, j = want // L, want % L
+    p = p_n[n]
+    rows = torch.where(j >= p, n * Ls + j - p, p_n.numel() * Ls + (n // t) * (Q + Pmax) + Q + j)
+    return rows, j < p + Ls
+
+
+def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, keys, params, shared=None, used=None):
     """Forward-only decoder pass over [prefix v | text n] for N = V*t texts, text n after prefix v = n // t, with each
     prefix computed once (engine.gpt_fwd_shared_prefix).  query_embeds [V,Q,H], input_embeds [N,L,H] (positions NOT
     yet added, the same dtype chain as GptFn on the concatenation), labels [N,L] of the text positions or None,
     hidden_rows: int tensor of text rows n*L + j whose final hidden states are wanted, or None.
+    shared: per-video count P_v of leading text columns that all t texts of video v have in common (the title prompt of
+    the Cls evaluation), or None.  Those columns are computed once per video, from its first text, after the prefix;
+    each text then computes its columns P_v .. P_v + Ls - 1 (used: per-video count Le_v of columns its texts use,
+    default L; Ls = max_v (Le_v - P_v)).  A text column that is not computed has loss +0 and hidden state +0: those
+    before P_v have no loss (hidden rows there are read from the shared block), those from P_v + Ls on have neither.
     Returns (losses [N,L] fp32 or None, hidden [len(hidden_rows), H] bf16 or None); text position j of sequence n is
     bit-identical to position Q + j of GptFn on the repeated [N, Q+L] layout."""
     _require_cuda(input_embeds, "gpt_shared_prefix")
@@ -488,20 +514,51 @@ def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, key
     N, L, _ = input_embeds.shape
     if V == 0 or N % V:
         raise ValueError(f"gpt_shared_prefix: {N} texts do not split evenly over {V} prefixes")
-    T = N * L
+    t, dev = N // V, input_embeds.device
+    P, Ls, Pmax = shared_title_layout(V, L, shared, used)
+    B, T = Q + Pmax, N * Ls
     pos = W[engine.GPT + "embedding.position_embeddings.weight"]
-    x = torch.empty((T + V * Q, H), device=input_embeds.device, dtype=torch.float32)  # [text rows | prefix rows]
-    x[:T] = (input_embeds.float() + pos[Q:Q + L][None].float()).reshape(T, H)
-    x[T:] = (query_embeds.float() + pos[:Q][None].float()).reshape(V * Q, H)
-    rows = None if hidden_rows is None else hidden_rows.to(device=x.device, dtype=torch.int32).contiguous()
+    p_n = torch.tensor(P, device=dev).repeat_interleave(t)                   # P_v of each text
+    col = p_n[:, None] + torch.arange(Ls, device=dev)[None, :]                # [N, Ls] text column of each suffix row
+    cc = col.clamp(max=L - 1)             # (columns past the text's end: any finite row, computed and never read)
+    n_ix = torch.arange(N, device=dev)[:, None]
+    x = torch.empty((T + V * B, H), device=dev, dtype=torch.float32)  # [suffix rows | blocks (prefix, shared columns)]
+    x[:T] = (input_embeds[n_ix, cc].float() + pos[Q + cc].float()).reshape(T, H)
+    xb = x[T:].view(V, B, H)
+    xb[:, :Q] = query_embeds.float() + pos[:Q][None].float()
+    xb[:, Q:] = input_embeds[::t, :Pmax].float() + pos[Q:B][None].float()   # video v's first text (rows past P_v: padding)
+    complete = all(p + Ls >= L for p in P)   # every text column is computed somewhere
+    rows = keep = None
+    if hidden_rows is not None or labels is None:
+        want = (torch.arange(N * L, device=dev) if hidden_rows is None
+                else hidden_rows.to(device=dev, dtype=torch.long))
+        rows, keep = shared_title_rows(p_n, t, Q, L, Ls, Pmax, want)
+        if complete:
+            keep = None
+        else:
+            rows = torch.where(keep, rows, 0)
+        rows = rows.to(torch.int32).contiguous()
     with torch.no_grad():
-        hid = engine.gpt_fwd_shared_prefix(W, x, gcfg, V, N // V, Q, L, out_rows=None if labels is not None else rows)
+        if labels is None:
+            out_rows = rows
+        elif rows is None:
+            out_rows = None
+        else:   # the LM head's suffix rows, then the wanted hidden rows
+            out_rows = torch.cat([torch.arange(T, device=dev, dtype=torch.int32), rows])
+        hid = engine.gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, Ls, out_rows=out_rows, shared=P)
         losses = hidden = None
         if labels is not None:
-            _, losses, _ = engine.lm_head_fwd(W, hid, labels.contiguous())
-            losses = losses.view(N, L)
+            _, sl, _ = engine.lm_head_fwd(W, hid[:T], labels[n_ix, cc].contiguous())
+            if Pmax == 0 and Ls == L:
+                losses = sl.view(N, L)
+            else:
+                losses = torch.zeros((N, L), device=dev, dtype=torch.float32)
+                ok = col < L
+                losses[n_ix.expand(N, Ls)[ok], col[ok]] = sl.view(N, Ls)[ok]
             if rows is not None:
-                hidden = hid.index_select(0, rows.long())
+                hidden = hid[T:]
         else:
             hidden = hid
+        if hidden is not None and keep is not None:
+            hidden = torch.where(keep[:, None], hidden, torch.zeros((), device=dev, dtype=hidden.dtype))
     return losses, hidden

@@ -88,6 +88,10 @@ class AttnArgs(C.Structure):
     ]
 
 
+class AttnPrefixTableArgs(C.Structure):
+    _fields_ = [("attn", AttnArgs), ("n_prefix", c_vp)]
+
+
 class GemmSkinnyArgs(C.Structure):
     _fields_ = [("x", c_vp), ("w", c_vp), ("bias", c_vp), ("residual", c_vp), ("y", c_vp),
                 ("M", c_i32), ("N", c_i32), ("K", c_i32), ("ldx", c_i32), ("ldw", c_i32), ("ldr", c_i32), ("ldy", c_i32),
@@ -173,6 +177,7 @@ _gemm_skinny_wide = _declare("ymp_gemm_skinny_wide", GemmSkinnyArgs)
 _ln_fwd = _declare("ymp_layernorm_fwd", LayerNormArgs)
 _ln_bwd = _declare("ymp_layernorm_bwd", LayerNormBwdArgs)
 _attn_fwd = _declare("ymp_attn_fwd", AttnArgs)
+_attn_fwd_prefix_table = _declare("ymp_attn_fwd_prefix_table", AttnPrefixTableArgs)
 _attn_bwd = _declare("ymp_attn_bwd", AttnBwdArgs)
 _im2col = _declare("ymp_im2col", Im2colArgs)
 _clip = _declare("ymp_clip_normalize", ClipArgs)

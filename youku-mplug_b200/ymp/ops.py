@@ -278,15 +278,25 @@ def _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, sca
 
 
 def attn_fwd(q, k, v, o, *, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, lse=None, mask_block=0,
-             total_rows=0, drop=None, s_kv_dev=None, kv_rows=None):
+             total_rows=0, drop=None, s_kv_dev=None, kv_rows=None, n_prefix=None):
     """q,k,v,o: TView.  Returns lse [n_seq, n_heads, s_q] fp32.  s_kv_dev: int32 device scalar, only the first
     min(s_kv, s_kv_dev) keys exist (the captured decoding step).  kv_rows: int32 CUDA tensor [n_seq, >= s_kv], key j of
-    sequence s is row kv_rows[s, j] of k's / v's tensor (their seqmap is not used; s_q == 1 only, the decode kernel)."""
+    sequence s is row kv_rows[s, j] of k's / v's tensor (their seqmap is not used; s_q == 1 only, the decode kernel).
+    n_prefix: int32 CUDA tensor [n_seq // k.m.seq_div] of per-prefix key counts (ymp_attn_fwd_prefix_table): causal,
+    sequence s has n_prefix[s // seq_div] keys from k's / v's seqmap prefix rows before its s_q queries; s_kv is an
+    upper bound on n_prefix + s_q (k.m.n_prefix is not used)."""
     if lse is None:
         lse = torch.empty((n_seq, n_heads, s_q), device=q.t.device, dtype=torch.float32)
     a = _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, mask_block, total_rows, drop, s_kv_dev,
                    kv_rows)
-    L.call(L._attn_fwd, a, "ymp_attn_fwd")
+    if n_prefix is None:
+        L.call(L._attn_fwd, a, "ymp_attn_fwd")
+        return lse
+    assert n_prefix.dtype == torch.int32 and n_prefix.is_cuda and n_prefix.is_contiguous(), n_prefix
+    assert n_prefix.numel() == n_seq // max(1, k.m.seq_div), (n_prefix.numel(), n_seq, k.m.seq_div)
+    t = L.AttnPrefixTableArgs()
+    t.attn, t.n_prefix = a, n_prefix.data_ptr()
+    L.call(L._attn_fwd_prefix_table, t, "ymp_attn_fwd_prefix_table")
     return lse
 
 
