@@ -299,6 +299,26 @@ typedef struct ymp_attn_prefix_table_args {
 } ymp_attn_prefix_table_args;
 int ymp_attn_fwd_prefix_table(const ymp_attn_prefix_table_args* a, void* stream);
 
+/* ymp_attn_fwd_prefix_table whose prefix starts with keys from a separate K / V tensor, the prefix cache (a video's
+ * visual-query rows computed once by an earlier call and reused by every text chunk scored against that video).  The
+ * n_prefix[v] keys before sequence s's queries (v = s / map_kv.seq_div) are, in order:
+ *   key j <  n0:           row v * n0 + j of the cache: k_cache[(v * n0 + j) * ld_cache + h * cache_head_stride + d]
+ *                          (v_cache likewise: K and V may share one [rows, 2H] tensor at different column offsets);
+ *   n0 <= j < n_prefix[v]: map_kv's prefix row j - n0 of k / v (none when n_prefix[v] == n0);
+ * then the sequence's own rows, causal.  Tile alignment and key range follow n_prefix[v] as in the table call, so each
+ * row is bit-identical to the same row of that call with the cached rows copied in front of map_kv's prefix rows.
+ * Preconditions, not checked: n0 <= n_prefix[v] <= s_kv - s_q.  Same limits as ymp_attn_fwd_prefix_table. */
+typedef struct ymp_attn_prefix_kv_args {
+  ymp_attn_prefix_table_args table;
+  const void* k_cache;        /* bf16, 16-byte aligned, head offset h * cache_head_stride added by the kernel */
+  const void* v_cache;
+  int32_t ld_cache;           /* elements between consecutive cache rows (multiple of 8) */
+  int32_t cache_head_stride;  /* elements between consecutive heads in a cache row (multiple of 8) */
+  int32_t n0;                 /* cached keys per prefix, >= 0 */
+  int32_t _pad;
+} ymp_attn_prefix_kv_args;
+int ymp_attn_fwd_prefix_kv(const ymp_attn_prefix_kv_args* a, void* stream);
+
 typedef struct ymp_attn_bwd_args {
   ymp_attn_args fwd;      /* the forward call's arguments (q,k,v,o,lse and maps) */
   const void* dout;       /* bf16, addressed by map_do / lddo / do_head_stride */

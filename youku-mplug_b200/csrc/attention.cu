@@ -11,7 +11,8 @@
 // backward regenerates the same bits.  ymp_attn_fwd / ymp_attn_bwd (bottom of the file) dispatch first to
 // attention_small.cu (block-diagonal sequences of <= 16 rows: TimeSformer temporal attention) and to the
 // single-query decoding kernel, and run everything else here.  ymp_attn_fwd_prefix_table runs the wgmma forward's
-// TABLE variant: causal with a key prefix per sequence read from a device table.
+// TABLE variant: causal with a key prefix per sequence read from a device table; ymp_attn_fwd_prefix_kv its CACHE
+// variant, whose prefix starts with rows of a separate K / V tensor (a prefix's keys computed by an earlier call).
 //   forward   : CTA = 64 query rows x (seq, head); K/V tiles streamed with cp.async double buffering
 //   backward  : two kernels, no atomics, deterministic -
 //               dQ   kernel: CTA = 64 query rows, streams K/V   (also emits delta = rowsum(dO*O))
@@ -80,6 +81,16 @@ __device__ __forceinline__ RMat rmat(const __nv_bfloat16* p, const RSeq& r, int 
 __device__ __forceinline__ const __nv_bfloat16* mrow(const RMat& m, int i) {
   return i < m.n_prefix ? m.prefix + (long)i * m.ld : m.base + (long)(i - m.n_prefix) * m.stride;
 }
+// A key or value matrix of the prefix-cache variant (ymp_attn_fwd_prefix_kv): positions [0, n0) are rows of the
+// prefix cache, the later ones positions 0, 1, ... of m.
+struct RMatC {
+  RMat m;
+  const __nv_bfloat16* cache;  // position 0, head offset applied
+  int ldc, n0;
+};
+__device__ __forceinline__ const __nv_bfloat16* mrow(const RMatC& m, int i) {
+  return i < m.n0 ? m.cache + (long)i * m.ldc : mrow(m.m, i - m.n0);
+}
 
 constexpr int MASK_NONE = 0, MASK_CAUSAL = 1, MASK_BLOCK = 2;
 constexpr float LOG2E = 1.4426950408889634f;  // natural log -> the log2 units of the exp2f softmax
@@ -106,6 +117,8 @@ struct AttnKParams {
   int has_drop;
   const int* n_prefix; // per-prefix key counts (the wgmma forward's TABLE variant): sequence s has n_prefix[s / mkv.seq_div]
                        // keys before its s_q queries
+  const __nv_bfloat16 *kc, *vc;  // prefix cache (CACHE variant): key j < n0 of sequence s is row (s / mkv.seq_div) * n0 + j
+  int ldc, hsc, n0;
 };
 
 // keep-or-drop of the two adjacent key columns col, col+1 (col even) of `row`: scale or zero in place
@@ -425,8 +438,9 @@ enum TileLayout {
 };
 // Asynchronously load a [64 x D] bf16 tile: positions r0..r0+63 of the resolved sequence, zero outside [0, n_valid)
 // and in columns DIO..D-1.  rows (the forward's kv_rows table of this sequence, or null): position i is row rows[i] of m.
-template <TileLayout L, int D, int DIO>
-__device__ __forceinline__ void load_tile(void* dst, const RMat& m, int r0, int n_valid, const int* rows = nullptr) {
+// M: RMat, or RMatC for the keys and values of the prefix-cache variant.
+template <TileLayout L, int D, int DIO, class M>
+__device__ __forceinline__ void load_tile(void* dst, const M& m, int r0, int n_valid, const int* rows = nullptr) {
   constexpr int CH = D / 8;
 #pragma unroll
   for (int it = 0; it < (64 * CH + 127) / 128; ++it) {
@@ -858,9 +872,19 @@ __device__ __forceinline__ void wg_pv(float (&acc)[D / 8][4], const float (&pm)[
   wgmma_fence_acc(f);
 }
 
+// The key or value matrix of one (sequence, head) of the forward: m itself, or with CACHE its first n0 positions taken
+// from the prefix cache c.
+template <bool CACHE>
+__device__ __forceinline__ auto with_cache(const RMat& m, const __nv_bfloat16* c, const AttnKParams& p, int s, int h) {
+  if constexpr (CACHE) return RMatC{m, c + (long)(s / p.mkv.seq_div) * p.n0 * p.ldc + h * p.hsc, p.ldc, p.n0};
+  else return m;
+}
+
 // TABLE: causal with a key prefix per sequence (ymp_attn_fwd_prefix_table): sequence s has qoff = n_prefix[s / seq_div]
 // keys before its s_q queries, the first qoff taken from map_kv's prefix rows; s_kv only bounds the grid.
-template <int D, int DIO, bool TABLE = false>
+// CACHE (with TABLE, ymp_attn_fwd_prefix_kv): the first n0 of those qoff keys come from the prefix cache, the other
+// qoff - n0 from map_kv's prefix rows.  The tile alignment and key range still follow qoff alone.
+template <int D, int DIO, bool TABLE = false, bool CACHE = false>
 __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   constexpr int TB = WgTile<D>::BYTES;
   extern __shared__ uint8_t smem_wg[];
@@ -889,9 +913,10 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   if (q0 >= sq) return;  // (TABLE: the grid has a tile for every alignment; the surplus ones end here)
   RSeq mkv = resolve(p.mkv, s);
   const RSeq mo = resolve(p.mo, s);
-  if constexpr (TABLE) mkv.n_prefix = qoff;
+  if constexpr (TABLE) mkv.n_prefix = CACHE ? qoff - p.n0 : qoff;
   const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq);
-  const RMat Mk = rmat(p.k, mkv, p.ldk, h * p.hsk), Mv = rmat(p.v, mkv, p.ldv, h * p.hsv);
+  const auto Mk = with_cache<CACHE>(rmat(p.k, mkv, p.ldk, h * p.hsk), p.kc, p, s, h);
+  const auto Mv = with_cache<CACHE>(rmat(p.v, mkv, p.ldv, h * p.hsv), p.vc, p, s, h);
   int kv_begin;
   const int ntiles = key_tiles<false>(p, a0, sq, skv, kv_begin);
 
@@ -1263,11 +1288,12 @@ static int launch_wg_fwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
 }
 // The per-sequence prefix is only known on the device, so the grid has (s_q + 63 + 63) / 64 query tiles: enough for
 // any lead of 0 .. 63 padding rows.
+template <bool CACHE>
 static int launch_wg_fwd_table(const AttnKParams& p, int head_dim, cudaStream_t st) {
   const dim3 grid((p.s_q + 126) / 64, p.n_heads, p.n_seq);
   return for_head_dim<false>(head_dim, [&](auto hd) {
     using H = decltype(hd);
-    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO, true>, true>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
+    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO, true, CACHE>, true>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
   });
 }
 static int launch_wg_bwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
@@ -1349,23 +1375,47 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   return launch_fwd(p, a->head_dim, st);
 }
 
+// The checks and parameters that ymp_attn_fwd_prefix_table and ymp_attn_fwd_prefix_kv share.
+static int fill_table_params(const ymp_attn_prefix_table_args* t, ymp::AttnKParams& p, const char* who) {
+  using namespace ymp;
+  YMP_CHECK_ARG(t->n_prefix != nullptr, "%s: null n_prefix table", who);
+  const ymp_attn_args* a = &t->attn;
+  int rc = fill_params(a, p, who);
+  if (rc) return rc;
+  YMP_CHECK_ARG(a->o && aligned16(a->o), "%s: bad o", who);
+  YMP_CHECK_ARG(a->mask == YMP_MASK_CAUSAL, "%s: the mask must be causal", who);
+  YMP_CHECK_ARG(a->head_dim != 128, "%s: needs head_dim 64, 80, 88 or 96", who);
+  YMP_CHECK_ARG(!p.has_drop, "%s: takes no dropout", who);
+  YMP_CHECK_ARG(a->total_rows == 0 && !a->s_kv_dev && !a->kv_rows, "%s: takes no total_rows, s_kv_dev or kv_rows", who);
+  p.n_prefix = t->n_prefix;
+  return YMP_OK;
+}
+
 extern "C" int ymp_attn_fwd_prefix_table(const ymp_attn_prefix_table_args* t, void* stream) {
   using namespace ymp;
   YMP_CHECK_ARG(t != nullptr, "ymp_attn_fwd_prefix_table: null args");
-  YMP_CHECK_ARG(t->n_prefix != nullptr, "ymp_attn_fwd_prefix_table: null n_prefix table");
-  const ymp_attn_args* a = &t->attn;
   AttnKParams p = {};
-  int rc = fill_params(a, p, "ymp_attn_fwd_prefix_table");
+  const int rc = fill_table_params(t, p, "ymp_attn_fwd_prefix_table");
   if (rc) return rc;
-  YMP_CHECK_ARG(a->o && aligned16(a->o), "ymp_attn_fwd_prefix_table: bad o");
-  YMP_CHECK_ARG(a->mask == YMP_MASK_CAUSAL, "ymp_attn_fwd_prefix_table: the mask must be causal");
-  YMP_CHECK_ARG(a->head_dim != 128, "ymp_attn_fwd_prefix_table: needs head_dim 64, 80, 88 or 96");
-  YMP_CHECK_ARG(!p.has_drop, "ymp_attn_fwd_prefix_table: takes no dropout");
-  YMP_CHECK_ARG(a->total_rows == 0 && !a->s_kv_dev && !a->kv_rows,
-                "ymp_attn_fwd_prefix_table: takes no total_rows, s_kv_dev or kv_rows");
-  p.n_prefix = t->n_prefix;
   g_attn_path = YMP_ATTN_PATH_WGMMA;
-  return launch_wg_fwd_table(p, a->head_dim, (cudaStream_t)stream);
+  return launch_wg_fwd_table<false>(p, t->attn.head_dim, (cudaStream_t)stream);
+}
+
+extern "C" int ymp_attn_fwd_prefix_kv(const ymp_attn_prefix_kv_args* c, void* stream) {
+  using namespace ymp;
+  YMP_CHECK_ARG(c != nullptr, "ymp_attn_fwd_prefix_kv: null args");
+  AttnKParams p = {};
+  const int rc = fill_table_params(&c->table, p, "ymp_attn_fwd_prefix_kv");
+  if (rc) return rc;
+  YMP_CHECK_ARG(c->k_cache && c->v_cache && aligned16(c->k_cache) && aligned16(c->v_cache),
+                "ymp_attn_fwd_prefix_kv: k_cache / v_cache must be non-null and 16-byte aligned");
+  YMP_CHECK_ARG(c->ld_cache % 8 == 0 && c->cache_head_stride % 8 == 0,
+                "ymp_attn_fwd_prefix_kv: ld_cache and cache_head_stride must be multiples of 8");
+  YMP_CHECK_ARG(c->n0 >= 0, "ymp_attn_fwd_prefix_kv: n0 must be >= 0");
+  p.kc = (const __nv_bfloat16*)c->k_cache; p.vc = (const __nv_bfloat16*)c->v_cache;
+  p.ldc = c->ld_cache; p.hsc = c->cache_head_stride; p.n0 = c->n0;
+  g_attn_path = YMP_ATTN_PATH_WGMMA;
+  return launch_wg_fwd_table<true>(p, c->table.attn.head_dim, (cudaStream_t)stream);
 }
 
 extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {

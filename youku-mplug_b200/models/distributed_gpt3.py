@@ -342,9 +342,44 @@ class _PromptClsBase(_PrefixModelBase):
                                                   or any(p.requires_grad for p in self.text_decoder.parameters()))
         return not needs_grad and not self.text_decoder.dropout_active()
 
-    def _gen_pass_shared(self, query_features, text):
+    # An eval call keeps the prefixes' keys and values of its first pass (a lazy DistributedGPT3.prefix_kv) and its
+    # second pass reads them.
+    # The last clip's query features and PrefixKV are kept, so the text chunks that the ITM evaluation scores against
+    # one clip tensor run neither the visual encoder nor the prefix rows again (prefix_cache_hit is the rule).
+    _prefix_cache = None   # (image, (image._version, weights key), query_features, PrefixKV) or None
+
+    def train(self, mode=True):
+        if mode:
+            self._prefix_cache = None
+        return super().train(mode)
+
+    def _prefix_cache_ok(self, image):
+        """May this call read or create the prefix cache: eval mode, no backward possible, decoder dropout inactive."""
+        needs_grad = torch.is_grad_enabled() and (image.requires_grad or any(p.requires_grad for p in self.parameters()))
+        return not self.training and not needs_grad and not self.text_decoder.dropout_active()
+
+    def _weights_key(self):
+        return sum(p._version for p in self.parameters()), YF.weight_writes()
+
+    def _eval_prefix(self, image):
+        """(query_features, PrefixKV or None) of an eval call: the PrefixKV when the passes may share the prefixes."""
+        ok = self._prefix_cache_ok(image)
+        weights = self._weights_key() if ok else None
+        e = self._prefix_cache
+        if prefix_cache_hit(e, image, weights, ok):
+            return e[2], e[3]
+        if ok:
+            self._prefix_cache = e = None   # (freed before its replacement is built)
+        _, _, _, query_features = self.visual_prefix(image)
+        kv = self.text_decoder.prefix_kv(query_features, lazy=True) if self._shared_prefix_ok(query_features) else None
+        if ok and kv is not None:
+            self._prefix_cache = (image, (image._version, weights), query_features, kv)
+        return query_features, kv
+
+    def _gen_pass_shared(self, query_features, text, prefix_kv=None):
         """_gen_pass with text n after prefix n // t, prefixes not repeated: (losses [N, Q+L-1] fp32 with +0 in the prefix
-        and untouched columns, loss_mask [N, Q+L-1]) - the same values as (out.losses, loss_mask) of _gen_pass."""
+        and untouched columns, loss_mask [N, Q+L-1]) - the same values as (out.losses, loss_mask) of _gen_pass.
+        prefix_kv: the PrefixKV of query_features, or None."""
         V, Q = query_features.shape[:2]
         N, L = text.input_ids.shape
         text_loss_atts = mask_prompt(text.attention_mask[:, 1:].clone(), text.prompt_lengths)
@@ -353,12 +388,12 @@ class _PromptClsBase(_PrefixModelBase):
         Le = max(used)
         emb = self._word_embedding()(text.input_ids[:, :Le]).to(query_features.dtype)
         out = self.text_decoder.forward_shared_prefix(query_features, emb, labels=targets[:, Q:Q + Le], shared_cols=shared,
-                                                      used_cols=used)
+                                                      used_cols=used, prefix_kv=prefix_kv)
         losses = torch.zeros((N, Q + L), device=out.losses.device, dtype=torch.float32)
         losses[:, Q:Q + Le] = out.losses
         return losses[:, :-1].contiguous(), loss_mask
 
-    def _cls_pass_shared(self, query_features, prompt_text):
+    def _cls_pass_shared(self, query_features, prompt_text, prefix_kv=None):
         """_cls_pass (eval) with prompt n after prefix n // t, prefixes not repeated; the LM head is not run."""
         att = prompt_text.attention_mask
         last = att.sum(dim=-1) - 1   # the column whose hidden state is read
@@ -368,7 +403,17 @@ class _PromptClsBase(_PrefixModelBase):
         emb = self._word_embedding()(prompt_text.input_ids[:, :Le]).to(query_features.dtype)
         rows = torch.arange(att.shape[0], device=att.device) * Le + last
         return self.cls_head(self.text_decoder.forward_shared_prefix(query_features, emb, hidden_rows=rows,
-                                                                     shared_cols=shared, used_cols=used).hidden)
+                                                                     shared_cols=shared, used_cols=used,
+                                                                     prefix_kv=prefix_kv).hidden)
+
+
+def prefix_cache_hit(entry, image, weights, ok):
+    """May an eval call reuse the kept (image, (version, weights key), query_features, PrefixKV) entry: the call may
+    use the cache at all (ok: eval mode, no backward, no dropout), the clip is the same tensor object, unchanged in
+    place since (its version counter), and the weights are unchanged (weights: the parameters' summed version counters
+    and the count of optimizer steps and checkpoint loads).  The entry holds the clip tensor itself, so no new batch
+    can be allocated at its address while the entry lives."""
+    return ok and entry is not None and entry[0] is image and entry[1] == (image._version, weights)
 
 
 def shared_text_columns(input_ids, attention_mask, read, V):
@@ -413,19 +458,20 @@ class DistributedGPT3_Cls(_PromptClsBase):
                                           _Linear(self.text_width, self.num_classes))
 
     def forward(self, image, text=None, prompt_text=None, labels=None, train=True):
-        _, _, _, query_features = self.visual_prefix(image)
-        B, Q, _ = query_features.shape
         if train:
+            _, _, _, query_features = self.visual_prefix(image)
             out, _ = self._gen_pass(query_features, text)
             if self.use_cls:
                 loss_cls = F.cross_entropy(self._cls_pass(query_features, prompt_text, True).float(), labels)
             else:
                 loss_cls = out.loss.new_zeros(())
             return out.loss, loss_cls
+        query_features, prefix_kv = self._eval_prefix(image)
+        B, Q, _ = query_features.shape
         num_cls = text.input_ids.shape[0] // B
-        if self._shared_prefix_ok(query_features):
-            losses, loss_mask = self._gen_pass_shared(query_features, text)
-            cls_logits = self._cls_pass_shared(query_features, prompt_text) if self.use_cls else None
+        if prefix_kv is not None:
+            losses, loss_mask = self._gen_pass_shared(query_features, text, prefix_kv)
+            cls_logits = self._cls_pass_shared(query_features, prompt_text, prefix_kv) if self.use_cls else None
         else:
             qf = query_features.unsqueeze(1).repeat(1, num_cls, 1, 1).reshape(B * num_cls, Q, -1)
             out, loss_mask = self._gen_pass(qf, text)
@@ -449,8 +495,8 @@ class DistributedGPT3_Retrieval_Cls(_PromptClsBase):
                                           _Linear(self.text_width, 2))
 
     def forward(self, image, text=None, prompt_text=None, negative_indices=None, labels=None, train=True):
-        _, _, _, query_features = self.visual_prefix(image)
         if train:
+            _, _, _, query_features = self.visual_prefix(image)
             qf = torch.cat([query_features, query_features[negative_indices]], dim=0)
             out, _ = self._gen_pass(qf, text)
             if self.use_cls:
@@ -458,11 +504,12 @@ class DistributedGPT3_Retrieval_Cls(_PromptClsBase):
             else:
                 loss_cls = out.loss.new_zeros(())
             return out.loss, loss_cls
+        query_features, prefix_kv = self._eval_prefix(image)
         V = query_features.shape[0]
         t = text.input_ids.shape[0] // V
-        if self._shared_prefix_ok(query_features):
-            losses, loss_mask = self._gen_pass_shared(query_features, text)
-            cls_pass = partial(self._cls_pass_shared, query_features, prompt_text)
+        if prefix_kv is not None:
+            losses, loss_mask = self._gen_pass_shared(query_features, text, prefix_kv)
+            cls_pass = partial(self._cls_pass_shared, query_features, prompt_text, prefix_kv)
         else:
             qf = query_features.repeat_interleave(t, dim=0)
             out, loss_mask = self._gen_pass(qf, text)

@@ -647,8 +647,22 @@ class DistributedGPT3(nn.Module):
         """Does a pass in the current mode draw dropout masks (train() mode and a non-zero probability)?"""
         return YF.gpt_dropout_active(self.config.engine_cfg(self.training))
 
+    def prefix_kv(self, query_embeds, lazy=False):
+        """Keys and values of the V prefixes query_embeds [V,Q,H] at every decoder layer (ymp.engine.PrefixKV, [layers,
+        V*Q, 2H] bf16): pass it to forward_shared_prefix(prefix_kv=...) with the same query_embeds to score any number
+        of text batches against these prefixes without computing them again.  Forward only and without dropout.
+        lazy: only allocate it; the first forward_shared_prefix that receives it computes the prefixes and fills it."""
+        if self.dropout_active():
+            raise ValueError("prefix_kv: the decoder's dropout is active (train() mode with p > 0)")
+        if lazy:
+            from ymp import engine
+            V, Q, _ = query_embeds.shape
+            return engine.PrefixKV.empty(self.config.engine_cfg(self.training), V, Q, query_embeds.device)
+        keys, params = self._param_list()
+        return YF.gpt_prefix_kv(query_embeds, self.config.engine_cfg(self.training), keys, params)
+
     def forward_shared_prefix(self, query_embeds, input_embeds, labels=None, hidden_rows=None, shared_cols=None,
-                              used_cols=None):
+                              used_cols=None, prefix_kv=None):
         """Score N = V*t texts against V visual prefixes without repeating them: text n follows prefix n // t under the
         same plain causal mask as forward() on torch.cat([query_embeds.repeat_interleave(t, 0), input_embeds], 1).
         query_embeds [V,Q,H], input_embeds [N,L,H]; labels [N,L] are the targets of the text positions.
@@ -657,13 +671,15 @@ class DistributedGPT3(nn.Module):
         ymp.functional.gpt_shared_prefix for which columns are then computed; the others read +0.
         Forward only and without dropout (evaluation): returns Dict(losses [N,L] fp32 per-token CE of the text
         positions or None, hidden [len(hidden_rows), H] final hidden states of text rows n*L + j or None), each value
-        bit-identical to the matching position of forward() on the repeated layout."""
+        bit-identical to the matching position of forward() on the repeated layout.
+        prefix_kv: the handle prefix_kv(query_embeds) returned for these query_embeds; the prefixes are then not
+        computed at all.  A handle whose V, Q, H or layer count differs from the call's is rejected."""
         if self.dropout_active():
             raise ValueError("forward_shared_prefix: the decoder's dropout is active (train() mode with p > 0)")
         keys, params = self._param_list()
         losses, hidden = YF.gpt_shared_prefix(query_embeds, input_embeds.to(query_embeds.dtype), labels, hidden_rows,
                                               self.config.engine_cfg(self.training), keys, params, shared=shared_cols,
-                                              used=used_cols)
+                                              used=used_cols, prefix_kv=prefix_kv)
         return AttrDict(losses=losses, hidden=hidden)
 
     # ------------------------------------------------------------------------------------------ generation

@@ -669,7 +669,62 @@ def shared_title_maps(V, t, Q, Ls, Pmax):
     return ops.dense_map(Ls), keys, ops.dense_map(Q + Pmax)
 
 
-def gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, L, out_rows=None, shared=None):
+def cached_title_maps(V, t, Ls, Pmax):
+    """Sequence maps of gpt_fwd_shared_prefix's attention with a PrefixKV, over rows [N*Ls suffix rows | V*Pmax title
+    rows] (N = V*t, text n in video n // t): (suffix rows of a text, keys of a text after the cached ones = the first
+    P_v title rows of its video then its own suffix rows, title rows).  The key map's prefix length is not used: the
+    attention call reads it per video from its n_prefix table (Q + P_v, of which Q come from the cache)."""
+    N = V * t
+    keys = ops.seqmap(seq_div=t, outer_stride=t * Ls, inner_stride=Ls, pos_stride=1, prefix_base=N * Ls,
+                      prefix_stride=Pmax, prefix_per_seq=0)
+    return ops.dense_map(Ls), keys, ops.dense_map(Pmax)
+
+
+class PrefixKV:
+    """Keys and values of V visual prefixes of Q rows at every decoder layer (gpt_prefix_kv): kv [layers, V*Q, 2H] bf16,
+    row v*Q + i of layer l holds prefix row i of video v, each head's [k | v] columns side by side (head stride 2*hd).
+    A later gpt_fwd_shared_prefix reads them instead of computing the prefix rows again.  filled=False (empty()): the
+    first gpt_fwd_shared_prefix that receives the handle computes the prefix rows as without one and fills it, so the
+    passes of one call share the prefixes without a pass of their own."""
+
+    def __init__(self, kv, V, Q, filled=True):
+        self.kv, self.V, self.Q, self.filled = kv, V, Q, filled
+        self.layers, self.H = kv.shape[0], kv.shape[2] // 2
+
+    @staticmethod
+    def empty(gcfg, V, Q, device):
+        g = GptDims(gcfg)
+        return PrefixKV(torch.empty((g.layers, V * Q, 2 * g.H), device=device, dtype=bf16), V, Q, filled=False)
+
+    def views(self, li, hd):
+        """(kc, vc) TViews of layer li's cache for ops.attn_fwd(cache=...)."""
+        return ops.TView(self.kv[li], 0, 2 * hd, None), ops.TView(self.kv[li], hd, 2 * hd, None)
+
+
+def gpt_prefix_kv(W, query_embeds, gcfg):
+    """Run V visual prefixes (query_embeds [V, Q, H], positions 0 .. Q-1) through the decoder layers and keep every
+    layer's keys and values: a PrefixKV.  Square causal attention per prefix; no final LayerNorm and no LM head.  Each
+    kernel computes a row on its own, so the cached rows are bit-identical to the prefix rows of gpt_fwd_shared_prefix
+    and of gpt_fwd on [prefix | text] sequences."""
+    g = GptDims(gcfg)
+    V, Q, H = query_embeds.shape
+    pos = W[GPT + "embedding.position_embeddings.weight"]
+    x = (query_embeds.float() + pos[:Q][None].float()).reshape(V * Q, H)
+    kv = torch.empty((g.layers, V * Q, 2 * H), device=x.device, dtype=bf16)
+    m = ops.dense_map(Q)
+
+    def attend(qkv, att, li):
+        kv[li].view(V * Q, g.heads, 2, g.hd).copy_(qkv.view(V * Q, g.heads, 3, g.hd)[:, :, 1:])
+        ops.attn_fwd(*(TView(qkv, j * g.hd, 3 * g.hd, m) for j in range(3)), TView(att, 0, g.hd, m), n_seq=V,
+                     n_heads=g.heads, head_dim=g.hd, s_q=Q, s_kv=Q, causal=True, scale=g.scale)
+
+    for i in range(g.layers):   # (the last layer's output is not needed, only its keys and values)
+        x, _ = gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", x, g, None, None, compute_out=i + 1 < g.layers,
+                             attend=lambda qkv, att, i=i: attend(qkv, att, i))
+    return PrefixKV(kv, V, Q)
+
+
+def gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, L, out_rows=None, shared=None, prefix_kv=None):
     """Forward-only decoder pass over V prefixes of Q rows, each followed by t texts of L rows (the scoring evaluations:
     N = V*t sequences [prefix v | text n], v = n // t), without repeating the prefixes.
     x [N*L + V*Q, H] fp32: rows n*L + j are the text embeddings + positions Q + j, rows N*L + v*Q + i the prefix
@@ -684,27 +739,54 @@ def gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, L, out_rows=None, shared=None):
       row N*L + v*(Q + Pmax) + i:     prefix row i (i < Q), text column i - Q of video v's texts (position i) up to
                                       Q + P_v; the Pmax - P_v rows after them are padding that no kept row attends to.
     The text rows attend to Q + P_v block rows of their video through the per-video prefix table.
+    prefix_kv: a PrefixKV of the same V prefixes (gpt_prefix_kv).  No prefix row is computed then, and x holds only
+    [N*L suffix rows | V*Pmax title rows]: row N*L + v*Pmax + i is text column i of video v's texts (position Q + i);
+    the title rows attend to their video's Q cached keys, then causally to each other, and the text rows to the Q
+    cached keys, their video's P_v title rows, then their own rows.  Every row stays bit-identical.  An unfilled
+    prefix_kv (PrefixKV.empty) takes the layout without one; the pass fills it with its prefix rows' keys and values.
     Returns the final-LayerNorm hidden states of out_rows (int32 indices into x's rows; default: all text rows)."""
     g = GptDims(gcfg)
     N, hd = V * t, g.hd
     T = N * L
     shared = [0] * V if shared is None else [int(p) for p in shared]
     assert len(shared) == V and min(shared) >= 0, shared
-    B = Q + max(shared)   # rows of a video's block
+    Pmax = max(shared)
+    if prefix_kv is not None:
+        assert (prefix_kv.V, prefix_kv.Q, prefix_kv.H, prefix_kv.layers) == (V, Q, g.H, g.layers), "PrefixKV shape"
+    cached = prefix_kv is not None and prefix_kv.filled
+    fill = prefix_kv is not None and not cached
+    B = Pmax if cached else Q + Pmax   # rows of a video's block
     assert x.shape == (T + V * B, g.H) and x.dtype == torch.float32
-    m_txt, m_keys, m_blk = shared_title_maps(V, t, Q, L, B - Q)
     n_prefix = torch.tensor([Q + p for p in shared], dtype=torch.int32, device=x.device)
+    if not cached:
+        m_txt, m_keys, m_blk = shared_title_maps(V, t, Q, L, Pmax)
+    else:
+        m_txt, m_keys, m_blk = cached_title_maps(V, t, L, Pmax)
+        n_title = torch.full((V,), Q, dtype=torch.int32, device=x.device)
 
-    def attend(qkv, att):
+    def attend(qkv, att, li):
         pq, pa = qkv[T:], att[T:]
-        ops.attn_fwd(*(TView(pq, i * hd, 3 * hd, m_blk) for i in range(3)), TView(pa, 0, hd, m_blk), n_seq=V,
-                     n_heads=g.heads, head_dim=hd, s_q=B, s_kv=B, causal=True, scale=g.scale)
+        cache = None
+        if not cached:
+            ops.attn_fwd(*(TView(pq, i * hd, 3 * hd, m_blk) for i in range(3)), TView(pa, 0, hd, m_blk), n_seq=V,
+                         n_heads=g.heads, head_dim=hd, s_q=B, s_kv=B, causal=True, scale=g.scale)
+            if fill:
+                prefix_kv.kv[li].view(V, Q, g.heads, 2, hd).copy_(pq.view(V, B, g.heads, 3, hd)[:, :Q, :, 1:])
+        else:
+            cache = (*prefix_kv.views(li, hd), Q)
+            if Pmax:
+                ops.attn_fwd(*(TView(pq, i * hd, 3 * hd, m_blk) for i in range(3)), TView(pa, 0, hd, m_blk), n_seq=V,
+                             n_heads=g.heads, head_dim=hd, s_q=Pmax, s_kv=Q + Pmax, causal=True, scale=g.scale,
+                             n_prefix=n_title, cache=cache)
         ops.attn_fwd(TView(qkv, 0, 3 * hd, m_txt), TView(qkv, hd, 3 * hd, m_keys), TView(qkv, 2 * hd, 3 * hd, m_keys),
-                     TView(att, 0, hd, m_txt), n_seq=N, n_heads=g.heads, head_dim=hd, s_q=L, s_kv=B + L, causal=True,
-                     scale=g.scale, n_prefix=n_prefix)
+                     TView(att, 0, hd, m_txt), n_seq=N, n_heads=g.heads, head_dim=hd, s_q=L, s_kv=Q + Pmax + L,
+                     causal=True, scale=g.scale, n_prefix=n_prefix, cache=cache)
 
     for i in range(g.layers):
-        x, _ = gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", x, g, None, None, attend=attend)
+        x, _ = gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", x, g, None, None,
+                             attend=lambda qkv, att, i=i: attend(qkv, att, i))
+    if fill:
+        prefix_kv.filled = True
     if out_rows is None:
         out_rows = torch.arange(T, device=x.device, dtype=torch.int32)
     hid, _, _ = ops.layernorm_fwd(x, W[GPT + "encoder.final_layernorm.weight"], W[GPT + "encoder.final_layernorm.bias"], g.eps,

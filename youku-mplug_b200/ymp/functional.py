@@ -128,6 +128,21 @@ def gpt_drop(gcfg, dev):
     return engine.GptDrop(_pass_rng(dev), ph, pa)
 
 
+# Writes to the model weights that the parameters' autograd version counters do not see: the fused AdamW writes the
+# bf16 parameters through raw pointers.  TrainEngine bumps this count on every optimizer step and checkpoint load, and
+# state derived from the weights (the evaluation's prefix cache) keys on it.
+_weight_writes = 0
+
+
+def note_weight_write():
+    global _weight_writes
+    _weight_writes += 1
+
+
+def weight_writes():
+    return _weight_writes
+
+
 def gpt_dropout_active(gcfg):
     """Would gpt_drop draw masks for a pass with this config (without drawing them)?"""
     return bool(gcfg.get("training", False)) and (float(gcfg.get("hidden_dropout", 0.0) or 0.0) > 0.0
@@ -494,7 +509,28 @@ def shared_title_rows(p_n, t, Q, L, Ls, Pmax, want):
     return rows, j < p + Ls
 
 
-def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, keys, params, shared=None, used=None):
+def cached_title_rows(p_n, t, L, Ls, Pmax, want):
+    """shared_title_rows for the layout of a pass with a PrefixKV, [N*Ls suffix rows | V*Pmax title rows]: the rows of
+    x that hold the caller's text rows want = n*L + j, and whether column j of text n is computed at all."""
+    n, j = want // L, want % L
+    p = p_n[n]
+    rows = torch.where(j >= p, n * Ls + j - p, p_n.numel() * Ls + (n // t) * Pmax + j)
+    return rows, j < p + Ls
+
+
+def gpt_prefix_kv(query_embeds, gcfg, keys, params):
+    """engine.gpt_prefix_kv on the decoder parameters: the keys and values of the V prefixes query_embeds [V,Q,H] at
+    every layer, for later gpt_shared_prefix(prefix_kv=...) calls on the same prefixes.  Forward only, no dropout."""
+    _require_cuda(query_embeds, "gpt_prefix_kv")
+    if gpt_dropout_active(gcfg):
+        raise ValueError("gpt_prefix_kv: the decoder's dropout is active; the prefix cache is for evaluation")
+    W = {k: as_bf16(p) for k, p in zip(keys, params)}
+    with torch.no_grad():
+        return engine.gpt_prefix_kv(W, query_embeds, gcfg)
+
+
+def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, keys, params, shared=None, used=None,
+                      prefix_kv=None):
     """Forward-only decoder pass over [prefix v | text n] for N = V*t texts, text n after prefix v = n // t, with each
     prefix computed once (engine.gpt_fwd_shared_prefix).  query_embeds [V,Q,H], input_embeds [N,L,H] (positions NOT
     yet added, the same dtype chain as GptFn on the concatenation), labels [N,L] of the text positions or None,
@@ -505,7 +541,10 @@ def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, key
     default L; Ls = max_v (Le_v - P_v)).  A text column that is not computed has loss +0 and hidden state +0: those
     before P_v have no loss (hidden rows there are read from the shared block), those from P_v + Ls on have neither.
     Returns (losses [N,L] fp32 or None, hidden [len(hidden_rows), H] bf16 or None); text position j of sequence n is
-    bit-identical to position Q + j of GptFn on the repeated [N, Q+L] layout."""
+    bit-identical to position Q + j of GptFn on the repeated [N, Q+L] layout.
+    prefix_kv: the PrefixKV of these query_embeds (gpt_prefix_kv), or None.  With it, no prefix row is computed and the
+    values stay bit-identical; query_embeds then only give V, Q and H.  An unfilled one (PrefixKV.empty) is filled by
+    this pass, which computes the prefix rows as without it."""
     _require_cuda(input_embeds, "gpt_shared_prefix")
     if gpt_dropout_active(gcfg):
         raise ValueError("gpt_shared_prefix: the decoder's dropout is active; the shared-prefix pass is for evaluation")
@@ -514,9 +553,15 @@ def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, key
     N, L, _ = input_embeds.shape
     if V == 0 or N % V:
         raise ValueError(f"gpt_shared_prefix: {N} texts do not split evenly over {V} prefixes")
+    if prefix_kv is not None:
+        got, want_ = (prefix_kv.V, prefix_kv.Q, prefix_kv.H, prefix_kv.layers), (V, Q, H, gcfg["num_hidden_layers"])
+        if got != want_:
+            raise ValueError(f"gpt_shared_prefix: the PrefixKV holds (V, Q, H, layers) = {got}, the call needs {want_}")
     t, dev = N // V, input_embeds.device
     P, Ls, Pmax = shared_title_layout(V, L, shared, used)
-    B, T = Q + Pmax, N * Ls
+    T = N * Ls
+    cached = prefix_kv is not None and prefix_kv.filled
+    B = Pmax if cached else Q + Pmax   # block rows per video: [prefix | title] or [title]
     pos = W[engine.GPT + "embedding.position_embeddings.weight"]
     p_n = torch.tensor(P, device=dev).repeat_interleave(t)                   # P_v of each text
     col = p_n[:, None] + torch.arange(Ls, device=dev)[None, :]                # [N, Ls] text column of each suffix row
@@ -525,14 +570,16 @@ def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, key
     x = torch.empty((T + V * B, H), device=dev, dtype=torch.float32)  # [suffix rows | blocks (prefix, shared columns)]
     x[:T] = (input_embeds[n_ix, cc].float() + pos[Q + cc].float()).reshape(T, H)
     xb = x[T:].view(V, B, H)
-    xb[:, :Q] = query_embeds.float() + pos[:Q][None].float()
-    xb[:, Q:] = input_embeds[::t, :Pmax].float() + pos[Q:B][None].float()   # video v's first text (rows past P_v: padding)
+    if not cached:
+        xb[:, :Q] = query_embeds.float() + pos[:Q][None].float()
+    xb[:, B - Pmax:] = input_embeds[::t, :Pmax].float() + pos[Q:Q + Pmax][None].float()   # video v's first text (rows past P_v: padding)
     complete = all(p + Ls >= L for p in P)   # every text column is computed somewhere
     rows = keep = None
     if hidden_rows is not None or labels is None:
         want = (torch.arange(N * L, device=dev) if hidden_rows is None
                 else hidden_rows.to(device=dev, dtype=torch.long))
-        rows, keep = shared_title_rows(p_n, t, Q, L, Ls, Pmax, want)
+        rows, keep = (cached_title_rows(p_n, t, L, Ls, Pmax, want) if cached
+                      else shared_title_rows(p_n, t, Q, L, Ls, Pmax, want))
         if complete:
             keep = None
         else:
@@ -545,7 +592,7 @@ def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, key
             out_rows = None
         else:   # the LM head's suffix rows, then the wanted hidden rows
             out_rows = torch.cat([torch.arange(T, device=dev, dtype=torch.int32), rows])
-        hid = engine.gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, Ls, out_rows=out_rows, shared=P)
+        hid = engine.gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, Ls, out_rows=out_rows, shared=P, prefix_kv=prefix_kv)
         losses = hidden = None
         if labels is not None:
             _, sl, _ = engine.lm_head_fwd(W, hid[:T], labels[n_ix, cc].contiguous())

@@ -92,6 +92,11 @@ class AttnPrefixTableArgs(C.Structure):
     _fields_ = [("attn", AttnArgs), ("n_prefix", c_vp)]
 
 
+class AttnPrefixKvArgs(C.Structure):
+    _fields_ = [("table", AttnPrefixTableArgs), ("k_cache", c_vp), ("v_cache", c_vp), ("ld_cache", c_i32),
+                ("cache_head_stride", c_i32), ("n0", c_i32), ("_pad", c_i32)]
+
+
 class GemmSkinnyArgs(C.Structure):
     _fields_ = [("x", c_vp), ("w", c_vp), ("bias", c_vp), ("residual", c_vp), ("y", c_vp),
                 ("M", c_i32), ("N", c_i32), ("K", c_i32), ("ldx", c_i32), ("ldw", c_i32), ("ldr", c_i32), ("ldy", c_i32),
@@ -178,6 +183,7 @@ _ln_fwd = _declare("ymp_layernorm_fwd", LayerNormArgs)
 _ln_bwd = _declare("ymp_layernorm_bwd", LayerNormBwdArgs)
 _attn_fwd = _declare("ymp_attn_fwd", AttnArgs)
 _attn_fwd_prefix_table = _declare("ymp_attn_fwd_prefix_table", AttnPrefixTableArgs)
+_attn_fwd_prefix_kv = _declare("ymp_attn_fwd_prefix_kv", AttnPrefixKvArgs)
 _attn_bwd = _declare("ymp_attn_bwd", AttnBwdArgs)
 _im2col = _declare("ymp_im2col", Im2colArgs)
 _clip = _declare("ymp_clip_normalize", ClipArgs)

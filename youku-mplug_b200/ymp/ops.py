@@ -278,13 +278,16 @@ def _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, sca
 
 
 def attn_fwd(q, k, v, o, *, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, lse=None, mask_block=0,
-             total_rows=0, drop=None, s_kv_dev=None, kv_rows=None, n_prefix=None):
+             total_rows=0, drop=None, s_kv_dev=None, kv_rows=None, n_prefix=None, cache=None):
     """q,k,v,o: TView.  Returns lse [n_seq, n_heads, s_q] fp32.  s_kv_dev: int32 device scalar, only the first
     min(s_kv, s_kv_dev) keys exist (the captured decoding step).  kv_rows: int32 CUDA tensor [n_seq, >= s_kv], key j of
     sequence s is row kv_rows[s, j] of k's / v's tensor (their seqmap is not used; s_q == 1 only, the decode kernel).
     n_prefix: int32 CUDA tensor [n_seq // k.m.seq_div] of per-prefix key counts (ymp_attn_fwd_prefix_table): causal,
     sequence s has n_prefix[s // seq_div] keys from k's / v's seqmap prefix rows before its s_q queries; s_kv is an
-    upper bound on n_prefix + s_q (k.m.n_prefix is not used)."""
+    upper bound on n_prefix + s_q (k.m.n_prefix is not used).
+    cache (with n_prefix): (kc, vc, n0), TViews of the prefix cache (their seqmaps are not used) and its keys per prefix
+    (ymp_attn_fwd_prefix_kv): the first n0 of sequence s's n_prefix keys are rows (s // seq_div) * n0 + j of kc / vc,
+    the other n_prefix - n0 are k's / v's seqmap prefix rows."""
     if lse is None:
         lse = torch.empty((n_seq, n_heads, s_q), device=q.t.device, dtype=torch.float32)
     a = _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, mask_block, total_rows, drop, s_kv_dev,
@@ -296,7 +299,15 @@ def attn_fwd(q, k, v, o, *, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, 
     assert n_prefix.numel() == n_seq // max(1, k.m.seq_div), (n_prefix.numel(), n_seq, k.m.seq_div)
     t = L.AttnPrefixTableArgs()
     t.attn, t.n_prefix = a, n_prefix.data_ptr()
-    L.call(L._attn_fwd_prefix_table, t, "ymp_attn_fwd_prefix_table")
+    if cache is None:
+        L.call(L._attn_fwd_prefix_table, t, "ymp_attn_fwd_prefix_table")
+        return lse
+    kc, vc, n0 = cache
+    assert kc.ld == vc.ld and kc.hs == vc.hs, "kc and vc need one row stride and one head stride"
+    c = L.AttnPrefixKvArgs()
+    c.table, c.k_cache, c.v_cache = t, kc.p, vc.p
+    c.ld_cache, c.cache_head_stride, c.n0 = kc.ld, kc.hs, n0
+    L.call(L._attn_fwd_prefix_kv, c, "ymp_attn_fwd_prefix_kv")
     return lse
 
 

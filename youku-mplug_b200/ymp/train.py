@@ -128,6 +128,7 @@ class TrainEngine:
             groups.append(dict(params=g["params"], weight_decay=g.get("weight_decay", weight_decay),
                                lr_scale=g.get("lr_scale", 1.0), lr=lr * g.get("lr_scale", 1.0), betas=list(betas),
                                eps=eps, _range=(start, off)))
+        YF.note_weight_write()   # the parameters now live in flat_param (in this dtype)
         self.exp_avg = torch.zeros_like(self.master)
         self.exp_avg_sq = torch.zeros_like(self.master)
         self._sumsq = torch.zeros(1, device=dev, dtype=torch.float32)
@@ -232,6 +233,7 @@ class TrainEngine:
                       self.exp_avg_sq[a:b], step=self.global_steps, lr=g["lr"], beta1=g["betas"][0], beta2=g["betas"][1],
                       eps=g["eps"], weight_decay=g["weight_decay"], grad_scale=scale,
                       max_grad_norm=self.clip_grad or 0.0, sumsq_t=self._sumsq if self.clip_grad else None, zero_grad=True)
+        YF.note_weight_write()
         self.optimizer._global_grad_norm = _LazyNorm(self._sumsq.clone(), scale)
         # every group range was reset by its AdamW pass (the ranges tile the flat buffer)
 
@@ -309,6 +311,7 @@ class TrainEngine:
         self.exp_avg.copy_(ck["exp_avg"])
         self.exp_avg_sq.copy_(ck["exp_avg_sq"])
         self.global_steps = ck["global_steps"]
+        YF.note_weight_write()
         return load_dir, ck.get("client_state", {})
 
 
