@@ -39,6 +39,15 @@ uint64_t ymp_launch_count(void);
  * mma.sync ymp_attn_fwd (the single-token decoding step): each of those kernels may then start while its predecessor in
  * the stream drains (it waits on the device before reading the predecessor's output).  Returns the previous setting. */
 int ymp_set_pdl(int on);
+/* Deterministic mode (process-wide; off by default): every order-dependent sum of the library - the split-K GEMM, the
+ * gamma / beta gradients of ymp_layernorm_bwd, ymp_colsum and ymp_sumsq - then combines its per-CTA partial sums in an
+ * order fixed by the partial's index instead of by fp32 atomics in arrival order: each partial is stored to a workspace
+ * and the destination becomes ((D + P0) + P1) + ..., so equal inputs give bit-identical outputs on the same GPU model.
+ * Grids and split plans are those of the mode off.  The mode is read when a call is launched (a captured CUDA graph
+ * keeps the mode it was captured under).  Those calls then need a device workspace of the size their
+ * ymp_*_workspace_size function returns (0: none; the sizes are 0 whenever the mode is off), passed to the *_ws entry
+ * point; the plain entry points reject a call that needs one.  Returns the previous setting. */
+int ymp_set_deterministic(int on);
 
 /* ------------------------------------------------------------------------------------------
  * Dropout of the GPT-3 decoder (the reference keeps the frozen decoder in train() mode, so
@@ -87,7 +96,8 @@ typedef struct ymp_dropout_spec {
  *                                          so the backward epilogue needs no transcendental)
  *   if drop:    v = dropout(v)           (row = m, column = n; bias-dropout-add: residual + dropout(x + bias))
  *   v += residual[m,n]                   (bf16 or fp32 [M,N], row stride ldr, optional)
- *   D[m,n] = v  (bf16 or fp32) ; or atomically D[m,n] += v (fp32, accumulate=1, used by split-K)
+ *   D[m,n] = v  (bf16 or fp32) ; or atomically D[m,n] += v (fp32, accumulate=1, used by split-K; in the deterministic
+ *   mode the K slices are added in slice order instead, see ymp_gemm_ws)
  *   accumulate=1 allows alpha only: no bias, act, aux_out, aux_in or residual (each K-split adds its own partial
  *   product to D, so a bias would be counted once per split; the library picks the split when split_k = 0)
  * ------------------------------------------------------------------------------------------ */
@@ -135,6 +145,12 @@ int ymp_gemm(const ymp_gemm_args* a, void* stream);
 /* ymp_gemm with the tile height chosen by the caller: tile_m = 0 (auto: what ymp_gemm does), 128 or 192.  192-row tiles
  * need the 256-column tile (tile_n = 0, 256 or 512) and no fused im2col operand; other combinations are rejected. */
 int ymp_gemm_tiled(const ymp_gemm_args* a, int tile_m, void* stream);
+/* Deterministic mode (ymp_set_deterministic): bytes of workspace ymp_gemm_ws needs for this call, split * M * ldd fp32
+ * partials when the plan splits K, else 0 (negative: a YMP_E* code).  ymp_gemm_ws: ymp_gemm_tiled with that workspace
+ * (16-byte aligned; NULL when the size is 0).  Slice k of K (k-blocks [k, k + 1) * kb_per_split) stores alpha times its
+ * product to the workspace, then D = ((D + P0) + P1) + ...; d_row_block is not taken then. */
+int64_t ymp_gemm_workspace_size(const ymp_gemm_args* a, int tile_m);
+int ymp_gemm_ws(const ymp_gemm_args* a, int tile_m, void* workspace, void* stream);
 
 /* Skinny GEMM for single-token decoding (KV-cache steps of sample() / beam_search(),
  * models/modeling_distributed_gpt3.py:1620-1886): y[M, N] = epilogue(x[M, K] . w[N, K]^T).  One pass over the weights on
@@ -215,6 +231,9 @@ typedef struct ymp_layernorm_bwd_args {
 /* Rows are read and written in 16-byte vectors: dy, x, gamma, dx, add, dx_drop, dgamma and dbeta must be 16-byte
  * aligned, and ldx, lddy, ldadd must be multiples of 8 and >= D (YMP_EINVAL otherwise). */
 int ymp_layernorm_bwd(const ymp_layernorm_bwd_args* a, void* stream);
+/* Deterministic mode: blocks * 2 * D fp32 partials of dgamma / dbeta (0 without them); ymp_layernorm_bwd with it. */
+int64_t ymp_layernorm_bwd_workspace_size(const ymp_layernorm_bwd_args* a);
+int ymp_layernorm_bwd_ws(const ymp_layernorm_bwd_args* a, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Fused attention: O = softmax(scale * Q K^T [causal]) V, scores never materialised.
@@ -425,6 +444,9 @@ typedef struct ymp_colsum_args {
   int32_t R, C, ld;
 } ymp_colsum_args;
 int ymp_colsum(const ymp_colsum_args* a, void* stream);
+/* Deterministic mode: one fp32 row of partial column sums per row split; ymp_colsum with it. */
+int64_t ymp_colsum_workspace_size(const ymp_colsum_args* a);
+int ymp_colsum_ws(const ymp_colsum_args* a, void* workspace, void* stream);
 
 /* broadcast=0: out[g,:] = scale * sum_t in[g,t,:]   (cls mean over frames, vision_transformer.py:262)
  * broadcast=1: out[g,t,:] = scale * in[g,:]          (its backward) */
@@ -441,12 +463,15 @@ int ymp_group_reduce(const ymp_group_args* a, void* stream);
  * Optimizer step on flat buffers (next row N1 of SURVEY.md section 8f; needed so that the timed
  * training step skips no work).  Replaces DeepSpeed FusedAdam(adam_w_mode) + global-norm clipping
  * (reference utils.py:490-526; invoked by model.step(), run_pretrain_distributed_gpt3.py:137).
- *   ymp_sumsq : *out += sum(g[i]^2)            (fp32, atomics; the caller zeroes *out)
+ *   ymp_sumsq : *out += sum(g[i]^2)            (fp32, atomics or fixed order; the caller zeroes *out)
  *   ymp_adamw : g' = g * grad_scale * min(1, max_grad_norm / (sqrt(*sumsq)*grad_scale + 1e-6))
  *               AdamW on the fp32 master weights, bf16 model weights refreshed in the same pass
  *               (128-bit accesses, 26 bytes of HBM traffic per parameter incl. the optional gradient reset).
  * ------------------------------------------------------------------------------------------ */
 int ymp_sumsq(const float* g, int64_t n, float* out, void* stream);
+/* Deterministic mode: one fp32 partial per block; ymp_sumsq with it. */
+int64_t ymp_sumsq_workspace_size(int64_t n);
+int ymp_sumsq_ws(const float* g, int64_t n, float* out, void* workspace, void* stream);
 
 typedef struct ymp_adamw_args {
   float* master;        /* fp32 [n] */

@@ -32,6 +32,18 @@ inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t sme
   (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);  // errors surface in YMP_LAUNCH_CHECK
 }
 
+// Deterministic mode (ymp_set_deterministic, process-wide): the launchers of the four order-dependent sums (split-K
+// GEMM, LayerNorm gamma/beta gradients, column sums, sum of squares) then write one partial per CTA to a caller-provided
+// workspace and add the partials to the output in index order (ordered_sum below) instead of by atomics.  Read when a
+// call is launched, so a captured CUDA graph keeps the mode it was captured under.
+extern int g_deterministic;
+
+// out[r * ld_out + c] = ((out + parts[0]) + parts[1]) + ... + parts[nparts - 1], part k of element (r, c) at
+// parts[k * part_stride + r * ld_parts + c]; r < rows, c < cols (one fixed order, whatever the launch).  With out2 set,
+// the same launch also sums parts2 into out2 (same geometry).
+int ordered_sum(float* out, long ld_out, const float* parts, long ld_parts, long part_stride, int rows, int cols,
+                int nparts, cudaStream_t st, float* out2 = nullptr, const float* parts2 = nullptr);
+
 #define YMP_CHECK_ARG(cond, ...)                                   \
   do {                                                             \
     if (!(cond)) return ymp::set_error(YMP_EINVAL, __VA_ARGS__);   \

@@ -4,7 +4,8 @@
 //                   epilogue: accumulators staged through shared memory -> each warp along one row, two 4-column quads a thread ->
 //                   bias / GELU / GELU' / dropout / residual -> bf16 | fp32 | atomic fp32
 // Operands may be K-major or MN-major (the transpose bits of wgmma), so the same kernel serves forward (x.W^T),
-// dgrad (dy.W) and wgrad (dy^T.x, split-K with fp32 atomics).
+// dgrad (dy.W) and wgrad (dy^T.x, split-K with fp32 atomics, or per-slice partials added in slice order in the
+// deterministic mode).
 #include <cuda.h>
 
 #include <algorithm>
@@ -331,10 +332,11 @@ __device__ __forceinline__ void epilogue_rows(const GemmKParams& p, const float*
   }
 }
 
-template <int BM, int BN, int AMN, int BMN>
-__global__ void __launch_bounds__(GemmCfg<BM, BN>::THREADS, 1)
-gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                       const GemmKParams p) {
+// One CTA: the tile's K range [kb0, kb1) of slice ks, then the epilogue.  PARTIAL (deterministic split-K): the
+// alpha-scaled fp32 tile is stored, without any other epilogue step, to slice ks of the workspace p.D ([split_k, M,
+// ldd]); ordered_sum then adds the slices to D in slice order.
+template <int BM, int BN, int AMN, int BMN, bool PARTIAL>
+__device__ __forceinline__ void gemm_tile(const CUtensorMap& tma_a, const CUtensorMap& tma_b, const GemmKParams& p) {
   using Cfg = GemmCfg<BM, BN>;
   constexpr int NSTAGE = Cfg::NSTAGE;
   constexpr int A_STAGE_BYTES = Cfg::A_STAGE_BYTES;
@@ -472,6 +474,12 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
     }
   }
   named_sync(1, 128 * Cfg::CONSUMERS);
+  if constexpr (PARTIAL) {
+    GemmKParams q = p;
+    q.D = reinterpret_cast<float*>(p.D) + (size_t)ks * p.M * p.ldd;
+    epilogue_rows<BM, BN, epi_kind(EPI_AUX_NONE, 0, EPI_OUT_F32)>(q, stg, m_blk, n_blk);
+    return;
+  }
   switch (epi_kind_of(p)) {  // uniform over the launch
 #define YMP_EPI_CASE(aux, res, out) \
     case epi_kind(aux, res, out): epilogue_rows<BM, BN, epi_kind(aux, res, out)>(p, stg, m_blk, n_blk); break;
@@ -484,6 +492,20 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_c
 #undef YMP_EPI_CASE
     default: epilogue_rows<BM, BN, EPI_ANY>(p, stg, m_blk, n_blk);
   }
+}
+
+template <int BM, int BN, int AMN, int BMN>
+__global__ void __launch_bounds__(GemmCfg<BM, BN>::THREADS, 1)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+                       const GemmKParams p) {
+  gemm_tile<BM, BN, AMN, BMN, false>(tma_a, tma_b, p);
+}
+
+template <int BM, int BN, int AMN, int BMN>
+__global__ void __launch_bounds__(GemmCfg<BM, BN>::THREADS, 1)
+gemm_bf16_wgmma_partial_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+                               const GemmKParams p) {
+  gemm_tile<BM, BN, AMN, BMN, true>(tma_a, tma_b, p);
 }
 
 // ------------------------------------------------------------------------------ host side
@@ -543,19 +565,19 @@ static int make_video_map(CUtensorMap* m, const ymp_gemm_args* a) {
   return YMP_OK;
 }
 
-template <int BM, int BN, int AMN, int BMN>
+template <int BM, int BN, int AMN, int BMN, bool PARTIAL>
 static int launch_gemm_t(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& kp, int grid, cudaStream_t stream) {
   using Cfg = GemmCfg<BM, BN>;
+  constexpr auto kernel = PARTIAL ? gemm_bf16_wgmma_partial_kernel<BM, BN, AMN, BMN> : gemm_bf16_wgmma_kernel<BM, BN, AMN, BMN>;
   static DeviceOnce once;
   if (once.first())
-    YMP_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BM, BN, AMN, BMN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  Cfg::SMEM_BYTES));
-  gemm_bf16_wgmma_kernel<BM, BN, AMN, BMN><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, kp);
+    YMP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+  kernel<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, kp);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }
 
-template <int BM, int BN>
+template <int BM, int BN, bool PARTIAL = false>
 static int launch_gemm(const ymp_gemm_args* a, const GemmKParams& kp, cudaStream_t stream) {
   CUtensorMap ta, tb;
   int rc;
@@ -569,10 +591,10 @@ static int launch_gemm(const ymp_gemm_args* a, const GemmKParams& kp, cudaStream
   const int num_m = (a->M + BM - 1) / BM, num_n = (a->N + BN - 1) / BN;
   const int grid = num_m * num_n * kp.split_k;
   switch (kp.a_mn * 2 + kp.b_mn) {
-    case 0: return launch_gemm_t<BM, BN, 0, 0>(ta, tb, kp, grid, stream);
-    case 1: return launch_gemm_t<BM, BN, 0, 1>(ta, tb, kp, grid, stream);
-    case 2: return launch_gemm_t<BM, BN, 1, 0>(ta, tb, kp, grid, stream);
-    default: return launch_gemm_t<BM, BN, 1, 1>(ta, tb, kp, grid, stream);
+    case 0: return launch_gemm_t<BM, BN, 0, 0, PARTIAL>(ta, tb, kp, grid, stream);
+    case 1: return launch_gemm_t<BM, BN, 0, 1, PARTIAL>(ta, tb, kp, grid, stream);
+    case 2: return launch_gemm_t<BM, BN, 1, 0, PARTIAL>(ta, tb, kp, grid, stream);
+    default: return launch_gemm_t<BM, BN, 1, 1, PARTIAL>(ta, tb, kp, grid, stream);
   }
 }
 
@@ -602,12 +624,9 @@ static GemmPlan plan_gemm(long tiles, int kb_total, int split, bool accumulate, 
   return best;
 }
 
-}  // namespace ymp
-
-extern "C" int ymp_gemm(const ymp_gemm_args* a, void* stream) { return ymp_gemm_tiled(a, 0, stream); }
-
-extern "C" int ymp_gemm_tiled(const ymp_gemm_args* a, int tile_m, void* stream) {
-  using namespace ymp;
+// Checks, plans and launches one GEMM; with ws_bytes set it only reports the workspace the launch needs (bytes of the
+// deterministic split-K partials, 0 when the mode is off or the plan has one K slice) and launches nothing.
+static int gemm_run(const ymp_gemm_args* a, int tile_m, void* workspace, void* stream, int64_t* ws_bytes) {
   YMP_CHECK_ARG(a != nullptr, "ymp_gemm: null args");
   YMP_CHECK_ARG(a->A && a->B && a->D, "ymp_gemm: null A/B/D");
   YMP_CHECK_ARG(a->M > 0 && a->N > 0 && a->K > 0, "ymp_gemm: bad shape M=%d N=%d K=%d", a->M, a->N, a->K);
@@ -694,8 +713,39 @@ extern "C" int ymp_gemm_tiled(const ymp_gemm_args* a, int tile_m, void* stream) 
   kp.has_drop = (a->drop.rng && a->drop.p > 0.f) ? 1 : 0;
   kp.drop.rng = a->drop.rng; kp.drop.site = a->drop.site; kp.drop.p = a->drop.p;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const bool partial = g_deterministic && split > 1;
+  if (ws_bytes) {
+    *ws_bytes = partial ? (int64_t)split * a->M * a->ldd * sizeof(float) : 0;
+    return YMP_OK;
+  }
+  if (partial) {
+    YMP_CHECK_ARG(workspace && aligned16(workspace), "ymp_gemm: deterministic split-K needs a 16-byte aligned workspace of "
+                  "ymp_gemm_workspace_size bytes (ymp_gemm_ws)");
+    YMP_CHECK_ARG(a->d_row_block == 0, "ymp_gemm: deterministic split-K does not take d_row_block");
+    kp.D = workspace;
+    kp.accumulate = 0;
+    const int rc = bm == 192 ? launch_gemm<192, 256, true>(a, kp, st)
+                   : bn == 256 ? launch_gemm<128, 256, true>(a, kp, st) : launch_gemm<128, 128, true>(a, kp, st);
+    if (rc) return rc;
+    return ordered_sum(reinterpret_cast<float*>(a->D), a->ldd, reinterpret_cast<const float*>(workspace), a->ldd,
+                       (long)a->M * a->ldd, a->M, a->N, split, st);
+  }
   if (bm == 192) return launch_gemm<192, 256>(a, kp, st);
   if (bn == 256) return launch_gemm<128, 256>(a, kp, st);
   return launch_gemm<128, 128>(a, kp, st);
 }
+}  // namespace ymp
 
+extern "C" int ymp_gemm(const ymp_gemm_args* a, void* stream) { return ymp_gemm_tiled(a, 0, stream); }
+
+extern "C" int ymp_gemm_tiled(const ymp_gemm_args* a, int tile_m, void* stream) { return ymp::gemm_run(a, tile_m, nullptr, stream, nullptr); }
+
+extern "C" int ymp_gemm_ws(const ymp_gemm_args* a, int tile_m, void* workspace, void* stream) {
+  return ymp::gemm_run(a, tile_m, workspace, stream, nullptr);
+}
+
+extern "C" int64_t ymp_gemm_workspace_size(const ymp_gemm_args* a, int tile_m) {
+  int64_t bytes = 0;
+  const int rc = ymp::gemm_run(a, tile_m, nullptr, nullptr, &bytes);
+  return rc ? rc : bytes;
+}

@@ -130,6 +130,9 @@ struct LnBwdParams {
   DropSpec drop;
 };
 
+// ln_bwd_partial_kernel below is a copy of this kernel for the deterministic mode that differs only in the final store
+// of dgamma / dbeta: a change to the row arithmetic here goes there too.  tests/test_deterministic_gpu.py checks that
+// both give the same dx and dx_drop bit for bit.
 template <int VPL, bool WGRAD, bool XF32, bool DROP>
 __global__ void __launch_bounds__(LN_WARPS * 32, WGRAD ? (VPL <= 4 ? 3 : 1) : (DROP ? 2 : 4)) ln_bwd_kernel(const LnBwdParams p) {
   const int lane = threadIdx.x & 31;
@@ -229,6 +232,106 @@ __global__ void __launch_bounds__(LN_WARPS * 32, WGRAD ? (VPL <= 4 ? 3 : 1) : (D
   }
 }
 
+
+// Deterministic mode: ln_bwd_kernel<VPL, true, XF32, DROP> whose block stores its dgamma / dbeta sums to rows
+// 2 blockIdx.x and 2 blockIdx.x + 1 of the [blocks, 2, D] workspace p.dgamma instead of adding them to the outputs;
+// ordered_sum then adds the rows in block order.  A copy rather than a template flag of ln_bwd_kernel: folded into that
+// kernel, the flag changed the code ptxas makes for the atomic path.
+template <int VPL, bool XF32, bool DROP>
+__global__ void __launch_bounds__(LN_WARPS * 32, VPL <= 4 ? 3 : 1) ln_bwd_partial_kernel(const LnBwdParams p) {
+  constexpr bool WGRAD = true;
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  const int nvec = p.D >> 3;
+  float dg[WGRAD ? VPL : 1][8], db[WGRAD ? VPL : 1][8];
+  if (WGRAD) {
+#pragma unroll
+    for (int j = 0; j < VPL; ++j)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { dg[j][e] = 0.f; db[j][e] = 0.f; }
+  }
+  const uint4* g4 = reinterpret_cast<const uint4*>(p.gamma);
+  DropState ds = {};
+  if (DROP) ds = drop_state(p.drop);
+  for (int row = blockIdx.x * LN_WARPS + warp; row < p.rows; row += gridDim.x * LN_WARPS) {
+    const int irow = p.in_rows ? p.in_rows[row] : row;
+    if (irow < 0) continue;  // padding slot of the forward: no input row behind it
+    const uint4* dyr = reinterpret_cast<const uint4*>(p.dy + (size_t)row * p.lddy);
+    const float mu = p.mean[row], rs = p.rstd[row];
+    // Two passes over the row keep the register footprint small (high occupancy for an HBM-bound
+    // kernel); the second pass re-reads the 3-8 KB row from L1/L2, not from HBM.
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int j = 0; j < VPL; ++j) {
+      const int vi = j * 32 + lane;
+      if (vi < nvec) {
+        float xv[8], dyv[8], g[8];
+        load8<XF32>(p.x, (size_t)irow, p.ldx, vi, xv);
+        unpack8(__ldg(dyr + vi), dyv);
+        unpack8(__ldg(g4 + vi), g);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const float xh = (xv[e] - mu) * rs, gy = dyv[e] * g[e];
+          s1 += gy;
+          s2 += gy * xh;
+          if (WGRAD) { dg[j][e] += dyv[e] * xh; db[j][e] += dyv[e]; }
+        }
+      }
+    }
+    s1 = warp_sum(s1) / (float)p.D;
+    s2 = warp_sum(s2) / (float)p.D;
+    uint4* dxr = reinterpret_cast<uint4*>(p.dx + (size_t)irow * p.ldx);
+    const uint4* ar = p.add ? reinterpret_cast<const uint4*>(p.add + (size_t)irow * p.ldadd) : nullptr;
+#pragma unroll
+    for (int j = 0; j < VPL; ++j) {
+      const int vi = j * 32 + lane;
+      if (vi < nvec) {
+        float xv[8], dyv[8], g[8], o[8];
+        load8<XF32>(p.x, (size_t)irow, p.ldx, vi, xv);
+        unpack8(__ldg(dyr + vi), dyv);
+        unpack8(__ldg(g4 + vi), g);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) o[e] = rs * (dyv[e] * g[e] - s1 - (xv[e] - mu) * rs * s2);
+        if (ar) {
+          float a[8];
+          unpack8(__ldg(ar + vi), a);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) o[e] += a[e];
+        }
+        dxr[vi] = pack8(o);
+        if (DROP) {  // gradient w.r.t. the pre-dropout branch output: same mask bits as the forward epilogue
+          drop4(ds, (uint32_t)irow, (uint32_t)(vi * 8), o[0], o[1], o[2], o[3]);
+          drop4(ds, (uint32_t)irow, (uint32_t)(vi * 8 + 4), o[4], o[5], o[6], o[7]);
+          reinterpret_cast<uint4*>(p.dx_drop + (size_t)irow * p.ldx)[vi] = pack8(o);
+        }
+      }
+    }
+  }
+  if (WGRAD) {
+    // block-level reduce across the 8 warps, then one store per column per block
+    __shared__ float red[LN_WARPS][32 * 8 + 1];
+    for (int j = 0; j < VPL; ++j) {
+      for (int pass = 0; pass < 2; ++pass) {
+        __syncthreads();
+#pragma unroll
+        for (int e = 0; e < 8; ++e) red[warp][lane * 8 + e] = pass == 0 ? dg[j][e] : db[j][e];
+        __syncthreads();
+        // 256 columns per (j, pass): thread t < 64 owns 4 consecutive columns -> one 16-byte reduction
+        if (threadIdx.x < 64) {
+          float s[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+          for (int w = 0; w < LN_WARPS; ++w)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) s[e] += red[w][threadIdx.x * 4 + e];
+          const int col = j * 256 + threadIdx.x * 4;
+          if (col < p.D)  // D % 8 == 0: the 4 columns are all inside
+            *reinterpret_cast<float4*>(p.dgamma + (size_t)(2 * blockIdx.x + pass) * p.D + col) = make_float4(s[0], s[1], s[2], s[3]);
+        }
+      }
+    }
+  }
+}
+
 }  // namespace ymp
 
 extern "C" int ymp_layernorm_fwd(const ymp_layernorm_args* a, void* stream) {
@@ -259,7 +362,25 @@ extern "C" int ymp_layernorm_fwd(const ymp_layernorm_args* a, void* stream) {
   return YMP_OK;
 }
 
-extern "C" int ymp_layernorm_bwd(const ymp_layernorm_bwd_args* a, void* stream) {
+namespace ymp {
+// Grid of ymp_layernorm_bwd: with weight grads each block ends with 2*D atomics; resident blocks per SM: 3 with weight
+// grads (80 registers at D <= 1024), 4 without; the grid is a whole number of such waves so that the row loop stays
+// balanced.
+static int ln_bwd_blocks(const ymp_layernorm_bwd_args* a) {
+  const int cap = a->dgamma ? num_sms() * (a->D <= 1024 ? 3 : 2) : num_sms() * 8;
+  return min((a->rows + LN_WARPS - 1) / LN_WARPS, cap);
+}
+}  // namespace ymp
+
+extern "C" int64_t ymp_layernorm_bwd_workspace_size(const ymp_layernorm_bwd_args* a) {
+  using namespace ymp;
+  if (!g_deterministic || !a || !a->dgamma || a->rows <= 0 || a->D <= 0) return 0;
+  return (int64_t)ln_bwd_blocks(a) * 2 * a->D * sizeof(float);
+}
+
+extern "C" int ymp_layernorm_bwd(const ymp_layernorm_bwd_args* a, void* stream) { return ymp_layernorm_bwd_ws(a, nullptr, stream); }
+
+extern "C" int ymp_layernorm_bwd_ws(const ymp_layernorm_bwd_args* a, void* workspace, void* stream) {
   using namespace ymp;
   YMP_CHECK_ARG(a && a->dy && a->x && a->gamma && a->mean && a->rstd && a->dx, "ymp_layernorm_bwd: null pointer");
   YMP_CHECK_ARG(a->rows > 0 && a->D > 0 && a->D % 8 == 0 && a->D <= 4096, "ymp_layernorm_bwd: bad D=%d", a->D);
@@ -281,14 +402,22 @@ extern "C" int ymp_layernorm_bwd(const ymp_layernorm_bwd_args* a, void* stream) 
   cudaStream_t st = (cudaStream_t)stream;
   const int vpl = (a->D / 8 + 31) / 32;
   const bool wg = a->dgamma != nullptr;
-  // with weight grads each block ends with 2*D atomics; 6 blocks per SM keeps enough warps in
-  // flight for HBM while bounding the atomic tail (~900 adds per address)
-  // resident blocks per SM: 3 with weight grads (80 registers at D <= 1024), 4 without; the grid is a whole
-  // number of such waves so that the row loop stays balanced
-  const int cap = wg ? num_sms() * (a->D <= 1024 ? 3 : 2) : num_sms() * 8;
-  const int blocks = min((a->rows + LN_WARPS - 1) / LN_WARPS, cap);
+  const int blocks = ln_bwd_blocks(a);
   const int thr = LN_WARPS * 32;
   const bool xf = (a->x_dtype == YMP_DT_F32);
+  if (wg && g_deterministic) {
+    YMP_CHECK_ARG(workspace && aligned16(workspace), "ymp_layernorm_bwd: deterministic mode needs a 16-byte aligned workspace "
+                  "of ymp_layernorm_bwd_workspace_size bytes (ymp_layernorm_bwd_ws)");
+    p.dgamma = (float*)workspace;
+#define YMP_LN_BWD_P(V, X) do { if (p.dx_drop) ln_bwd_partial_kernel<V, X, true><<<blocks, thr, 0, st>>>(p); else ln_bwd_partial_kernel<V, X, false><<<blocks, thr, 0, st>>>(p); } while (0)
+#define YMP_LN_BWD_PV(X) do { if (vpl <= 3) YMP_LN_BWD_P(3, X); else if (vpl <= 8) YMP_LN_BWD_P(8, X); else YMP_LN_BWD_P(16, X); } while (0)
+    if (xf) YMP_LN_BWD_PV(true); else YMP_LN_BWD_PV(false);
+#undef YMP_LN_BWD_PV
+#undef YMP_LN_BWD_P
+    YMP_LAUNCH_CHECK();
+    const float* ws = (const float*)workspace;
+    return ordered_sum(a->dgamma, 0, ws, 0, 2L * a->D, 1, a->D, blocks, st, a->dbeta, ws + a->D);
+  }
 #define YMP_LN_BWD(V, W, X) do { if (p.dx_drop) ln_bwd_kernel<V, W, X, true><<<blocks, thr, 0, st>>>(p); else ln_bwd_kernel<V, W, X, false><<<blocks, thr, 0, st>>>(p); } while (0)
 #define YMP_LN_BWD_V(W, X) do { if (vpl <= 3) YMP_LN_BWD(3, W, X); else if (vpl <= 8) YMP_LN_BWD(8, W, X); else YMP_LN_BWD(16, W, X); } while (0)
   if (wg) { if (xf) YMP_LN_BWD_V(true, true); else YMP_LN_BWD_V(true, false); }

@@ -3,6 +3,8 @@
 // small group reductions.  All use 128-bit coalesced accesses where the layout allows.
 #include <math_constants.h>
 
+#include <algorithm>
+
 #include "common.h"
 #include "philox.cuh"
 #include "ptx.cuh"
@@ -201,9 +203,10 @@ __device__ __forceinline__ void acc8(float (&acc)[8], const uint4& u) {
   acc[0] += bf16_lo(u.x); acc[1] += bf16_hi(u.x); acc[2] += bf16_lo(u.y); acc[3] += bf16_hi(u.y);
   acc[4] += bf16_lo(u.z); acc[5] += bf16_hi(u.z); acc[6] += bf16_lo(u.w); acc[7] += bf16_hi(u.w);
 }
-__global__ void __launch_bounds__(CS_WARPS * 32) colsum_kernel(const __nv_bfloat16* __restrict__ in,
-                                                               float* __restrict__ out, int R, int C, int ld,
-                                                               int rows_per_block) {
+// PARTIAL: the block's sums are stored to row blockIdx.y of `out` (stride ld_out) instead of added to out[0..C).
+template <bool PARTIAL>
+__device__ __forceinline__ void colsum_block(const __nv_bfloat16* __restrict__ in, float* __restrict__ out, int R, int C,
+                                             int ld, int rows_per_block, long ld_out) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int v = blockIdx.x * 32 + lane;  // 8-column vector index
   const bool active = v * 8 < C;
@@ -234,13 +237,60 @@ __global__ void __launch_bounds__(CS_WARPS * 32) colsum_kernel(const __nv_bfloat
 #pragma unroll
       for (int e = 0; e < 4; ++e) s[e] += red[w][l][e0 + e];
     const int col = (blockIdx.x * 32 + l) * 8 + e0;
-    if (col + 3 < C) {
+    if constexpr (PARTIAL) {
+      float* dst = out + blockIdx.y * ld_out + col;
+      if (col + 3 < C) {
+        *reinterpret_cast<float4*>(dst) = make_float4(s[0], s[1], s[2], s[3]);
+      } else {
+        for (int e = 0; e < 4; ++e)
+          if (col + e < C) dst[e] = s[e];
+      }
+    } else if (col + 3 < C) {
       asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(out + col), "f"(s[0]), "f"(s[1]), "f"(s[2]), "f"(s[3]) : "memory");
     } else {
       for (int e = 0; e < 4; ++e)
         if (col + e < C) atomicAdd(out + col + e, s[e]);
     }
   }
+}
+__global__ void __launch_bounds__(CS_WARPS * 32) colsum_kernel(const __nv_bfloat16* __restrict__ in,
+                                                               float* __restrict__ out, int R, int C, int ld,
+                                                               int rows_per_block) {
+  colsum_block<false>(in, out, R, C, ld, rows_per_block, 0);
+}
+// Deterministic mode: split s writes its partial to ws[s * ld_ws ..]; ordered_sum adds them in split order.
+__global__ void __launch_bounds__(CS_WARPS * 32) colsum_partial_kernel(const __nv_bfloat16* __restrict__ in,
+                                                                       float* __restrict__ ws, int R, int C, int ld,
+                                                                       int rows_per_block, long ld_ws) {
+  colsum_block<true>(in, ws, R, C, ld, rows_per_block, ld_ws);
+}
+
+// ------------------------------------------------------------------------------ fixed-order partial sums
+// blockIdx.y selects the (out, parts) pair: the LayerNorm gamma and beta sums go in one launch.
+__global__ void __launch_bounds__(256) ordered_sum_kernel(float* __restrict__ out, float* __restrict__ out2, long ld_out,
+                                                          const float* __restrict__ parts, const float* __restrict__ parts2,
+                                                          long ld_parts, long part_stride, int rows, int cols, int nparts) {
+  float* o = blockIdx.y ? out2 : out;
+  const float* pp = blockIdx.y ? parts2 : parts;
+  const long total = (long)rows * cols;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const long r = i / cols, c = i - r * cols;
+    const float* p = pp + r * ld_parts + c;
+    float v = o[r * ld_out + c];
+#pragma unroll 16
+    for (int k = 0; k < nparts; ++k) v += p[k * part_stride];  // the loads run ahead, the adds stay in order
+    o[r * ld_out + c] = v;
+  }
+}
+
+int ordered_sum(float* out, long ld_out, const float* parts, long ld_parts, long part_stride, int rows, int cols,
+                int nparts, cudaStream_t st, float* out2, const float* parts2) {
+  const long total = (long)rows * cols;
+  const int blocks = (int)std::min((total + 255) / 256, (long)num_sms() * 8);
+  ordered_sum_kernel<<<dim3(blocks, out2 ? 2 : 1), 256, 0, st>>>(out, out2, ld_out, parts, parts2, ld_parts, part_stride, rows,
+                                                                 cols, nparts);
+  YMP_LAUNCH_CHECK();
+  return YMP_OK;
 }
 
 // ------------------------------------------------------------------------------ group reduce
@@ -439,16 +489,39 @@ extern "C" int ymp_ce_bwd(const ymp_ce_args* a, void* stream) {
   return YMP_OK;
 }
 
-extern "C" int ymp_colsum(const ymp_colsum_args* a, void* stream) {
+static void colsum_grid(const ymp_colsum_args* a, int* gx, int* splits, int* rpb) {
+  *gx = ((a->C + 7) / 8 + 31) / 32;
+  *splits = max(1, min((a->R + 63) / 64, (num_sms() * 4 + *gx - 1) / *gx));
+  *rpb = (a->R + *splits - 1) / *splits;
+  *splits = (a->R + *rpb - 1) / *rpb;
+}
+
+extern "C" int64_t ymp_colsum_workspace_size(const ymp_colsum_args* a) {
+  if (!g_deterministic || !a || a->R <= 0 || a->C <= 0) return 0;
+  int gx, splits, rpb;
+  colsum_grid(a, &gx, &splits, &rpb);
+  return (int64_t)splits * gx * 256 * sizeof(float);
+}
+
+extern "C" int ymp_colsum(const ymp_colsum_args* a, void* stream) { return ymp_colsum_ws(a, nullptr, stream); }
+
+extern "C" int ymp_colsum_ws(const ymp_colsum_args* a, void* workspace, void* stream) {
   YMP_CHECK_ARG(a && a->in && a->out, "ymp_colsum: null pointer");
   // C need not be a multiple of 8: rows are read in 8-column vectors, so the row stride must cover the
   // rounded-up width (the columns beyond C are read and discarded)
   YMP_CHECK_ARG(a->R > 0 && a->C > 0 && a->ld % 8 == 0 && a->ld >= (a->C + 7) / 8 * 8 && aligned16(a->in), "ymp_colsum: bad shape/alignment");
   YMP_CHECK_ARG(aligned16(a->out), "ymp_colsum: out must be 16-byte aligned");
-  const int gx = ((a->C + 7) / 8 + 31) / 32;
-  int splits = max(1, min((a->R + 63) / 64, (num_sms() * 4 + gx - 1) / gx));
-  const int rpb = (a->R + splits - 1) / splits;
-  splits = (a->R + rpb - 1) / rpb;
+  int gx, splits, rpb;
+  colsum_grid(a, &gx, &splits, &rpb);
+  if (g_deterministic) {
+    YMP_CHECK_ARG(workspace && aligned16(workspace), "ymp_colsum: deterministic mode needs a 16-byte aligned workspace of "
+                  "ymp_colsum_workspace_size bytes (ymp_colsum_ws)");
+    const long ld_ws = (long)gx * 256;
+    colsum_partial_kernel<<<dim3(gx, splits), CS_WARPS * 32, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)a->in, (float*)workspace,
+                                                                                       a->R, a->C, a->ld, rpb, ld_ws);
+    YMP_LAUNCH_CHECK();
+    return ordered_sum(a->out, 0, (const float*)workspace, 0, ld_ws, 1, a->C, splits, (cudaStream_t)stream);
+  }
   colsum_kernel<<<dim3(gx, splits), CS_WARPS * 32, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)a->in, a->out, a->R, a->C, a->ld, rpb);
   YMP_LAUNCH_CHECK();
   return YMP_OK;

@@ -6,7 +6,9 @@
 
 namespace ymp {
 
-__global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g, long n, float* __restrict__ out) {
+// PARTIAL: the block's sum is stored to out[blockIdx.x] instead of added to *out.
+template <bool PARTIAL>
+__device__ __forceinline__ void sumsq_block(const float* __restrict__ g, long n, float* __restrict__ out) {
   float acc = 0.f;
   const long n4 = n >> 2;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
@@ -23,8 +25,18 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g,
     float v = s[threadIdx.x];
 #pragma unroll
     for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(out, v);
+    if (threadIdx.x == 0) {
+      if constexpr (PARTIAL) out[blockIdx.x] = v;
+      else atomicAdd(out, v);
+    }
   }
+}
+__global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g, long n, float* __restrict__ out) {
+  sumsq_block<false>(g, n, out);
+}
+// Deterministic mode: block b writes its sum to ws[b]; ordered_sum adds them to *out in block order.
+__global__ void __launch_bounds__(256) sumsq_partial_kernel(const float* __restrict__ g, long n, float* __restrict__ ws) {
+  sumsq_block<true>(g, n, ws);
 }
 
 struct AdamParams {
@@ -88,10 +100,24 @@ __global__ void __launch_bounds__(256) adamw_kernel(const AdamParams p) {
 
 using namespace ymp;
 
-extern "C" int ymp_sumsq(const float* g, int64_t n, float* out, void* stream) {
+static int sumsq_blocks(int64_t n) { return (int)min((long)((n / 4 + 255) / 256) + 1, (long)num_sms() * 8); }
+
+extern "C" int64_t ymp_sumsq_workspace_size(int64_t n) {
+  return g_deterministic && n > 0 ? (int64_t)sumsq_blocks(n) * sizeof(float) : 0;
+}
+
+extern "C" int ymp_sumsq(const float* g, int64_t n, float* out, void* stream) { return ymp_sumsq_ws(g, n, out, nullptr, stream); }
+
+extern "C" int ymp_sumsq_ws(const float* g, int64_t n, float* out, void* workspace, void* stream) {
   YMP_CHECK_ARG(g && out && n > 0, "ymp_sumsq: bad args");
   YMP_CHECK_ARG(aligned16(g), "ymp_sumsq: g must be 16-byte aligned");
-  const int blocks = (int)min((long)((n / 4 + 255) / 256) + 1, (long)num_sms() * 8);
+  const int blocks = sumsq_blocks(n);
+  if (g_deterministic) {
+    YMP_CHECK_ARG(workspace, "ymp_sumsq: deterministic mode needs a workspace of ymp_sumsq_workspace_size bytes (ymp_sumsq_ws)");
+    sumsq_partial_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(g, (long)n, (float*)workspace);
+    YMP_LAUNCH_CHECK();
+    return ordered_sum(out, 0, (const float*)workspace, 0, 1, 1, 1, blocks, (cudaStream_t)stream);
+  }
   sumsq_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(g, (long)n, out);
   YMP_LAUNCH_CHECK();
   return YMP_OK;

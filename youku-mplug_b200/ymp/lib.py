@@ -6,6 +6,7 @@ memory and streams; tensors cross this boundary as raw pointers.
 """
 import ctypes as C
 import os
+import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libymp_b200.so")
@@ -163,6 +164,8 @@ lib.ymp_launch_count.restype = C.c_uint64
 lib.ymp_attn_last_path.restype = C.c_int
 lib.ymp_set_pdl.restype = C.c_int
 lib.ymp_set_pdl.argtypes = [C.c_int]
+lib.ymp_set_deterministic.restype = C.c_int
+lib.ymp_set_deterministic.argtypes = [C.c_int]
 ATTN_PATH_MMA_SYNC, ATTN_PATH_WGMMA, ATTN_PATH_SMALL, ATTN_PATH_DECODE = 0, 1, 2, 3
 
 
@@ -199,6 +202,21 @@ _sumsq.restype = C.c_int
 _sumsq.argtypes = [c_vp, C.c_int64, c_vp, c_vp]
 
 
+def _declare_ws(name, argtypes, size_argtypes=None):
+    """The deterministic-mode entry points: <name>_workspace_size(args...) -> int64, <name>_ws(args..., workspace, stream)."""
+    size = getattr(lib, name + "_workspace_size")
+    size.restype, size.argtypes = C.c_int64, size_argtypes or argtypes
+    fn = getattr(lib, name + "_ws")
+    fn.restype, fn.argtypes = C.c_int, argtypes + [c_vp, c_vp]
+    return size, fn
+
+
+_gemm_ws_size, _gemm_ws = _declare_ws("ymp_gemm", [C.POINTER(GemmArgs), C.c_int])
+_ln_bwd_ws_size, _ln_bwd_ws = _declare_ws("ymp_layernorm_bwd", [C.POINTER(LayerNormBwdArgs)])
+_colsum_ws_size, _colsum_ws = _declare_ws("ymp_colsum", [C.POINTER(ColsumArgs)])
+_sumsq_ws_size, _sumsq_ws = _declare_ws("ymp_sumsq", [c_vp, C.c_int64, c_vp], [C.c_int64])
+
+
 def check(rc, what):
     if rc != 0:
         raise YmpError(f"{what} failed ({rc}): {lib.ymp_last_error().decode()}")
@@ -212,6 +230,48 @@ def set_pdl(on):
     """Programmatic dependent launch for this thread's next skinny-GEMM / LayerNorm / mma.sync attention launches
     (the decoding step).  Returns the previous setting."""
     return int(lib.ymp_set_pdl(int(bool(on))))
+
+
+def deterministic_mode(enabled, warn_only):
+    """The library's deterministic mode for torch's flags (torch.are_deterministic_algorithms_enabled(),
+    torch.is_deterministic_algorithms_warn_only_enabled()): on exactly when deterministic algorithms are enabled, with
+    or without warn_only.  warn_only alone does not enable them (use_deterministic_algorithms(False, warn_only=True)
+    leaves torch's deterministic mode off), so it leaves the library's off too."""
+    del warn_only   # on / off does not depend on it: the library never warns, it has a fixed-order path for every sum
+    return 1 if enabled else 0
+
+
+def sync_deterministic():
+    """Set the library's deterministic mode from torch.use_deterministic_algorithms (called by every op that launches
+    an order-dependent sum, before it launches); returns the mode."""
+    import torch
+    mode = deterministic_mode(torch.are_deterministic_algorithms_enabled(),
+                              torch.is_deterministic_algorithms_warn_only_enabled())
+    lib.ymp_set_deterministic(mode)
+    return mode
+
+
+_FILL_LOCK = threading.Lock()
+
+
+def workspace(nbytes, device):
+    """Device workspace of a deterministic-mode call on `device` (the operands' device) from the torch allocator on the
+    current stream, so a CUDA graph capture owns it; None when the call needs none."""
+    if nbytes < 0:
+        check(int(nbytes), "workspace size")
+    if nbytes == 0:
+        return None
+    import torch
+    import torch.utils.deterministic as det
+    # Every byte the call reads it has written first, so torch's NaN fill of uninitialised memory under
+    # use_deterministic_algorithms would be a pass over the workspace for nothing.  torch has no per-allocation switch
+    # for it; the lock keeps concurrent calls from restoring each other's saved value.
+    with _FILL_LOCK:
+        fill, det.fill_uninitialized_memory = det.fill_uninitialized_memory, False
+        try:
+            return torch.empty(nbytes, dtype=torch.uint8, device=device)
+        finally:
+            det.fill_uninitialized_memory = fill
 
 
 def attn_last_path():

@@ -112,6 +112,10 @@ def gemm(a, b, *, a_t=False, b_t=False, bias=None, residual=None, act=ACT_NONE, 
     _set_drop(g.drop, drop)
     if _im2col is not None:
         g.im2col_P, g.im2col_B, g.im2col_C, g.im2col_T, g.im2col_H, g.im2col_W = _im2col
+    if accumulate and L.sync_deterministic():   # split-K: fixed-order sum of the K slices
+        ws = L.workspace(L._gemm_ws_size(L.C.byref(g), tile_m), out.device)
+        L.check(L._gemm_ws(L.C.byref(g), tile_m, L.ptr(ws), L.cur_stream()), "ymp_gemm")
+        return out
     L.check(L._gemm_tiled(L.C.byref(g), tile_m, L.cur_stream()), "ymp_gemm")
     return out
 
@@ -219,10 +223,18 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, add=None, dgamma=None, dbeta=None, i
         assert dx_drop.dtype == bf16 and dx_drop.stride(0) == dx.stride(0)
         a.dx_drop = dx_drop.data_ptr()
         _set_drop(a.drop, drop)
-        L.call(L._ln_bwd, a, "ymp_layernorm_bwd")
+        _ln_bwd(a, dx.device)
         return dx, dx_drop
-    L.call(L._ln_bwd, a, "ymp_layernorm_bwd")
+    _ln_bwd(a, dx.device)
     return dx
+
+
+def _ln_bwd(a, device):
+    if a.dgamma and L.sync_deterministic():   # gamma / beta gradients: fixed-order sum of the block partials
+        ws = L.workspace(L._ln_bwd_ws_size(L.C.byref(a)), device)
+        L.check(L._ln_bwd_ws(L.C.byref(a), L.ptr(ws), L.cur_stream()), "ymp_layernorm_bwd")
+    else:
+        L.call(L._ln_bwd, a, "ymp_layernorm_bwd")
 
 
 # ---------------------------------------------------------------------------------- attention
@@ -461,7 +473,11 @@ def colsum(x, out):
     assert out.dtype == torch.float32 and out.numel() == x.shape[1]
     a = L.ColsumArgs()
     a.in_, a.out, a.R, a.C, a.ld = x.data_ptr(), out.data_ptr(), x.shape[0], x.shape[1], x.stride(0)
-    L.call(L._colsum, a, "ymp_colsum")
+    if L.sync_deterministic():
+        ws = L.workspace(L._colsum_ws_size(L.C.byref(a)), out.device)
+        L.check(L._colsum_ws(L.C.byref(a), L.ptr(ws), L.cur_stream()), "ymp_colsum")
+    else:
+        L.call(L._colsum, a, "ymp_colsum")
     return out
 
 
@@ -478,7 +494,11 @@ def group_reduce(x, G, T, out, scale=1.0, broadcast=False):
 def sumsq(g, out):
     """out (fp32 scalar tensor, accumulated) += sum(g^2)."""
     assert g.dtype == torch.float32 and g.is_contiguous()
-    L.check(L._sumsq(g.data_ptr(), g.numel(), out.data_ptr(), L.cur_stream()), "ymp_sumsq")
+    if L.sync_deterministic():
+        ws = L.workspace(L._sumsq_ws_size(g.numel()), g.device)
+        L.check(L._sumsq_ws(g.data_ptr(), g.numel(), out.data_ptr(), L.ptr(ws), L.cur_stream()), "ymp_sumsq")
+    else:
+        L.check(L._sumsq(g.data_ptr(), g.numel(), out.data_ptr(), L.cur_stream()), "ymp_sumsq")
     return out
 
 

@@ -248,7 +248,7 @@ class TrainEngine:
         all-reduces are part of the graph (fork/join on NCCL's stream); the remaining all-reduce, the
         grad-norm and the fused AdamW (6 launches) stay outside the graph.  Inputs are copied into the graph's static buffers (the copy
         also casts fp32 frames to bf16), so callers may pass fresh tensors every step."""
-        key = tuple(_signature(x) for x in inputs)
+        key = graph_key(inputs)
         st = self._graphs.setdefault(key, dict(calls=0))
         if self.gas > 1:
             use_graph = False   # boundary / non-boundary micro-steps differ (all-reduce, step): run eagerly
@@ -323,6 +323,14 @@ def _tensors_of(x):
     if hasattr(x, "data") and isinstance(x.data, dict):
         return {k: v for k, v in x.data.items() if torch.is_tensor(v)}
     raise TypeError(f"train_step: unsupported input type {type(x).__name__}")
+
+
+def graph_key(inputs):
+    """Key of train_step's CUDA graphs: the library's deterministic mode (from torch.use_deterministic_algorithms;
+    a graph replays the kernels of the mode it was captured under) and the input signature."""
+    from . import lib
+    return (lib.deterministic_mode(torch.are_deterministic_algorithms_enabled(),
+                                   torch.is_deterministic_algorithms_warn_only_enabled()),) + tuple(_signature(x) for x in inputs)
 
 
 def _signature(x):
