@@ -35,10 +35,6 @@ const char* ymp_last_error(void);
 int ymp_abi_version(void);
 /* Number of kernel launches this process has enqueued through the library (for gpu_launches). */
 uint64_t ymp_launch_count(void);
-/* Programmatic dependent launch for the calling thread's next launches of ymp_gemm_skinny, ymp_layernorm_fwd and the
- * mma.sync ymp_attn_fwd (the single-token decoding step): each of those kernels may then start while its predecessor in
- * the stream drains (it waits on the device before reading the predecessor's output).  Returns the previous setting. */
-int ymp_set_pdl(int on);
 /* Deterministic mode (process-wide; off by default): every order-dependent sum of the library - the split-K GEMM, the
  * gamma / beta gradients of ymp_layernorm_bwd, ymp_colsum and ymp_sumsq - then combines its per-CTA partial sums in an
  * order fixed by the partial's index instead of by fp32 atomics in arrival order: each partial is stored to a workspace
@@ -159,8 +155,8 @@ int ymp_gemm_ws(const ymp_gemm_args* a, int tile_m, void* workspace, void* strea
  *   ymp_gemm_skinny      : 1 <= M <= 8 (one beam search, sample()).
  *   ymp_gemm_skinny_wide : 1 <= M <= 64 (a batched beam search: clips x beams).  M <= 8 runs exactly the launch of
  *                          ymp_gemm_skinny; 9 <= M <= 64 a kernel with the same per-element arithmetic, so row m of the
- *                          result is bit-identical to the same row computed by any call with the same N and K.  The
- *                          fused LayerNorm (ln_out) needs M <= 8; M > 64 is rejected. */
+ *                          result is bit-identical to the same row computed by any call with the same N and K.  M > 64
+ *                          is rejected. */
 typedef struct ymp_gemm_skinny_args {
   const void* x;         /* bf16 [M, K], row stride ldx */
   const void* w;         /* bf16 [N, K], row stride ldw (an nn.Linear weight) */
@@ -174,15 +170,6 @@ typedef struct ymp_gemm_skinny_args {
   void* y2;
   const int64_t* y2_off_dev;
   int64_t ldy2, y2_off_stride;
-  /* optional fused LayerNorm of the complete fp32 result (the next sub-layer's input): the CTA that finishes last
-   * (ticket in *ln_counter, which must be 0 at launch and is reset to 0) writes ln_out[m, :] = LN(y[m, :]) in bf16 with
-   * exactly the arithmetic of ymp_layernorm_fwd - one kernel boundary less per sub-layer of the decoding step */
-  const void* ln_gamma;  /* bf16 [N] */
-  const void* ln_beta;   /* bf16 [N] */
-  void* ln_out;          /* bf16 [M, N], row stride ld_ln */
-  uint32_t* ln_counter;
-  int32_t ld_ln;
-  float ln_eps;
 } ymp_gemm_skinny_args;
 int ymp_gemm_skinny(const ymp_gemm_skinny_args* a, void* stream);
 int ymp_gemm_skinny_wide(const ymp_gemm_skinny_args* a, void* stream);

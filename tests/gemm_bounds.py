@@ -44,7 +44,7 @@ rounds relative to the running sum, split u32 (|D0| + |alpha| |A||B|).  A bf16 s
 covers results that underflow.
     e_out = C [e + u32 |out| [residual] + split u32 (|D0| + |alpha||A||B|) [accumulate] + u |out| [bf16]] + 2^-100
 
-LayerNorm of the skinny kernel (fp32 y, two-pass statistics over n = N columns, rsqrt.approx):
+LayerNorm of an fp32 row y (two-pass statistics over n = N columns, rsqrt.approx):
     e_mean = (n + 1) u32 mean|y|,   relative error of var + eps: e_var = ((n + 4) u32 var + e_mean^2) / (var + eps)
     (the sum of squares of the deviations from the computed mean is off by n e_mean^2 at most),
     e_rstd = 0.5 e_var + 2^-22 (rsqrt.approx) + 2 u32,
@@ -270,8 +270,8 @@ def layernorm_stat_errors(y, eps):
 
 
 def layernorm_bound(y, gamma, beta, eps, out_bf16=True):
-    """Per-element bound on |ln_out - LN(y)| (module docstring, LayerNorm of the skinny kernel; an fp32 output rounds
-    once, u32 |ln|, instead of u |ln|)."""
+    """Per-element bound on the error of a LayerNorm of the fp32 rows y against the float64 LN(y) (module docstring;
+    an fp32 output rounds once, u32 |ln|, instead of u |ln|)."""
     ln, z, rstd, _, _ = layernorm_reference(y, gamma, beta, eps)
     e_mean, e_rstd = layernorm_stat_errors(y, eps)
     g = gamma.double().abs()

@@ -11,7 +11,7 @@ the exact sum (each rounding is relative to a partial sum, at most sum|x_i|).  A
 k atomic adds onto x0 cost k u32 (|x0| + sum|x_i|) in any order.
 
 LayerNorm forward (ln_fwd_kernel: lane-sequential sums over 8 ceil(D/256) elements, a 5-level butterfly, two-pass
-variance, rsqrtf): the skinny-LayerNorm bound of gemm_bounds.py with n = D (a sum is at most D/32 + 5 <= D + 1 roundings
+variance, rsqrtf): the LayerNorm bound of gemm_bounds.py with n = D (a sum is at most D/32 + 5 <= D + 1 roundings
 deep): mean C e_mean, rstd C e_rstd rstd, y layernorm_bound (an fp32 y rounds once, u32 |y|, a bf16 y u |y|).  A
 padding slot (in_rows -1) is a bf16 zero row with mean = rstd = 0, exactly.
 

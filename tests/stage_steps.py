@@ -52,8 +52,8 @@ history of cached QKV rows (KVHistory) and applies the events to it; every atten
 through the call's row table (kv_rows, min(s_kv, *s_kv_dev) keys), must equal that history bit for bit, and a skinny
 QKV GEMM's cache copy must land in slot b max_len + len and equal its output row bit for bit.  The GPU walks fill each
 new cache store with a finite +-3e4 poison, so a read of a slot no step wrote fails.  The skinny GEMMs use
-gemm_bounds.bounds with split = skinny_slices(N, K) (each K slice is its own chain) and their fused LayerNorm
-gemm_bounds.layernorm_bound of the kernel's own fp32 y; the table gather is exact.  No bound is added.
+gemm_bounds.bounds with split = skinny_slices(N, K) (each K slice is its own chain); the table gather is exact.  No
+bound is added.
 """
 import json
 import math
@@ -145,12 +145,6 @@ def _k_skinny(a, kw, sms):
     ref = GB.reference(A, B, bias=a.get("bias"), act=kw.get("act", 0), residual=a.get("residual"))
     e_out, _ = GB.bounds(ref, A.shape[1], split=GB.skinny_slices(B.shape[0], A.shape[1]), out_bf16=kw["out_dtype"] == BF16)
     return dict(D=(ref["out"], e_out), out2=(ref["out"], e_out))
-
-
-def _skinny_ln(y, a, kw):
-    """The skinny kernel's fused LayerNorm is of its own fp32 result y: (float64 LN(y), bound)."""
-    g, b, eps = a["ln_gamma"], a["ln_beta"], kw["ln_eps"]
-    return GB.layernorm_reference(y, g, b, eps)[0], GB.layernorm_bound(y, g, b, eps)
 
 
 def _k_im2col(a, kw, sms):
@@ -331,9 +325,7 @@ class Exec:
             if self.mode == "synth" and name in self.tamper:
                 ins, kw = self.tamper[name](dict(ins), dict(kw), self.vals)
             refs = KERNELS[op](ins, kw, self.sms)
-            res = {o: (refs[o][0] if self.mode == "exact" else self.rnd(refs[o][0], outs[o])) for o in outs if o != "ln"}
-            if "ln" in outs:
-                res["ln"] = self.rnd(_skinny_ln(res["D"], ins, kw)[0], outs["ln"])
+            res = {o: (refs[o][0] if self.mode == "exact" else self.rnd(refs[o][0], outs[o])) for o in outs}
             if self.mode == "synth":
                 targets = {o: (acc[o] if (o in acc and acc[o] is not None) else None) for o in outs}
                 self.out_trace.append(Rec(op, {k: v.clone() for k, v in ins.items()}, kw,
@@ -398,7 +390,7 @@ class Exec:
             if o not in rec.outs:
                 raise StepFailure(name, f"output {o} missing from the trace")
             got = rec.outs[o]
-            want, bound = _skinny_ln(rec.outs["D"].to(F64), ins, kw) if o == "ln" else refs[o]
+            want, bound = refs[o]
             if o == "out2" and not torch.equal(got, rec.outs["D"].to(got.dtype)):
                 raise StepFailure(name, "value out2: the cache row is not the output row bit for bit")
             if got.dtype != dt:
@@ -575,21 +567,15 @@ def attn(X, name, q, k, v, *, scale, causal=False, drop=None, temporal=False, ke
     return r["o"], r["lse"]
 
 
-def skinny(X, name, op, A, B, *, bias=None, residual=None, act=ACT_NONE, out=BF16, out2_rows=None, ln=None):
+def skinny(X, name, op, A, B, *, bias=None, residual=None, act=ACT_NONE, out=BF16, out2_rows=None):
     """ymp_gemm_skinny(_wide): D = act(A B^T + bias) + residual.  out2_rows: the KV-cache rows the result is also
-    written to (the step names them); ln = (W, prefix, eps): the kernel's last CTA also returns LN(D) (y, ln)."""
+    written to (the step names them)."""
     ins = dict(A=A, B=B, bias=bias, residual=residual)
-    kw = dict(act=act, out_dtype=out, out2_rows=out2_rows, ln_eps=None)
+    kw = dict(act=act, out_dtype=out, out2_rows=out2_rows)
     outs = dict(D=out)
     if out2_rows is not None:
         outs["out2"] = BF16
-    if ln is not None:
-        Wl, pre, eps = ln
-        ins.update(ln_gamma=Wl[pre + ".weight"], ln_beta=Wl[pre + ".bias"])
-        kw["ln_eps"] = eps
-        outs["ln"] = BF16
-    r = X.call(name, op, ins, kw, outs)
-    return (r["D"], r["ln"]) if ln is not None else r["D"]
+    return X.call(name, op, ins, kw, outs)["D"]
 
 
 def attn_b(X, name, q, k, v, o, lse, do, *, scale, causal=False, drop=None, temporal=False):
@@ -1301,9 +1287,9 @@ def decode_token(X, W, tok, hist, gcfg, kind, name, max_len):
     kind "skinny" is TokenStep: x = fl32(bf16 emb(tok) + bf16 pos[len]), every linear a skinny GEMM (the wide entry
     point above 8 rows); the QKV GEMM writes q to the staging rows and the same row to cache slot b max_len + len;
     attention reads the len + 1 keys of each sequence's history (the new one last) through the row table; the
-    LayerNorms are separate calls, or with kind "skinny_ln" computed by the last CTA of the GEMM that completes their
-    input; fp32 logits.  kind "gemm" is gpt_decode with n = 1: wgmma GEMMs, the QKV rows stored straight into the
-    cache slots, share_prefill(1), the final LayerNorm through in_rows, bf16 logits.  Returns the logits [B, V]."""
+    LayerNorms are separate calls; fp32 logits.  kind "gemm" is gpt_decode with n = 1: wgmma GEMMs, the QKV rows stored
+    straight into the cache slots, share_prefill(1), the final LayerNorm through in_rows, bf16 logits.  Returns the
+    logits [B, V]."""
     g = dims_gpt(gcfg)
     nh, hd, H, eps = g["nh"], g["hd"], g["H"], g["eps"]
     B, p = hist.B, hist.len
@@ -1318,9 +1304,6 @@ def decode_token(X, W, tok, hist, gcfg, kind, name, max_len):
         return skinny(X, nm, op, a, W[wname + ".weight"], **wb, **k)
 
     def lin_ln(nm, a, wname, residual, ln_pre, ln_name):
-        if kind == "skinny_ln":
-            return skinny(X, nm, op, a, W[wname + ".weight"], bias=W[wname + ".bias"], residual=residual, out=F32,
-                          ln=(W, ln_pre, eps))
         y = lin(nm, a, wname, residual=residual, out=F32)
         if kind == "gemm":    # gpt_decode normalises at the start of the next layer, the final rows after the loop
             return y, None
@@ -1529,32 +1512,26 @@ class Recorder:
         return r
 
     def _skinny(self, op, fn, x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_dtype=BF16, out2=None,
-                out2_row_stride=0, out2_off=None, ln=None):
+                out2_row_stride=0, out2_off=None):
         """out2: the cache rows m out2_row_stride + *out2_off (offset read after the sync) as output out2 and their
-        indices as argument out2_rows; ln: the fused LayerNorm's (gamma, beta) operands, eps and output ln."""
+        indices as argument out2_rows."""
         ins = dict(A=x.to(F64).clone(), B=w.to(F64).clone())
         if bias is not None:
             ins["bias"] = bias.to(F64).clone()
         if residual is not None:
             ins["residual"] = residual.to(F64).clone()
-        kw = dict(act=act, out2_rows=None, ln_eps=None)
-        if ln is not None:
-            ins["ln_gamma"], ins["ln_beta"] = ln[0].to(F64).clone(), ln[1].to(F64).clone()
-            kw["ln_eps"] = ln[2]
-        r = fn(x, w, bias=bias, residual=residual, act=act, out=out, out_dtype=out_dtype, out2=out2,
-               out2_row_stride=out2_row_stride, out2_off=out2_off, ln=ln)
+        kw = dict(act=act, out2_rows=None)
+        y = fn(x, w, bias=bias, residual=residual, act=act, out=out, out_dtype=out_dtype, out2=out2,
+               out2_row_stride=out2_row_stride, out2_off=out2_off)
         torch.cuda.synchronize()
-        y = r[0] if ln is not None else r
         kw["out_dtype"] = y.dtype
         outs = dict(D=y.clone())
         if out2 is not None:
             rows = torch.arange(y.shape[0], dtype=torch.int64) * out2_row_stride + int(out2_off.item())
             kw["out2_rows"] = rows
             outs["out2"] = out2[rows.to(out2.device)].clone()
-        if ln is not None:
-            outs["ln"] = r[1].clone()
         self._push(op, ins, kw, outs)
-        return r
+        return y
 
     def _gemm_skinny(self, fn, x, w, **kw):
         return self._skinny("gemm_skinny", fn, x, w, **kw)

@@ -10,7 +10,6 @@ B. Epilogue transfer function.  A single non-zero k column carries every bf16 va
    +-100, so the pre-activation is exact: act(x) and act'(x) against float64 within the activation bound, and the
    vector (full quads) and scalar (ragged N) epilogue paths, with and without aux_out, and the skinny kernels bit-equal.
 C. Gaussian operands at the model's shapes: err / bound <= 1 for every element.
-D. The skinny kernel's fused LayerNorm against a float64 LayerNorm of the kernel's own fp32 result.
 Set YMP_GEMM_BOUNDS_REPORT=<file> to write the largest err / bound per kernel, epilogue and tensor as JSON.
 """
 import json
@@ -431,22 +430,3 @@ def test_skinny_gaussian_model_shapes(cuda, kernel, M, N, K, epi):
     e_out, _ = GB.bounds(ref, K, split=GB.skinny_slices(N, K), out_bf16=out_dtype == bf16)
     epi_name = "+".join(k for k in epi if k != "out") or "plain"
     _check(f"{kernel}.{M}x{N}x{K}({epi_name}).y", y, ref["out"], e_out)
-
-
-# ---------------------------------------------------------------------------------- D. fused LayerNorm
-@pytest.mark.parametrize("M,N,K", [(5, 2048, 2048), (8, 2560, 2560), (1, 2048, 8192), (3, 72, 64)])
-def test_skinny_fused_layernorm_bounds(cuda, M, N, K):
-    """ln_out = LN(y) written by the last CTA, against a float64 LayerNorm of the kernel's own fp32 y."""
-    from ymp import ops
-    g = torch.Generator(device=cuda).manual_seed(N + K)
-    x = torch.randn(M, K, device=cuda, generator=g).to(bf16)
-    w = (torch.randn(N, K, device=cuda, generator=g) * K ** -0.5).to(bf16)
-    bias = torch.randn(N, device=cuda, generator=g).to(bf16)
-    res = torch.randn(M, N, device=cuda, generator=g) * 4 + 1
-    gamma = (1 + 0.5 * torch.randn(N, device=cuda, generator=g)).to(bf16)
-    beta = (0.5 * torch.randn(N, device=cuda, generator=g)).to(bf16)
-    ticket = torch.zeros(1, device=cuda, dtype=torch.int32)
-    y, ln_y = ops.gemm_skinny(x, w, bias=bias, residual=res, out_dtype=torch.float32, ln=(gamma, beta, 1e-5, ticket))
-    assert int(ticket) == 0
-    ref = GB.layernorm_reference(y, gamma, beta, 1e-5)[0]
-    _check(f"gemm_skinny.layernorm.{M}x{N}", ln_y, ref, GB.layernorm_bound(y, gamma, beta, 1e-5))

@@ -214,25 +214,17 @@ def test_gemm_skinny_rejects_wide_inputs(cuda):
 
 
 @pytest.mark.parametrize("M,N,K", [(5, 2048, 2048), (8, 2048, 8192), (1, 2560, 2560), (3, 72, 64)])
-def test_gemm_skinny_fused_layernorm_and_cache_row(cuda, M, N, K):
-    """The two fused outputs of the decoding step: LN(y) written by the last CTA (ymp_layernorm_fwd's formula on the same
-    y; only the fp32 summation order differs, so results agree to one bf16 ulp; the ticket counter resets itself) and the
-    second bf16 copy at a device-side row offset."""
+def test_gemm_skinny_cache_row(cuda, M, N, K):
+    """The decoding step's two epilogues: the fp32 residual-stream result y = x @ w^T + bias + res, and the second bf16
+    copy at a device-side row offset (the KV-cache row)."""
     from ymp import ops
     torch.manual_seed(N + K)
     x = torch.randn(M, K, device=cuda).bfloat16()
     w = (torch.randn(N, K, device=cuda) * K ** -0.5).bfloat16()
     bias = torch.randn(N, device=cuda).bfloat16()
     res = torch.randn(M, N, device=cuda)
-    gamma, beta = (1 + 0.1 * torch.randn(N, device=cuda)).bfloat16(), (0.1 * torch.randn(N, device=cuda)).bfloat16()
-    ticket = torch.zeros(1, device=cuda, dtype=torch.int32)
-    for _ in range(3):
-        y, ln_y = ops.gemm_skinny(x, w, bias=bias, residual=res, out_dtype=torch.float32, ln=(gamma, beta, 1e-5, ticket))
-        assert int(ticket) == 0
-        ref, _, _ = ops.layernorm_fwd(y, gamma, beta, 1e-5, stats=False)
-        assert (ln_y.float() - ref.float()).abs().max().item() <= 2 ** -7 * max(1.0, ref.float().abs().max().item())
-        assert (ln_y != ref).float().mean().item() < 0.02
-        _close(y, x.float() @ w.float().t() + bias.float() + res, tol=1e-4)
+    y = ops.gemm_skinny(x, w, bias=bias, residual=res, out_dtype=torch.float32)
+    _close(y, x.float() @ w.float().t() + bias.float() + res, tol=1e-4)
     ML = 7
     cache = torch.zeros(M * ML, N, device=cuda, dtype=torch.bfloat16)
     off = torch.tensor([4], device=cuda, dtype=torch.int64)

@@ -22,7 +22,7 @@ def test_abi_exports_every_declared_symbol():
     for n in sorted(names):
         assert hasattr(lib, n), f"{n} declared in include/ymp.h but not exported"
     lib.ymp_abi_version.restype = ctypes.c_int
-    assert lib.ymp_abi_version() == 3
+    assert lib.ymp_abi_version() == 4
 
 
 def test_ctypes_structs_match_header_field_order():

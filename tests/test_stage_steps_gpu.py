@@ -227,13 +227,12 @@ def test_component_path_walks(cuda, monkeypatch):
 
 # ---------------------------------------------------------------------------------- decoding
 GPT_HD128 = dict(port.GCFG_TINY, hidden_size=256, ffn_hidden_size=1024, num_attention_heads=2, max_position_embeddings=256)
-# case: (decoder config, clips, beam (0: sample), TokenStep's fused LayerNorms, step program kind)
+# case: (decoder config, clips, beam (0: sample), step program kind)
 DECODE_CASES = {
-    "1p3b_beam5": (GPT_1P3B, 1, 5, False, "skinny"),
-    "1p3b_beam5_fused_ln": (GPT_1P3B, 1, 5, True, "skinny_ln"),
-    "2p7b_12clips_beam5": (GPT_2P7B, 12, 5, False, "skinny"),
-    "1p3b_sample12": (GPT_1P3B, 12, 0, False, "gemm"),
-    "hd128_2clips_beam3": (GPT_HD128, 2, 3, False, "skinny"),
+    "1p3b_beam5": (GPT_1P3B, 1, 5, "skinny"),
+    "2p7b_12clips_beam5": (GPT_2P7B, 12, 5, "skinny"),
+    "1p3b_sample12": (GPT_1P3B, 12, 0, "gemm"),
+    "hd128_2clips_beam3": (GPT_HD128, 2, 3, "skinny"),
 }
 
 
@@ -264,7 +263,7 @@ def test_decode_walks(cuda, monkeypatch, case):
     at the 1.3B (32 x 64) and 2.7B (32 x 80) widths and at head_dim 128, Q = 128 prefix rows."""
     import models.modeling_distributed_gpt3 as M
     from ymp import engine, ops
-    gcfg, C, beam, fused_ln, kind = DECODE_CASES[case]
+    gcfg, C, beam, kind = DECODE_CASES[case]
     Q, L, n_new = 128, 8, 7
     H, V = gcfg["hidden_size"], gcfg["vocab_size"]
     dec = _decoder(cuda, gcfg, Q, n_new)
@@ -272,7 +271,6 @@ def test_decode_walks(cuda, monkeypatch, case):
     qf = (0.5 * torch.randn(C, Q, H, generator=g)).to(cuda, BF16)
     ids = torch.randint(0, V, (C, L), generator=g).to(cuda)
     monkeypatch.setenv("YMP_DECODE_GRAPH", "0")
-    monkeypatch.setenv("YMP_DECODE_FUSED_LN", "1" if fused_ln else "0")
     init = engine.KVCache.__init__
 
     def poisoned(cache, *a, **k):

@@ -467,8 +467,6 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 64, h = blockIdx.y, s = blockIdx.z;
   const int g = lane >> 2, t4 = lane & 3;
-  griddep_launch();   // (programmatic dependent launch in the decoding step; no-ops for an ordinary launch)
-  griddep_wait();
   int sq, skv;
   eff_len(p, s, sq, skv);
   if (q0 >= sq) return;
@@ -900,9 +898,7 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   // whole key range: bit-identical O and lse, and no key tile that is fully masked for a row.
   int qoff = p.mask == MASK_CAUSAL ? p.s_kv - p.s_q : 0;
   int q0 = blockIdx.x * 64 - (qoff & 63), a0 = q0 + qoff;  // first query row of the tile and its key position
-  griddep_launch();   // (programmatic dependent launch; no-ops for an ordinary launch)
-  griddep_wait();
-  if constexpr (TABLE) {  // (read after the wait: the table is an input like q / k / v)
+  if constexpr (TABLE) {
     qoff = __ldg(p.n_prefix + s / p.mkv.seq_div);
     q0 = blockIdx.x * 64 - (qoff & 63);
     a0 = q0 + qoff;
@@ -1117,8 +1113,6 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
   float* m_part = l_part + 128;                                              // [4]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int h = blockIdx.x, s = blockIdx.y;
-  griddep_launch();
-  griddep_wait();
   const int* table = p.kv_rows ? p.kv_rows + s * p.kv_rows_ld : nullptr;
   // with a table, mrow(Mk, r) is plain physical row r of k (and of v for Mv)
   const RSeq mkv = table ? RSeq{0, 1, 0, 0} : resolve(p.mkv, s);
@@ -1259,15 +1253,12 @@ static int for_head_dim(int head_dim, F&& launch) {
   if constexpr (WITH_128) return launch(HeadDim<128>{});
   else return set_error(YMP_EINVAL, "attention: no kernel of this family for head_dim %d", head_dim);
 }
-// One launch of 128 threads with `smem` bytes of dynamic shared memory (opted in once per device and kernel).  PDL: the
-// kernel calls griddep_wait before it reads its inputs, so it goes through launch_k, which honours ymp_set_pdl.  The
-// backward kernels never wait on the previous grid and must take an ordinary launch.
-template <void (*K)(AttnKParams), bool PDL>
+// One launch of 128 threads with `smem` bytes of dynamic shared memory (opted in once per device and kernel).
+template <void (*K)(AttnKParams)>
 static int launch_attn(dim3 grid, int smem, cudaStream_t st, const AttnKParams& p) {
   static DeviceOnce once;
   if (once.first()) { YMP_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); }
-  if constexpr (PDL) launch_k(K, grid, dim3(128), smem, st, p);
-  else K<<<grid, 128, smem, st>>>(p);
+  K<<<grid, 128, smem, st>>>(p);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }
@@ -1275,7 +1266,7 @@ static int launch_attn(dim3 grid, int smem, cudaStream_t st, const AttnKParams& 
 static int launch_decode(const AttnKParams& p, int head_dim, cudaStream_t st) {
   return for_head_dim<false>(head_dim, [&](auto hd) {
     constexpr int D = decltype(hd)::D;
-    return launch_attn<attn_decode_kernel<D>, true>(dim3(p.n_heads, p.n_seq), (128 * (D + 1) + 128 + 4) * 4, st, p);
+    return launch_attn<attn_decode_kernel<D>>(dim3(p.n_heads, p.n_seq), (128 * (D + 1) + 128 + 4) * 4, st, p);
   });
 }
 static int launch_wg_fwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
@@ -1283,7 +1274,7 @@ static int launch_wg_fwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
   const dim3 grid((p.s_q + lead + 63) / 64, p.n_heads, p.n_seq);
   return for_head_dim<false>(head_dim, [&](auto hd) {
     using H = decltype(hd);
-    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO>, true>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
+    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO>>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
   });
 }
 // The per-sequence prefix is only known on the device, so the grid has (s_q + 63 + 63) / 64 query tiles: enough for
@@ -1293,31 +1284,31 @@ static int launch_wg_fwd_table(const AttnKParams& p, int head_dim, cudaStream_t 
   const dim3 grid((p.s_q + 126) / 64, p.n_heads, p.n_seq);
   return for_head_dim<false>(head_dim, [&](auto hd) {
     using H = decltype(hd);
-    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO, true, CACHE>, true>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
+    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO, true, CACHE>>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
   });
 }
 static int launch_wg_bwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
   return for_head_dim<false>(head_dim, [&](auto hd) {
     using H = decltype(hd);
     const int smem = 6 * WgTile<H::D>::BYTES + 1024 + 1024;
-    const int rc = launch_attn<attn_wg_bwd_dq_kernel<H::D, H::DIO>, false>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
+    const int rc = launch_attn<attn_wg_bwd_dq_kernel<H::D, H::DIO>>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
     if (rc) return rc;
-    return launch_attn<attn_wg_bwd_dkdv_kernel<H::D, H::DIO>, false>(dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
+    return launch_attn<attn_wg_bwd_dkdv_kernel<H::D, H::DIO>>(dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
   });
 }
 static int launch_fwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
   return for_head_dim<true>(head_dim, [&](auto hd) {
     using H = decltype(hd);
-    return launch_attn<attn_fwd_kernel<H::D, H::DIO>, true>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), 5 * 64 * (H::D + 8) * 2, st, p);
+    return launch_attn<attn_fwd_kernel<H::D, H::DIO>>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), 5 * 64 * (H::D + 8) * 2, st, p);
   });
 }
 static int launch_bwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
   return for_head_dim<true>(head_dim, [&](auto hd) {
     using H = decltype(hd);
     const int smem = 6 * 64 * (H::D + 8) * 2 + 1024;
-    const int rc = launch_attn<attn_bwd_dq_kernel<H::D, H::DIO>, false>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
+    const int rc = launch_attn<attn_bwd_dq_kernel<H::D, H::DIO>>(dim3((p.s_q + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
     if (rc) return rc;
-    return launch_attn<attn_bwd_dkdv_kernel<H::D, H::DIO>, false>(dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
+    return launch_attn<attn_bwd_dkdv_kernel<H::D, H::DIO>>(dim3((p.s_kv + 63) / 64, p.n_heads, p.n_seq), smem, st, p);
   });
 }
 

@@ -6,7 +6,6 @@ namespace ymp {
 
 static thread_local char g_err[512] = "";
 std::atomic<uint64_t> g_launches{0};
-thread_local int g_pdl = 0;
 int g_deterministic = 0;
 
 int set_error(int code, const char* fmt, ...) {
@@ -34,8 +33,7 @@ int num_sms() {
 
 extern "C" {
 const char* ymp_last_error(void) { return ymp::g_err; }
-int ymp_abi_version(void) { return 3; }
+int ymp_abi_version(void) { return 4; }
 uint64_t ymp_launch_count(void) { return ymp::g_launches.load(std::memory_order_relaxed); }
-int ymp_set_pdl(int on) { const int prev = ymp::g_pdl; ymp::g_pdl = on ? 1 : 0; return prev; }
 int ymp_set_deterministic(int on) { const int prev = ymp::g_deterministic; ymp::g_deterministic = on ? 1 : 0; return prev; }
 }

@@ -16,22 +16,6 @@ extern std::atomic<uint64_t> g_launches;
 inline void count_launch(uint64_t n = 1) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int num_sms();  // SM count of the current device (cached)
 
-// Programmatic dependent launch (PDL) for the latency-bound decoding step: when on (ymp_set_pdl, thread-local), launch_k
-// adds cudaLaunchAttributeProgrammaticStreamSerialization, so the kernel may start while its predecessor in the stream is
-// still draining; the kernels launched this way call griddep_wait() (ptx.cuh) before they touch anything the predecessor
-// wrote and griddep_launch() as early as possible.  Off: an ordinary launch (the two instructions are then no-ops).
-extern thread_local int g_pdl;
-template <typename... KArgs, typename... Args>
-inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = g_pdl ? 1 : 0;
-  (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);  // errors surface in YMP_LAUNCH_CHECK
-}
-
 // Deterministic mode (ymp_set_deterministic, process-wide): the launchers of the four order-dependent sums (split-K
 // GEMM, LayerNorm gamma/beta gradients, column sums, sum of squares) then write one partial per CTA to a caller-provided
 // workspace and add the partials to the output in index order (ordered_sum below) instead of by atomics.  Read when a

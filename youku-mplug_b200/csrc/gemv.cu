@@ -16,7 +16,7 @@
 //     8..15 of the group.  Every output element sees the same MMA chain and the same epilogue as in an M <= 8 call, so
 //     row r of an M-row call is bit-identical to the same row computed alone;
 //   * the 8 warps of a CTA are `ksplit` K-slices x (8 / ksplit) column tiles (ksplit depends on N and K only); every lane
-//     keeps UNROLL k-blocks (UNROLL x 16 bytes of weights) in flight;
+//     keeps SK_UNROLL = 4 k-blocks (4 x 16 bytes of weights) in flight;
 //   * partial sums meet in shared memory and are added in slice order; lane (g, t) of the slice-0 warp owns (row g (+8,
 //     +16, ...), columns n0+2t, n0+2t+1) and applies
 //       v = acc + bias[n] ; v = gelu(v) (optional) ; v += residual[m, n] (bf16 or fp32) ; store bf16 or fp32
@@ -28,9 +28,12 @@
 
 namespace ymp {
 
-constexpr int SK_MAXM = 8, SK_TILE_N = 8, SK_WARPS = 8;
+constexpr int SK_MAXM = 8, SK_TILE_N = 8, SK_WARPS = 8, SK_UNROLL = 4;
 constexpr int SK_WIDE_MAXM = 64, SK_WIDE_GROUPS = SK_WIDE_MAXM / 16;
 
+// Both kernels take it as __grid_constant__: the epilogue then reads each field from the parameter bank where it uses
+// it.  From a by-value copy the compiler unswitches the k-block loop and the epilogue on the fields (several times the
+// code, 114 instead of 84 registers in the wide kernel).
 struct SkinnyParams {
   const __nv_bfloat16* x;
   const __nv_bfloat16* w;
@@ -42,87 +45,7 @@ struct SkinnyParams {
   long long ldy2, y2_stride;
   int M, N, K, ldx, ldw, ldr, ldy;
   int act, res_f32, out_f32, ksplit;
-  const __nv_bfloat16* ln_gamma;
-  const __nv_bfloat16* ln_beta;
-  __nv_bfloat16* ln_out;
-  unsigned int* ln_counter;
-  int ld_ln;
-  float ln_eps;
 };
-
-// LayerNorm of all M rows of the finished fp32 result by the whole (last) CTA, read back from L2 (ld.cg: other CTAs
-// wrote it).  Three passes (sum, squared deviations, normalise), each with every load of every row in flight at once -
-// three L2 round trips on the critical path, not one per 8-element chunk.  Same formula as ln_fwd_kernel (layernorm.cu):
-// mean = sum / N, rstd = rsqrt(sum((x - mean)^2) / N + eps), y = ((x - mean) * rstd) * gamma + beta.
-template <int PASS>
-__device__ __forceinline__ void skinny_ln_pass(const SkinnyParams& p, const float* mu, const float* rs, float* red) {
-  const int nvec = p.N >> 3, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float acc[SK_MAXM];
-#pragma unroll
-  for (int m = 0; m < SK_MAXM; ++m) acc[m] = 0.f;
-  for (int vi = threadIdx.x; vi < nvec; vi += SK_WARPS * 32) {
-    float4 a[SK_MAXM], b[SK_MAXM];
-#pragma unroll
-    for (int m = 0; m < SK_MAXM; ++m) {
-      if (m < p.M) {
-        const float4* yr = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.y) + (size_t)m * p.ldy) + 2 * vi;
-        a[m] = __ldcg(yr); b[m] = __ldcg(yr + 1);
-      }
-    }
-    uint4 gv, bv;
-    if (PASS == 2) { gv = __ldg(reinterpret_cast<const uint4*>(p.ln_gamma) + vi); bv = __ldg(reinterpret_cast<const uint4*>(p.ln_beta) + vi); }
-#pragma unroll
-    for (int m = 0; m < SK_MAXM; ++m) {
-      if (m < p.M) {
-        const float v[8] = {a[m].x, a[m].y, a[m].z, a[m].w, b[m].x, b[m].y, b[m].z, b[m].w};
-        if (PASS == 0) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) acc[m] += v[e];
-        } else if (PASS == 1) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) { const float d = v[e] - mu[m]; acc[m] += d * d; }
-        } else {
-          const uint32_t* gp = &gv.x; const uint32_t* bp = &bv.x;
-          uint32_t o[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            o[e] = pack_bf16(fmaf((v[2 * e] - mu[m]) * rs[m], bf16_lo(gp[e]), bf16_lo(bp[e])),
-                             fmaf((v[2 * e + 1] - mu[m]) * rs[m], bf16_hi(gp[e]), bf16_hi(bp[e])));
-          reinterpret_cast<uint4*>(p.ln_out + (size_t)m * p.ld_ln)[vi] = make_uint4(o[0], o[1], o[2], o[3]);
-        }
-      }
-    }
-  }
-  if (PASS < 2) {
-#pragma unroll
-    for (int m = 0; m < SK_MAXM; ++m) {
-      const float t = warp_sum(acc[m]);
-      if (lane == 0) red[warp * SK_MAXM + m] = t;
-    }
-    __syncthreads();
-  }
-}
-__device__ __forceinline__ void skinny_ln_rows(const SkinnyParams& p, float* red /* [SK_WARPS * SK_MAXM] */) {
-  float mu[SK_MAXM], rs[SK_MAXM];
-  skinny_ln_pass<0>(p, mu, rs, red);
-#pragma unroll
-  for (int m = 0; m < SK_MAXM; ++m) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < SK_WARPS; ++w) t += red[w * SK_MAXM + m];
-    mu[m] = t / (float)p.N;
-  }
-  __syncthreads();
-  skinny_ln_pass<1>(p, mu, rs, red);
-#pragma unroll
-  for (int m = 0; m < SK_MAXM; ++m) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < SK_WARPS; ++w) t += red[w * SK_MAXM + m];
-    rs[m] = rsqrtf(t / (float)p.N + p.ln_eps);
-  }
-  skinny_ln_pass<2>(p, mu, rs, red);
-}
 
 // Epilogue of result row m, columns n, n + 1 (the accumulators of one lane): identical for both kernels
 __device__ __forceinline__ void skinny_store(const SkinnyParams& p, int m, int n_base, float acc0, float acc1) {
@@ -151,8 +74,7 @@ __device__ __forceinline__ void mma16816_bf16(float (&c)[4], uint32_t a0, uint32
       : "r"(a0), "r"(0u), "r"(a2), "r"(b0), "r"(b1));
 }
 
-template <int SK_UNROLL, bool LN>
-__global__ void __launch_bounds__(SK_WARPS * 32, (LN ? 2 : 1)) gemm_skinny_kernel(const SkinnyParams p) {
+__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_kernel(const __grid_constant__ SkinnyParams p) {
   __shared__ float part[SK_WARPS][64];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, t = lane & 3;
@@ -160,7 +82,6 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (LN ? 2 : 1)) gemm_skinny_kerne
   const int n0 = tile * SK_TILE_N;
   const bool live = n0 < p.N;
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
-  griddep_launch();
   if (live) {
     // 16-byte chunks of the K dimension: chunk c = elements [8c, 8c+8); a k-block is 4 chunks (one per t)
     const int nchunk = p.K >> 3, nblk = (nchunk + 3) >> 2;
@@ -185,10 +106,7 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (LN ? 2 : 1)) gemm_skinny_kerne
         xd[u] = ((b + u) < b_hi && c < nchunk && xrow) ? __ldg(xr + c) : make_uint4(0, 0, 0, 0);
       }
     };
-    // the weights do not depend on the previous kernel of the stream: their first batch is already in flight while that
-    // kernel drains (programmatic dependent launch); the activations are read only after it has completed
     fetch_w(b_lo, wv);
-    griddep_wait();
     fetch_x(b_lo, xv);
     for (int b = b_lo; b < b_hi; b += SK_UNROLL) {
       uint4 wn[SK_UNROLL], xn[SK_UNROLL];
@@ -202,8 +120,6 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (LN ? 2 : 1)) gemm_skinny_kerne
 #pragma unroll
       for (int u = 0; u < SK_UNROLL; ++u) { wv[u] = wn[u]; xv[u] = xn[u]; }
     }
-  } else {
-    griddep_wait();
   }
   // acc[0], acc[1] = (row g, columns n0 + 2t, n0 + 2t + 1) summed over this warp's K slice
   if (ks > 1) {
@@ -213,31 +129,14 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (LN ? 2 : 1)) gemm_skinny_kerne
     if (kpart == 0)
       for (int j = 1; j < ks; ++j) { acc[0] += part[warp + j][2 * lane]; acc[1] += part[warp + j][2 * lane + 1]; }
   }
-  if (live && kpart == 0 && g < p.M) {
-    skinny_store(p, g, n0 + 2 * t, acc[0], acc[1]);
-    if (LN) __threadfence();   // this thread's rows are visible device-wide before its CTA takes a ticket
-  }
-  if constexpr (LN) {
-    // fused LayerNorm: the CTA that takes the last ticket sees every other CTA's rows (writers' fences + atomic) and
-    // normalises them
-    __shared__ unsigned int ticket;
-    __syncthreads();
-    if (threadIdx.x == 0) ticket = atomicAdd(p.ln_counter, 1u);
-    __syncthreads();
-    if (ticket == gridDim.x - 1) {
-      __threadfence();
-      skinny_ln_rows(p, &part[0][0]);
-      if (threadIdx.x == 0) *p.ln_counter = 0u;
-    }
-  }
+  if (live && kpart == 0 && g < p.M) skinny_store(p, g, n0 + 2 * t, acc[0], acc[1]);
 }
 
-// 9 <= M <= 64: gemm_skinny_kernel's grid, warp roles, K slices, weight stream and k-block loop (SK_UNROLL = 4, the same
-// zero-padded tail), with one accumulator set per group of 16 rows.  Group j's lane (g, t) holds rows 16j + g (acc[j][0..1])
+// 9 <= M <= 64: gemm_skinny_kernel's grid, warp roles, K slices, weight stream and k-block loop (the same zero-padded
+// tail), with one accumulator set per group of 16 rows.  Group j's lane (g, t) holds rows 16j + g (acc[j][0..1])
 // and 16j + 8 + g (acc[j][2..3]).  The activation chunks of the k-block being consumed are loaded from global memory
 // (L2-resident: every CTA reads them) next to the MMAs; only the weights are double-buffered in registers.
-template <int SK_UNROLL>
-__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(const SkinnyParams p) {
+__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(const __grid_constant__ SkinnyParams p) {
   __shared__ float part[SK_WARPS][32 * 4 * SK_WIDE_GROUPS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, t = lane & 3;
@@ -248,7 +147,6 @@ __global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(cons
   float acc[SK_WIDE_GROUPS][4];
 #pragma unroll
   for (int j = 0; j < SK_WIDE_GROUPS; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
-  griddep_launch();
   if (live) {
     const int nchunk = p.K >> 3, nblk = (nchunk + 3) >> 2;
     const int b_lo = (int)((long)nblk * kpart / ks), b_hi = (int)((long)nblk * (kpart + 1) / ks);
@@ -267,7 +165,6 @@ __global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(cons
                                                  : make_uint4(0, 0, 0, 0);
     };
     fetch_w(b_lo, wv);
-    griddep_wait();
     for (int b = b_lo; b < b_hi; b += SK_UNROLL) {
       uint4 wn[SK_UNROLL];
       fetch_w(b + SK_UNROLL, wn);
@@ -287,8 +184,6 @@ __global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(cons
 #pragma unroll
       for (int u = 0; u < SK_UNROLL; ++u) wv[u] = wn[u];
     }
-  } else {
-    griddep_wait();
   }
   if (ks > 1) {
 #pragma unroll
@@ -321,7 +216,6 @@ static int gemm_skinny_call(const ymp_gemm_skinny_args* a, void* stream, int max
   YMP_CHECK_ARG(a && a->x && a->w && a->y, "ymp_gemm_skinny: null pointer");
   YMP_CHECK_ARG(a->M >= 1 && a->M <= max_m && a->N > 0 && a->K > 0 && a->K % 8 == 0, "ymp_gemm_skinny%s: needs 1 <= M <= %d, K %% 8 == 0 (M=%d K=%d)",
                 max_m > SK_MAXM ? "_wide" : "", max_m, a->M, a->K);
-  YMP_CHECK_ARG(!a->ln_out || a->M <= SK_MAXM, "ymp_gemm_skinny_wide: the fused LayerNorm (ln_out) needs M <= 8 (M=%d)", a->M);
   YMP_CHECK_ARG(a->ldx % 8 == 0 && a->ldw % 8 == 0 && a->ldx >= a->K && a->ldw >= a->K && aligned16(a->x) && aligned16(a->w), "ymp_gemm_skinny: x / w rows must be 16-byte aligned");
   YMP_CHECK_ARG(a->act >= 0 && a->act <= 2, "ymp_gemm_skinny: bad act");
   SkinnyParams p;
@@ -330,29 +224,17 @@ static int gemm_skinny_call(const ymp_gemm_skinny_args* a, void* stream, int max
   YMP_CHECK_ARG(!a->y2 || (a->y2_off_dev && a->out_dtype == YMP_DT_BF16), "ymp_gemm_skinny: y2 needs y2_off_dev and a bf16 result");
   p.y2 = (__nv_bfloat16*)a->y2; p.y2_off = (const long long*)a->y2_off_dev; p.ldy2 = a->ldy2; p.y2_stride = a->y2_off_stride;
   p.M = a->M; p.N = a->N; p.K = a->K; p.ldx = a->ldx; p.ldw = a->ldw; p.ldr = a->ldr; p.ldy = a->ldy;
-  const bool ln = a->ln_out != nullptr;
-  YMP_CHECK_ARG(!ln || (a->ln_gamma && a->ln_beta && a->ln_counter && a->out_dtype == YMP_DT_F32 && a->N % 8 == 0 && a->ld_ln % 8 == 0 &&
-                        a->ldy % 4 == 0 && aligned16(a->y) && aligned16(a->ln_out) && aligned16(a->ln_gamma) && aligned16(a->ln_beta)),
-                "ymp_gemm_skinny: fused LayerNorm needs gamma/beta/counter, an fp32 result, N %% 8 == 0 and 16-byte aligned rows");
-  p.ln_gamma = (const __nv_bfloat16*)a->ln_gamma; p.ln_beta = (const __nv_bfloat16*)a->ln_beta; p.ln_out = (__nv_bfloat16*)a->ln_out;
-  p.ln_counter = a->ln_counter; p.ld_ln = a->ld_ln; p.ln_eps = a->ln_eps;
   p.act = a->act; p.res_f32 = a->residual_dtype == YMP_DT_F32; p.out_f32 = a->out_dtype == YMP_DT_F32;
   // K slices per CTA (the warps of a CTA that share one 8-column tile): as many as leave >= 4 k-blocks of 32 per slice
   int ks = 1;
-  static const int force = [] { const char* e = getenv("YMP_SKINNY_KSPLIT"); return e ? atoi(e) : 0; }();
   const int ks_max = a->N <= 4096 ? 8 : 4;   // wide outputs get fewer K slices per CTA (more column tiles)
   while (ks < ks_max && a->K / (2 * ks) >= 128) ks *= 2;
-  if (force == 1 || force == 2 || force == 4 || force == 8) ks = force;
   p.ksplit = ks;
   const int tiles = (a->N + SK_TILE_N - 1) / SK_TILE_N, tiles_per_cta = SK_WARPS / ks;
   const int blocks = (tiles + tiles_per_cta - 1) / tiles_per_cta;
-  static const int unroll = [] { const char* e = getenv("YMP_SKINNY_UNROLL"); return e ? atoi(e) : 4; }();
   cudaStream_t st = (cudaStream_t)stream;
-  if (a->M > SK_MAXM) launch_k(gemm_skinny_wide_kernel<4>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
-  else if (ln) launch_k(gemm_skinny_kernel<4, true>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
-  else if (unroll == 8) launch_k(gemm_skinny_kernel<8, false>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
-  else if (unroll == 2) launch_k(gemm_skinny_kernel<2, false>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
-  else launch_k(gemm_skinny_kernel<4, false>, dim3(blocks), dim3(SK_WARPS * 32), 0, st, p);
+  if (a->M > SK_MAXM) gemm_skinny_wide_kernel<<<blocks, SK_WARPS * 32, 0, st>>>(p);
+  else gemm_skinny_kernel<<<blocks, SK_WARPS * 32, 0, st>>>(p);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }

@@ -47,8 +47,6 @@ __device__ __forceinline__ void load8(const void* base, size_t row, int ld, int 
 // VPL = 8-element vectors per lane (D <= VPL*256)
 template <int VPL, bool XF32>
 __global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_kernel(const LnParams p) {
-  griddep_launch();   // (programmatic dependent launch in the decoding step; no-ops for an ordinary launch)
-  griddep_wait();
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int nvec = p.D >> 3;
@@ -350,13 +348,13 @@ extern "C" int ymp_layernorm_fwd(const ymp_layernorm_args* a, void* stream) {
   const int vpl = (a->D / 8 + 31) / 32;
   const int thr = LN_WARPS * 32;
   if (a->x_dtype == YMP_DT_F32) {
-    if (vpl <= 3) launch_k(ln_fwd_kernel<3, true>, dim3(blocks), dim3(thr), 0, st, p);
-    else if (vpl <= 8) launch_k(ln_fwd_kernel<8, true>, dim3(blocks), dim3(thr), 0, st, p);
-    else launch_k(ln_fwd_kernel<16, true>, dim3(blocks), dim3(thr), 0, st, p);
+    if (vpl <= 3) ln_fwd_kernel<3, true><<<blocks, thr, 0, st>>>(p);
+    else if (vpl <= 8) ln_fwd_kernel<8, true><<<blocks, thr, 0, st>>>(p);
+    else ln_fwd_kernel<16, true><<<blocks, thr, 0, st>>>(p);
   } else {
-    if (vpl <= 3) launch_k(ln_fwd_kernel<3, false>, dim3(blocks), dim3(thr), 0, st, p);
-    else if (vpl <= 8) launch_k(ln_fwd_kernel<8, false>, dim3(blocks), dim3(thr), 0, st, p);
-    else launch_k(ln_fwd_kernel<16, false>, dim3(blocks), dim3(thr), 0, st, p);
+    if (vpl <= 3) ln_fwd_kernel<3, false><<<blocks, thr, 0, st>>>(p);
+    else if (vpl <= 8) ln_fwd_kernel<8, false><<<blocks, thr, 0, st>>>(p);
+    else ln_fwd_kernel<16, false><<<blocks, thr, 0, st>>>(p);
   }
   YMP_LAUNCH_CHECK();
   return YMP_OK;

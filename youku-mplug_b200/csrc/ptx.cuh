@@ -133,10 +133,6 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
 }
 
 // ---------------------------------------------------------------- small math helpers
-// programmatic dependent launch: wait until the preceding kernel of the stream has completed and its writes are visible
-// (returns at once for an ordinary launch); allow the following kernel to start launching
-__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void griddep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 // streaming 128-bit load that does not allocate in L1 (weights read exactly once)
 __device__ __forceinline__ uint4 ld_nc_v4(const uint4* p) {
   uint4 v;

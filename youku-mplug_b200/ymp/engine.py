@@ -21,7 +21,6 @@ import math
 
 import torch
 
-from . import lib as L
 from . import ops
 from .ops import ACT_GELU_ERF, ACT_GELU_TANH, TView, bf16
 
@@ -918,48 +917,23 @@ class TokenStep:
         self.cache, self.W, self.sig, self.static = cache, W, sig, static
         self.emb_in = torch.zeros((cache.B, g.H), device=dev, dtype=emb_dtype)
         self.stage = torch.zeros((cache.B, 3 * g.H), device=dev, dtype=bf16)   # the new token's [q|k|v] row per sequence
-        self.ticket = torch.zeros(1, device=dev, dtype=torch.int32)            # last-CTA ticket of the fused LayerNorms
         self.graph = None
         self.out = None
         self.warm = False
 
     def body(self):
-        """Enqueue the step on the current stream (eagerly or under capture): reads emb_in, returns (hid, logits).
-        YMP_DECODE_PDL=1 chains the kernels by programmatic dependent launch (each may start - and the GEMMs already
-        stream their first weights - while the previous one drains).  Off by default: inside the captured graph it
-        has not been shown to help."""
-        import os
-        prev = L.set_pdl(os.environ.get("YMP_DECODE_PDL", "0") == "1")
-        try:
-            return self._body()
-        finally:
-            L.set_pdl(prev)
-
-    def _body(self):
+        """Enqueue the step on the current stream (eagerly or under capture): reads emb_in, returns (hid, logits)."""
         c, W = self.cache, self.W
         g, B, ML = c.g, c.B, c.max_len
         H, hd = g.H, g.hd
         pos = W[GPT + "embedding.position_embeddings.weight"]
         x = self.emb_in.float() + pos.index_select(0, c.len_idx).float()
         mkv = ops.dense_map(ML)
-
-        import os
-        # YMP_DECODE_FUSED_LN=1: every LayerNorm but the first is computed by the last CTA of the GEMM that completes its
-        # input (one kernel boundary less per sub-layer).  Off by default: the ticket + three L2 round trips of the tail
-        # cost about what the stand-alone kernel and its launch gap cost.
-        # The fused LayerNorm serves at most ops.SKINNY_MAX_ROWS rows.
-        fused_ln = os.environ.get("YMP_DECODE_FUSED_LN", "0") == "1" and B <= ops.SKINNY_MAX_ROWS
         # more rows than ymp_gemm_skinny takes (a batched beam search): the wide entry point, same per-row results
         skinny = ops.gemm_skinny if B <= ops.SKINNY_MAX_ROWS else ops.gemm_skinny_wide
 
-        def ln_of(prefix):
-            return (W[prefix + ".weight"], W[prefix + ".bias"], g.eps, self.ticket)
-
         def gemm_ln(a, wname, residual, ln_prefix):
             """fp32 residual-stream GEMM followed by the LayerNorm of its complete result: (y, LN(y))."""
-            if fused_ln:  # the LayerNorm is computed by the GEMM's last CTA
-                return skinny(a, W[wname + ".weight"], bias=W[wname + ".bias"], residual=residual, out_dtype=torch.float32,
-                              ln=ln_of(ln_prefix))
             y = skinny(a, W[wname + ".weight"], bias=W[wname + ".bias"], residual=residual, out_dtype=torch.float32)
             return y, ops.layernorm_fwd(y, W[ln_prefix + ".weight"], W[ln_prefix + ".bias"], g.eps, stats=False)[0]
 

@@ -102,9 +102,7 @@ class GemmSkinnyArgs(C.Structure):
     _fields_ = [("x", c_vp), ("w", c_vp), ("bias", c_vp), ("residual", c_vp), ("y", c_vp),
                 ("M", c_i32), ("N", c_i32), ("K", c_i32), ("ldx", c_i32), ("ldw", c_i32), ("ldr", c_i32), ("ldy", c_i32),
                 ("act", c_i32), ("residual_dtype", c_i32), ("out_dtype", c_i32),
-                ("y2", c_vp), ("y2_off_dev", c_vp), ("ldy2", C.c_int64), ("y2_off_stride", C.c_int64),
-                ("ln_gamma", c_vp), ("ln_beta", c_vp), ("ln_out", c_vp), ("ln_counter", c_vp), ("ld_ln", c_i32),
-                ("ln_eps", C.c_float)]
+                ("y2", c_vp), ("y2_off_dev", c_vp), ("ldy2", C.c_int64), ("y2_off_stride", C.c_int64)]
 
 
 class AttnBwdArgs(C.Structure):
@@ -162,8 +160,6 @@ lib.ymp_last_error.restype = C.c_char_p
 lib.ymp_abi_version.restype = C.c_int
 lib.ymp_launch_count.restype = C.c_uint64
 lib.ymp_attn_last_path.restype = C.c_int
-lib.ymp_set_pdl.restype = C.c_int
-lib.ymp_set_pdl.argtypes = [C.c_int]
 lib.ymp_set_deterministic.restype = C.c_int
 lib.ymp_set_deterministic.argtypes = [C.c_int]
 ATTN_PATH_MMA_SYNC, ATTN_PATH_WGMMA, ATTN_PATH_SMALL, ATTN_PATH_DECODE = 0, 1, 2, 3
@@ -224,12 +220,6 @@ def check(rc, what):
 
 def launch_count():
     return int(lib.ymp_launch_count())
-
-
-def set_pdl(on):
-    """Programmatic dependent launch for this thread's next skinny-GEMM / LayerNorm / mma.sync attention launches
-    (the decoding step).  Returns the previous setting."""
-    return int(lib.ymp_set_pdl(int(bool(on))))
 
 
 def deterministic_mode(enabled, warn_only):

@@ -125,25 +125,23 @@ SKINNY_WIDE_MAX_ROWS = 64  # rows of ymp_gemm_skinny_wide (a batched beam search
 
 
 def gemm_skinny(x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_dtype=bf16, out2=None, out2_row_stride=0,
-                out2_off=None, ln=None):
+                out2_off=None):
     """y[M, N] = act(x[M, K] @ w[N, K]^T + bias) + residual for M <= 8 rows (single-token decoding): one pass over
     the weights on the HBM-bound kernel of csrc/gemv.cu instead of a mostly empty 128-row tensor-core tile.
     out2 [R, N] bf16 with out2_off (int64 device scalar): result row m is also written to out2 row
-    m * out2_row_stride + out2_off (the KV-cache row at the device-side cache length).
-    ln = (gamma, beta, eps, counter): also returns LN(y) [M, N] bf16, computed inside the same kernel by the CTA that
-    finishes last (counter: uint32/int32 device scalar, zero at launch, reset by the kernel); result is then (y, ln_y)."""
-    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, ln, wide=False)
+    m * out2_row_stride + out2_off (the KV-cache row at the device-side cache length)."""
+    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, wide=False)
 
 
 def gemm_skinny_wide(x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_dtype=bf16, out2=None, out2_row_stride=0,
-                     out2_off=None, ln=None):
+                     out2_off=None):
     """gemm_skinny for up to SKINNY_WIDE_MAX_ROWS = 64 rows (ymp_gemm_skinny_wide): M <= 8 runs gemm_skinny's launch,
     9 <= M <= 64 a kernel with the same per-element arithmetic, so row m of the result is bit-identical to the same row
-    computed by gemm_skinny.  The library rejects ln with more than 8 rows and any call with more than 64."""
-    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, ln, wide=True)
+    computed by gemm_skinny.  The library rejects any call with more than 64."""
+    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, wide=True)
 
 
-def _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, ln, wide):
+def _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, wide):
     _chk2d(x, "x"); _chk2d(w, "w")
     assert x.dtype == bf16 and w.dtype == bf16 and x.shape[1] == w.shape[1] and (wide or x.shape[0] <= SKINNY_MAX_ROWS)
     M, K, N = x.shape[0], x.shape[1], w.shape[0]
@@ -166,19 +164,11 @@ def _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_strid
         assert out2.shape[0] >= (M - 1) * out2_row_stride + 1
         a.y2, a.y2_off_dev = out2.data_ptr(), out2_off.data_ptr()
         a.ldy2, a.y2_off_stride = out2_row_stride * out2.stride(0), out2.stride(0)
-    ln_out = None
-    if ln is not None:
-        gamma, beta, eps, counter = ln
-        assert out.dtype == torch.float32 and gamma.dtype == bf16 and beta.dtype == bf16 and counter.numel() == 1
-        assert counter.dtype in (torch.int32, torch.uint32) and gamma.numel() == N and beta.numel() == N
-        ln_out = torch.empty((M, N), device=x.device, dtype=bf16)
-        a.ln_gamma, a.ln_beta, a.ln_out, a.ln_counter = gamma.data_ptr(), beta.data_ptr(), ln_out.data_ptr(), counter.data_ptr()
-        a.ld_ln, a.ln_eps = ln_out.stride(0), eps
     if wide:
         L.call(L._gemm_skinny_wide, a, "ymp_gemm_skinny_wide")
     else:
         L.call(L._gemm_skinny, a, "ymp_gemm_skinny")
-    return out if ln is None else (out, ln_out)
+    return out
 
 
 # ---------------------------------------------------------------------------------- LayerNorm
@@ -376,8 +366,7 @@ def patch_embed_gemm(video, weight2d, P, **kw):
 
 
 def fused_im2col_ok(T, P):
-    import os
-    return os.environ.get("YMP_FUSED_IM2COL", "1") != "0" and P == 16 and T % 8 == 0 and 128 % T == 0
+    return P == 16 and T % 8 == 0 and 128 % T == 0
 
 
 def im2col(video, P, out=None):

@@ -140,8 +140,7 @@ class TrainEngine:
         # utils.py:528-529): the contiguous flat ranges of each TimeSformer block (>= 1 MB) are all-reduced as
         # soon as the block's backward has produced them, on NCCL's own stream, while the remaining blocks still
         # run; everything else (abstractor, embeddings, biases: the gaps) goes in step().
-        import os
-        self.overlap_comm = overlap_comm and self.world > 1 and os.environ.get("YMP_OVERLAP_COMM", "1") != "0"   # (env: A/B knob)
+        self.overlap_comm = overlap_comm and self.world > 1
         self._buckets, self._pending, self._reduced = {}, [], []
         if self.overlap_comm:
             self._buckets = plan_buckets(spans)
