@@ -173,6 +173,12 @@ typedef struct ymp_gemm_skinny_args {
 } ymp_gemm_skinny_args;
 int ymp_gemm_skinny(const ymp_gemm_skinny_args* a, void* stream);
 int ymp_gemm_skinny_wide(const ymp_gemm_skinny_args* a, void* stream);
+/* ymp_gemm_skinny / ymp_gemm_skinny_wide with one second-copy row offset per result row: row m is also written to
+ * y2[m * ldy2 + y2_row_off[m] * y2_off_stride + n], y2_row_off a DEVICE int64 array [M] (the KV-cache rows of a decoding
+ * step whose sequences sit at different cache lengths).  Needs y2 and a bf16 result; a->y2_off_dev must be NULL.  The
+ * product and the first copy are those of the scalar-offset call. */
+int ymp_gemm_skinny_rows(const ymp_gemm_skinny_args* a, const int64_t* y2_row_off, void* stream);
+int ymp_gemm_skinny_wide_rows(const ymp_gemm_skinny_args* a, const int64_t* y2_row_off, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * LayerNorm (fp32 statistics, bf16 in/out), one warp per row.
@@ -290,6 +296,13 @@ typedef struct ymp_attn_args {
   int64_t kv_rows_ld;      /* entries between consecutive sequences of kv_rows, >= s_kv */
 } ymp_attn_args;
 int ymp_attn_fwd(const ymp_attn_args* a, void* stream);
+/* ymp_attn_fwd with a key count per sequence: sequence s attends to its first min(s_kv, kv_lens[s]) keys, kv_lens a
+ * DEVICE int32 array [n_seq] with every entry >= 1 (one captured decoding step over sequences at different cache
+ * lengths).  With or without kv_rows (every table entry j < s_kv must still name a valid row: the first keys are
+ * requested before the count is read).  Only the streaming decode kernel: s_q == 1, mask none, no dropout, total_rows
+ * or s_kv_dev, head_dim 64 / 80 / 96; anything else is rejected.  O and lse of sequence s are bit-identical to an
+ * ymp_attn_fwd call with s_kv = kv_lens[s]. */
+int ymp_attn_fwd_seq_lens(const ymp_attn_args* a, const int32_t* kv_lens, void* stream);
 
 /* Causal attention with a key prefix per sequence: many texts behind prefixes of different lengths in one launch
  * (the scoring evaluations share each video's [visual queries | title] rows among its texts).  Sequence s has

@@ -1,17 +1,24 @@
-"""Time caption generation: the per-clip beam-search loop against the batched DistributedGPT3_Caption.generate.
+"""Time caption generation: the per-clip beam-search loop against the batched and streaming beam searches.
 
-    python tools/caption_generate.py [--shapes caption_1.3B caption_2.7B] [--rounds 3] [--kernel] [--counts] [--profile]
+    python tools/caption_generate.py [--shapes caption_1.3B caption_2.7B] [--rounds 3] [--workloads full varied]
+                                     [--stop-scale 4] [--kernel] [--counts] [--profile]
 
 Each shape builds DistributedGPT3_Caption with the shipped decoder json, random bf16 weights in eval mode, 128 queries
 and 16 frames, and decodes the caption eval's batch (24 clips at 1.3B, 36 at 2.7B): prompt ids [B, 20] with one
-common prompt length, beam 5, 100 tokens to generate.  Three arms, alternating in one process after a warm-up call of
+common prompt length, beam 5, 100 tokens to generate.  Four arms, alternating in one process after a warm-up call of
 each, every call ending in a device synchronise; the median of --rounds calls is reported:
   per_clip       - the composition before batching: the visual prefix, then one beam search per clip;
-  batched_moving - the batched call with the beams permuted by moving the cached K/V rows (KVCache.reorder);
-  batched        - model.generate(video, text): one beam search over all clips (chunks of 64 // beam clips per decode
-                   step), beams permuted through the cache's row table (KVCache.reindex).
-One JSON line per shape: card name, power limit and max SM clock, ms per call, decode steps, peak allocated memory and
-whether the three arms' sequences and scores are bit-equal.
+  batched_moving - the chunked batched search with the beams permuted by moving the cached K/V rows (KVCache.reorder);
+  batched        - the chunked batched search (chunks of 64 // beam clips per decode step, each running until its
+                   slowest clip is done), beams permuted through the cache's row table (KVCache.reindex);
+  stream         - model.generate(video, text): the streaming search (run_beam_search_stream), a finished clip's
+                   beam slots take the next clip while the others keep decoding.
+Two workloads: `full` (random weights almost never emit the stop token, so every caption runs all 100 tokens: the
+stream arm must do the batched arm's steps) and `varied` (the stop token's row of the tied word embedding scaled by
+--stop-scale, so captions end at varying steps: where the stream arm saves steps).
+One JSON line per shape and workload: card name, power limit and max SM clock, ms per call, single-token decode steps,
+rows stepped that no beam search reads (rows stepped minus beam x the per-clip arm's steps), peak allocated memory,
+the distribution of per-clip decode steps and whether the four arms' sequences and scores are bit-equal.
 --profile prints the device-time share of each kernel family in one batched 12-clip, 40-token call of each batched arm.
 --kernel times ymp_gemm_skinny_wide alone per decoder linear and for the LM head at M in {5, 8, 16, 32, 60, 64} rows (CUDA
 events over many launches, weights rotated through copies larger than L2): microseconds and GB/s next to the H100
@@ -148,17 +155,43 @@ def inputs(vis, name, B):
     return video, text
 
 
-def run(model, vis, name, rounds):
+def chunked_generate(model, video, text, moving=False):
+    """model.generate through the chunked batched beam search (DistributedGPT3._beam_search_batched)."""
+    dec = model.text_decoder
+    dec._beam_search_stream = dec._beam_search_batched
+    try:
+        return moving_generate(model, video, text) if moving else model.generate(video, text)
+    finally:
+        del dec._beam_search_stream
+
+
+def run(model, vis, name, rounds, workload="full", stop_scale=4.0):
     import torch
+    from ymp import engine
     B = SHAPES[name][1]
     video, text = inputs(vis, name, B)
     dec = model.text_decoder
+    emb = dec.dist_model.language_model.embedding.word_embeddings.weight
+    eod_row = emb[dec.config.eod_id].clone()
+    if workload == "varied":
+        with torch.no_grad():
+            emb[dec.config.eod_id] *= stop_scale
     orig = dec.beam_search
     found, steps = [], [0]
+    tok_steps, tok_rows, clip_steps = [0], [0], []
+    ts_run = engine.TokenStep.run
+
+    def counting_run(self, emb_in):   # single-token steps and the rows they step
+        tok_steps[0] += 1
+        tok_rows[0] += self.cache.B
+        return ts_run(self, emb_in)
+    engine.TokenStep.run = counting_run
 
     def beam_search(*a, **k):   # keeps every beam search's results (sequences and scores) for the comparison
+        n0 = tok_steps[0]
         out = orig(*a, **k)
         found.extend(out if isinstance(out, list) else [out])
+        clip_steps.append(tok_steps[0] - n0)
         return out
     dec.beam_search = beam_search
     orig_decode = dec._decode
@@ -168,15 +201,17 @@ def run(model, vis, name, rounds):
         return orig_decode(*a, **k)
     dec._decode = counting_decode
     arms = dict(per_clip=lambda: per_clip_generate(model, video, text),
-                batched_moving=lambda: moving_generate(model, video, text), batched=lambda: model.generate(video, text))
+                batched_moving=lambda: chunked_generate(model, video, text, moving=True),
+                batched=lambda: chunked_generate(model, video, text), stream=lambda: model.generate(video, text))
     ms = {a: [] for a in arms}
     peak = {a: 0 for a in arms}
-    n_steps, outs = {}, {}
+    n_steps, outs, n_tok, n_rows, per_clip_steps = {}, {}, {}, {}, []
     for r in range(rounds + 1):   # round 0 warms up every arm
         for a, fn in arms.items():
             found.clear()
+            clip_steps.clear()
             outs.pop(a, None)
-            steps[0] = 0
+            steps[0] = tok_steps[0] = tok_rows[0] = 0
             # the decoder pools one KV cache + captured step per shape on the model: every arm allocates (and counts in
             # its peak) and captures its own, rather than one arm inheriting the cache of the arm before it
             dec.__dict__.pop("_decode_pool", None)
@@ -189,20 +224,33 @@ def run(model, vis, name, rounds):
             dt = (time.perf_counter() - t0) * 1e3
             outs[a] = [(o.sequences.cpu(), o.scores.cpu()) for o in found]
             n_steps[a] = steps[0]
+            n_tok[a], n_rows[a] = tok_steps[0], tok_rows[0]
+            if a == "per_clip":
+                per_clip_steps = list(clip_steps)
             if r > 0:
                 ms[a].append(dt)
                 peak[a] = max(peak[a], torch.cuda.max_memory_allocated() - base)
     del dec.beam_search, dec._decode
+    engine.TokenStep.run = ts_run
+    with torch.no_grad():
+        emb[dec.config.eod_id] = eod_row
     equal = all(len(outs[a]) == B and all(torch.equal(s0, s1) and torch.equal(c0, c1)
                                           for (s0, c0), (s1, c1) in zip(outs["per_clip"], outs[a])) for a in arms)
-    res = dict(shape=name, clips=B, frames=FRAMES, queries=Q, beam=BEAM, tokens_to_generate=NEW, **card_info())
+    res = dict(shape=name, workload=workload, stop_scale=stop_scale if workload == "varied" else 1.0, clips=B,
+               frames=FRAMES, queries=Q, beam=BEAM, tokens_to_generate=NEW, **card_info())
+    read_rows = BEAM * sum(per_clip_steps)
     for a in arms:
         res[f"{a}_ms"] = round(statistics.median(ms[a]), 1)
         res[f"{a}_ms_all"] = [round(x, 1) for x in ms[a]]
         res[f"{a}_decoder_calls"] = n_steps[a]
+        res[f"{a}_decode_steps"] = n_tok[a]
+        res[f"{a}_unread_rows"] = n_rows[a] - read_rows
         res[f"{a}_peak_gb"] = round(peak[a] / 1e9, 2)
+    res["clip_steps"] = dict(min=min(per_clip_steps), median=statistics.median(per_clip_steps), max=max(per_clip_steps),
+                             all=per_clip_steps)
     res["speedup"] = round(res["per_clip_ms"] / res["batched_ms"], 2)
     res["speedup_over_moving"] = round(res["batched_moving_ms"] / res["batched_ms"], 2)
+    res["stream_over_batched"] = round(res["batched_ms"] / res["stream_ms"], 2)
     res["bit_equal"] = bool(equal)
     res["counts"] = counts(name)
     print(json.dumps(res), flush=True)
@@ -218,7 +266,8 @@ def profile(model, vis, name, clips=12, new=40):
     dec = model.text_decoder
     dec.config.tokens_to_generate = new
     video, text = inputs(vis, name, clips)
-    arms = dict(batched_moving=lambda: moving_generate(model, video, text), batched=lambda: model.generate(video, text))
+    arms = dict(batched_moving=lambda: chunked_generate(model, video, text, moving=True),
+                batched=lambda: chunked_generate(model, video, text))
     info = card_info()
     try:
         for a, fn in arms.items():
@@ -282,6 +331,8 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--shapes", nargs="*", default=list(SHAPES), choices=list(SHAPES))
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--workloads", nargs="*", default=["full", "varied"], choices=["full", "varied"])
+    ap.add_argument("--stop-scale", type=float, default=4.0, help="varied workload: factor on the stop token's embedding row")
     ap.add_argument("--kernel", action="store_true", help="time ymp_gemm_skinny_wide per decoder linear and M")
     ap.add_argument("--counts", action="store_true", help="print the counted bytes only (no GPU)")
     ap.add_argument("--profile", action="store_true", help="device-time shares of one batched 12-clip, 40-token call per "
@@ -302,7 +353,8 @@ def main():
         if args.profile:
             profile(model, vis, s)
         else:
-            run(model, vis, s, args.rounds)
+            for w in args.workloads:
+                run(model, vis, s, args.rounds, w, args.stop_scale)
         del model
         torch.cuda.empty_cache()
 

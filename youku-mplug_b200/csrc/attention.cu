@@ -1104,8 +1104,10 @@ __global__ void __launch_bounds__(128) attn_wg_bwd_dkdv_kernel(const AttnKParams
 // With a row table (kv_rows) each lane first loads its key's table entry, then that row's K and V: a beam search
 // permutes its beams by gathering the small table, and the cache rows are never moved.  The per-key arithmetic and the
 // lane <-> key assignment are the same either way, so O and lse are bit-identical to a call on the gathered cache.
-template <int D>
-__global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
+// SEQ_LENS (ymp_attn_fwd_seq_lens): skv_dev is a per-sequence array, sequence s attends to its first
+// min(s_kv, skv_dev[s]) keys (sequences of one decoding step at different cache lengths).
+template <int D, bool SEQ_LENS>
+__device__ __forceinline__ void attn_decode(const AttnKParams& p) {
   constexpr int CH = D / 8;
   extern __shared__ __align__(16) uint8_t smem_attn[];
   float (*o_part)[D + 1] = reinterpret_cast<float (*)[D + 1]>(smem_attn);   // [128][D + 1]
@@ -1142,7 +1144,8 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
     if (!TWO_PHASE) fetch_v(row);
   }
   int sq, skv;
-  eff_len(p, s, sq, skv);
+  if constexpr (SEQ_LENS) skv = min(p.s_kv, p.skv_dev[s]);
+  else eff_len(p, s, sq, skv);
   float o[D];
 #pragma unroll
   for (int d = 0; d < D; ++d) o[d] = 0.f;
@@ -1206,6 +1209,10 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) {
   }
   if (p.lse && threadIdx.x == 0) p.lse[((long)s * p.n_heads + h) * p.s_q] = (m_all + log2f(l_all)) * 0.6931471805599453f;
 }
+template <int D>
+__global__ void __launch_bounds__(128) attn_decode_kernel(const AttnKParams p) { attn_decode<D, false>(p); }
+template <int D>
+__global__ void __launch_bounds__(128) attn_decode_lens_kernel(const AttnKParams p) { attn_decode<D, true>(p); }
 static int fill_params(const ymp_attn_args* a, AttnKParams& p, const char* who) {
   YMP_CHECK_ARG(a && a->q && a->k && a->v, "%s: null q/k/v", who);
   YMP_CHECK_ARG(a->head_dim == 64 || a->head_dim == 80 || a->head_dim == 88 || a->head_dim == 96 || a->head_dim == 128,
@@ -1263,10 +1270,12 @@ static int launch_attn(dim3 grid, int smem, cudaStream_t st, const AttnKParams& 
   return YMP_OK;
 }
 
+template <bool SEQ_LENS = false>
 static int launch_decode(const AttnKParams& p, int head_dim, cudaStream_t st) {
   return for_head_dim<false>(head_dim, [&](auto hd) {
     constexpr int D = decltype(hd)::D;
-    return launch_attn<attn_decode_kernel<D>>(dim3(p.n_heads, p.n_seq), (128 * (D + 1) + 128 + 4) * 4, st, p);
+    constexpr auto kernel = SEQ_LENS ? attn_decode_lens_kernel<D> : attn_decode_kernel<D>;
+    return launch_attn<kernel>(dim3(p.n_heads, p.n_seq), (128 * (D + 1) + 128 + 4) * 4, st, p);
   });
 }
 static int launch_wg_fwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
@@ -1364,6 +1373,23 @@ extern "C" int ymp_attn_fwd(const ymp_attn_args* a, void* stream) {
   }
   g_attn_path = YMP_ATTN_PATH_MMA_SYNC;
   return launch_fwd(p, a->head_dim, st);
+}
+
+extern "C" int ymp_attn_fwd_seq_lens(const ymp_attn_args* a, const int32_t* kv_lens, void* stream) {
+  using namespace ymp;
+  AttnKParams p = {};
+  int rc = fill_params(a, p, "ymp_attn_fwd_seq_lens");
+  if (rc) return rc;
+  YMP_CHECK_ARG(kv_lens != nullptr, "ymp_attn_fwd_seq_lens: null kv_lens");
+  YMP_CHECK_ARG(a->o && aligned16(a->o), "ymp_attn_fwd_seq_lens: bad o");
+  YMP_CHECK_ARG(a->s_q == 1 && a->mask == YMP_MASK_NONE && !p.has_drop && a->total_rows == 0,
+                "ymp_attn_fwd_seq_lens: needs s_q == 1, mask none, no dropout and no total_rows");
+  YMP_CHECK_ARG(a->head_dim != 88 && a->head_dim != 128, "ymp_attn_fwd_seq_lens: needs head_dim 64, 80 or 96");
+  YMP_CHECK_ARG(!a->s_kv_dev, "ymp_attn_fwd_seq_lens: takes no s_kv_dev (kv_lens replaces it)");
+  YMP_CHECK_ARG(!a->kv_rows || a->kv_rows_ld >= a->s_kv, "ymp_attn_fwd_seq_lens: kv_rows_ld must be >= s_kv");
+  p.skv_dev = kv_lens;
+  g_attn_path = YMP_ATTN_PATH_DECODE;
+  return launch_decode<true>(p, a->head_dim, (cudaStream_t)stream);
 }
 
 // The checks and parameters that ymp_attn_fwd_prefix_table and ymp_attn_fwd_prefix_kv share.

@@ -20,7 +20,8 @@
 //   * partial sums meet in shared memory and are added in slice order; lane (g, t) of the slice-0 warp owns (row g (+8,
 //     +16, ...), columns n0+2t, n0+2t+1) and applies
 //       v = acc + bias[n] ; v = gelu(v) (optional) ; v += residual[m, n] (bf16 or fp32) ; store bf16 or fp32
-//     (+ an optional second bf16 copy at a device-side row offset: the KV-cache row of the new token).
+//     (+ an optional second bf16 copy at a device-side row offset: the KV-cache row of the new token; ROW_OFF: one
+//     offset per result row, y2_off[m], for sequences at different cache lengths).
 // Algorithmic bytes per call: N*K*2 (weights) + M*(K + N)*2..4.  The wide kernel re-reads the activations once per
 // 8-column tile (from L2): M*K*2 * N/8 bytes of L2 traffic, 8x the weight bytes at M = 64.
 #include "common.h"
@@ -41,13 +42,14 @@ struct SkinnyParams {
   const void* residual;
   void* y;
   __nv_bfloat16* y2;
-  const long long* y2_off;
+  const long long* y2_off;   // device scalar, or [M] per-row offsets (ROW_OFF)
   long long ldy2, y2_stride;
   int M, N, K, ldx, ldw, ldr, ldy;
   int act, res_f32, out_f32, ksplit;
 };
 
 // Epilogue of result row m, columns n, n + 1 (the accumulators of one lane): identical for both kernels
+template <bool ROW_OFF>
 __device__ __forceinline__ void skinny_store(const SkinnyParams& p, int m, int n_base, float acc0, float acc1) {
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
@@ -62,7 +64,7 @@ __device__ __forceinline__ void skinny_store(const SkinnyParams& p, int m, int n
                      : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[(size_t)m * p.ldr + n]);
     if (p.out_f32) reinterpret_cast<float*>(p.y)[(size_t)m * p.ldy + n] = v;
     else reinterpret_cast<__nv_bfloat16*>(p.y)[(size_t)m * p.ldy + n] = __float2bfloat16(v);
-    if (p.y2) p.y2[(long long)m * p.ldy2 + *p.y2_off * p.y2_stride + n] = __float2bfloat16(v);
+    if (p.y2) p.y2[(long long)m * p.ldy2 + (ROW_OFF ? p.y2_off[m] : *p.y2_off) * p.y2_stride + n] = __float2bfloat16(v);
   }
 }
 
@@ -74,7 +76,8 @@ __device__ __forceinline__ void mma16816_bf16(float (&c)[4], uint32_t a0, uint32
       : "r"(a0), "r"(0u), "r"(a2), "r"(b0), "r"(b1));
 }
 
-__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_kernel(const __grid_constant__ SkinnyParams p) {
+template <bool ROW_OFF>
+__device__ __forceinline__ void gemm_skinny(const SkinnyParams& p) {
   __shared__ float part[SK_WARPS][64];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, t = lane & 3;
@@ -129,14 +132,21 @@ __global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_kernel(const __g
     if (kpart == 0)
       for (int j = 1; j < ks; ++j) { acc[0] += part[warp + j][2 * lane]; acc[1] += part[warp + j][2 * lane + 1]; }
   }
-  if (live && kpart == 0 && g < p.M) skinny_store(p, g, n0 + 2 * t, acc[0], acc[1]);
+  if (live && kpart == 0 && g < p.M) skinny_store<ROW_OFF>(p, g, n0 + 2 * t, acc[0], acc[1]);
+}
+__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_kernel(const __grid_constant__ SkinnyParams p) {
+  gemm_skinny<false>(p);
+}
+__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_rows_kernel(const __grid_constant__ SkinnyParams p) {
+  gemm_skinny<true>(p);
 }
 
 // 9 <= M <= 64: gemm_skinny_kernel's grid, warp roles, K slices, weight stream and k-block loop (the same zero-padded
 // tail), with one accumulator set per group of 16 rows.  Group j's lane (g, t) holds rows 16j + g (acc[j][0..1])
 // and 16j + 8 + g (acc[j][2..3]).  The activation chunks of the k-block being consumed are loaded from global memory
 // (L2-resident: every CTA reads them) next to the MMAs; only the weights are double-buffered in registers.
-__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(const __grid_constant__ SkinnyParams p) {
+template <bool ROW_OFF>
+__device__ __forceinline__ void gemm_skinny_wide(const SkinnyParams& p) {
   __shared__ float part[SK_WARPS][32 * 4 * SK_WIDE_GROUPS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, t = lane & 3;
@@ -201,18 +211,25 @@ __global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(cons
   if (live && kpart == 0) {
 #pragma unroll
     for (int j = 0; j < SK_WIDE_GROUPS; ++j) {
-      if (16 * j + g < p.M) skinny_store(p, 16 * j + g, n0 + 2 * t, acc[j][0], acc[j][1]);
-      if (16 * j + 8 + g < p.M) skinny_store(p, 16 * j + 8 + g, n0 + 2 * t, acc[j][2], acc[j][3]);
+      if (16 * j + g < p.M) skinny_store<ROW_OFF>(p, 16 * j + g, n0 + 2 * t, acc[j][0], acc[j][1]);
+      if (16 * j + 8 + g < p.M) skinny_store<ROW_OFF>(p, 16 * j + 8 + g, n0 + 2 * t, acc[j][2], acc[j][3]);
     }
   }
+}
+__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_kernel(const __grid_constant__ SkinnyParams p) {
+  gemm_skinny_wide<false>(p);
+}
+__global__ void __launch_bounds__(SK_WARPS * 32, 1) gemm_skinny_wide_rows_kernel(const __grid_constant__ SkinnyParams p) {
+  gemm_skinny_wide<true>(p);
 }
 
 }  // namespace ymp
 
 using namespace ymp;
 
-// ymp_gemm_skinny (max_m = 8) and ymp_gemm_skinny_wide (max_m = 64): the same arguments, checks and M <= 8 launch
-static int gemm_skinny_call(const ymp_gemm_skinny_args* a, void* stream, int max_m) {
+// ymp_gemm_skinny (max_m = 8) and ymp_gemm_skinny_wide (max_m = 64): the same arguments, checks and M <= 8 launch.
+// row_off (the *_rows entry points): per-row offsets of the second copy in place of a->y2_off_dev.
+static int gemm_skinny_call(const ymp_gemm_skinny_args* a, void* stream, int max_m, const int64_t* row_off = nullptr) {
   YMP_CHECK_ARG(a && a->x && a->w && a->y, "ymp_gemm_skinny: null pointer");
   YMP_CHECK_ARG(a->M >= 1 && a->M <= max_m && a->N > 0 && a->K > 0 && a->K % 8 == 0, "ymp_gemm_skinny%s: needs 1 <= M <= %d, K %% 8 == 0 (M=%d K=%d)",
                 max_m > SK_MAXM ? "_wide" : "", max_m, a->M, a->K);
@@ -221,8 +238,13 @@ static int gemm_skinny_call(const ymp_gemm_skinny_args* a, void* stream, int max
   SkinnyParams p;
   p.x = (const __nv_bfloat16*)a->x; p.w = (const __nv_bfloat16*)a->w; p.bias = (const __nv_bfloat16*)a->bias;
   p.residual = a->residual; p.y = a->y;
-  YMP_CHECK_ARG(!a->y2 || (a->y2_off_dev && a->out_dtype == YMP_DT_BF16), "ymp_gemm_skinny: y2 needs y2_off_dev and a bf16 result");
-  p.y2 = (__nv_bfloat16*)a->y2; p.y2_off = (const long long*)a->y2_off_dev; p.ldy2 = a->ldy2; p.y2_stride = a->y2_off_stride;
+  if (row_off) {
+    YMP_CHECK_ARG(a->y2 && !a->y2_off_dev && a->out_dtype == YMP_DT_BF16,
+                  "ymp_gemm_skinny_rows: needs y2, a bf16 result and no y2_off_dev (y2_row_off replaces it)");
+  } else {
+    YMP_CHECK_ARG(!a->y2 || (a->y2_off_dev && a->out_dtype == YMP_DT_BF16), "ymp_gemm_skinny: y2 needs y2_off_dev and a bf16 result");
+  }
+  p.y2 = (__nv_bfloat16*)a->y2; p.y2_off = (const long long*)(row_off ? row_off : a->y2_off_dev); p.ldy2 = a->ldy2; p.y2_stride = a->y2_off_stride;
   p.M = a->M; p.N = a->N; p.K = a->K; p.ldx = a->ldx; p.ldw = a->ldw; p.ldr = a->ldr; p.ldy = a->ldy;
   p.act = a->act; p.res_f32 = a->residual_dtype == YMP_DT_F32; p.out_f32 = a->out_dtype == YMP_DT_F32;
   // K slices per CTA (the warps of a CTA that share one 8-column tile): as many as leave >= 4 k-blocks of 32 per slice
@@ -233,8 +255,8 @@ static int gemm_skinny_call(const ymp_gemm_skinny_args* a, void* stream, int max
   const int tiles = (a->N + SK_TILE_N - 1) / SK_TILE_N, tiles_per_cta = SK_WARPS / ks;
   const int blocks = (tiles + tiles_per_cta - 1) / tiles_per_cta;
   cudaStream_t st = (cudaStream_t)stream;
-  if (a->M > SK_MAXM) gemm_skinny_wide_kernel<<<blocks, SK_WARPS * 32, 0, st>>>(p);
-  else gemm_skinny_kernel<<<blocks, SK_WARPS * 32, 0, st>>>(p);
+  if (a->M > SK_MAXM) (row_off ? gemm_skinny_wide_rows_kernel : gemm_skinny_wide_kernel)<<<blocks, SK_WARPS * 32, 0, st>>>(p);
+  else (row_off ? gemm_skinny_rows_kernel : gemm_skinny_kernel)<<<blocks, SK_WARPS * 32, 0, st>>>(p);
   YMP_LAUNCH_CHECK();
   return YMP_OK;
 }
@@ -243,4 +265,14 @@ extern "C" int ymp_gemm_skinny(const ymp_gemm_skinny_args* a, void* stream) { re
 
 extern "C" int ymp_gemm_skinny_wide(const ymp_gemm_skinny_args* a, void* stream) {
   return gemm_skinny_call(a, stream, SK_WIDE_MAXM);
+}
+
+extern "C" int ymp_gemm_skinny_rows(const ymp_gemm_skinny_args* a, const int64_t* y2_row_off, void* stream) {
+  YMP_CHECK_ARG(y2_row_off, "ymp_gemm_skinny_rows: null y2_row_off");
+  return gemm_skinny_call(a, stream, SK_MAXM, y2_row_off);
+}
+
+extern "C" int ymp_gemm_skinny_wide_rows(const ymp_gemm_skinny_args* a, const int64_t* y2_row_off, void* stream) {
+  YMP_CHECK_ARG(y2_row_off, "ymp_gemm_skinny_wide_rows: null y2_row_off");
+  return gemm_skinny_call(a, stream, SK_WIDE_MAXM, y2_row_off);
 }

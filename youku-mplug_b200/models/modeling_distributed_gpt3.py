@@ -535,6 +535,158 @@ def run_beam_search_batched(step, reorder, tokens, prompt_length, n_query, *, be
     return out
 
 
+def _prefill_runs(groups, plens):
+    """Refills of one step that can share a prefill launch: groups whose clips have one prompt length and whose slots
+    are equally spaced.  groups ascending; returns [(prompt_length, first_group, group_stride, [groups])]."""
+    by_len = {}
+    for g, p in zip(groups, plens):
+        by_len.setdefault(int(p), []).append(g)
+    runs = []
+    for p, gs in by_len.items():
+        run = [gs[0]]
+        for g in gs[1:]:
+            if len(run) == 1 or g - run[-1] == run[1] - run[0]:
+                run.append(g)
+            else:
+                runs.append((p, run))
+                run = [g]
+        runs.append((p, run))
+    return [(p, r[0], r[1] - r[0] if len(r) > 1 else 1, r) for p, r in runs]
+
+
+def run_beam_search_stream(step, prefill, reorder, tokens, prompt_lengths, n_query, *, beam_size, num_return_gen, stop_token,
+                           tokens_to_generate, max_position_embeddings, groups):
+    """run_beam_search for N clips (tokens [N, L], one prompt length per clip) over `groups` slot groups of beam_size
+    rows each (group g owns rows g*beam .. g*beam + beam - 1), filled with clips in input order.  Each clip keeps its
+    own context length, ranking, BeamHypotheses and stopping rule, so its result equals run_beam_search on that clip
+    alone.  When a group's clip is done (its pool is done or its own last position is reached) the next waiting clip is
+    prefilled into that group while the other groups keep decoding; a group with no successor is frozen.
+      step(new_tokens [groups*beam, 1], live [groups] bools) -> logits [groups*beam, V] of one single-token step of the
+        live groups (a frozen group's rows are not read and must not advance);
+      prefill(first_group, group_stride, clips, n) -> logits [len(clips), V]: clip clips[i]'s [prefix | tokens[:n]] into
+        group first_group + i * group_stride (refills of one step with one prompt length and equally spaced groups
+        share a call);
+      reorder(idx [groups*beam]) permutes the decode state's rows (within groups).
+    A decoding step ranks every live group's candidates in one device sort and copies them to the host in one
+    transfer; the step that starts clips ranks their first candidates in one more sort and transfer.  Returns a list of
+    N AttrDict(sequences, scores) in input order."""
+    N, dev = tokens.size(0), tokens.device
+    plens = [int(p) for p in prompt_lengths]
+    assert len(plens) == N
+    tokens = torch.cat((tokens, torch.full((N, tokens_to_generate), stop_token, dtype=torch.long, device=dev)), dim=-1)
+    final_len = min(tokens.size(1), max_position_embeddings)
+    if max(plens) >= final_len:
+        raise ValueError('context length + tokens_to_generate too large')
+    G, beam, top = groups, beam_size, 2 * beam_size
+    clip_of = [None] * G        # clip decoding in group g (None: free / frozen)
+    ctx = [0] * G               # the group's next context position (run_beam_search's ctx)
+    pools = [None] * G
+    out = [None] * N
+    rows = torch.full((G * beam, tokens.size(1)), stop_token, dtype=torch.long, device=dev)
+    scores = torch.zeros(G * beam, 1, dtype=torch.float32, device=dev)
+    waiting = list(range(N))
+
+    def finish(g, add):
+        c, pool, base = clip_of[g], pools[g], g * beam
+        if add:   # the clip reached its last position without being done: its live beams join the pool
+            for b in range(beam):
+                pool.add(rows[base + b].clone(), scores[base + b], ctx[g] + 1 - plens[c])
+        best = sorted(pool.beams, key=lambda x: float(x[0]), reverse=True)[:min(num_return_gen, len(pool.beams))]
+        out[c] = AttrDict(sequences=torch.stack([h for _, h, _ in best], dim=0),
+                          scores=torch.stack([torch.as_tensor(sc, device=dev).reshape(-1)[0] for sc, _, _ in best], dim=0))
+        clip_of[g] = None
+
+    def rank(gs, cand, first):
+        """Rank groups gs from cand [len(gs), width] (one sort, one transfer), apply the survivors to rows / scores,
+        advance or finish each group.  Returns keep (row -> source row) for the reorder."""
+        ranked_scores, ranked = torch.sort(cand, dim=-1, descending=True)
+        ranked, ranked_scores = ranked[:, :top], ranked_scores[:, :top]
+        host = torch.cat((ranked.double(), ranked_scores.double()), dim=1).cpu()   # indices < 2**53 and fp32 are exact
+        vocab = cand.size(1) if first else cand.size(1) // beam
+        idx = host[:, :top].long()
+        beam_of, word_of = torch.div(idx, vocab, rounding_mode='floor').tolist(), (idx % vocab).tolist()
+        best_score = host[:, top:].max(dim=1).values.tolist()
+        keep, at, words, picked, ended = [], [], [], [], []
+        for i, g in enumerate(gs):
+            c, base = clip_of[g], g * beam
+            survivors = []
+            for r, (word, b) in enumerate(zip(word_of[i], beam_of[i])):
+                if word == stop_token:
+                    if r >= beam:  # a finished hypothesis outside the top beam_size candidates is dropped
+                        continue
+                    pools[g].add(rows[base + b].clone(), ranked_scores[i, r], ctx[g] + 1 - plens[c])
+                else:
+                    survivors.append((word, r, b))
+                if len(survivors) == beam:
+                    break
+            if pools[g].is_done(best_score[i], ctx[g] + 1 - plens[c]):
+                ended.append((g, False))
+                continue
+            keep += [base + b for _, _, b in survivors]
+            at += [(base + j, ctx[g]) for j in range(beam)]
+            words += [w for w, _, _ in survivors]
+            picked += [i * top + r for _, r, _ in survivors]
+            if ctx[g] + 1 == final_len:
+                ended.append((g, True))
+        perm = torch.arange(G * beam, device=dev)
+        if keep:
+            dst = torch.tensor([r for r, _ in at], dtype=torch.long, device=dev)
+            perm[dst] = torch.tensor(keep, dtype=torch.long, device=dev)
+            rows[dst] = rows[perm[dst]]
+            rows[dst, torch.tensor([p for _, p in at], dtype=torch.long, device=dev)] = torch.tensor(words, dtype=torch.long, device=dev)
+            scores[dst] = ranked_scores.reshape(-1)[torch.tensor(picked, dtype=torch.long, device=dev)].reshape(-1, 1).float()
+        for g, add in ended:
+            finish(g, add)
+        for g in gs:
+            ctx[g] += 1
+        return perm
+
+    def refill(free):
+        """Start waiting clips in the free groups (ascending) and rank their first candidates; repeat for clips that
+        end at once."""
+        while free and waiting:
+            gs, cs = free[:len(waiting)], waiting[:len(free)]
+            del waiting[:len(gs)]
+            for g, c in zip(gs, cs):
+                clip_of[g], ctx[g], pools[g] = c, plens[c], BeamHypotheses(beam)
+                rows[g * beam:(g + 1) * beam] = tokens[c]
+                scores[g * beam:(g + 1) * beam] = 0
+            first = [None] * len(gs)
+            for p, g0, gstride, run in _prefill_runs(gs, [plens[c] for c in cs]):
+                lg = prefill(g0, gstride, [clip_of[g] for g in run], p)
+                for j, g in enumerate(run):
+                    first[gs.index(g)] = lg[j:j + 1]
+            lg = torch.cat(first)
+            # identical beams: only the first beam of every clip is ranked
+            rank(gs, torch.log_softmax(lg.float(), dim=-1) + scores.view(G, beam)[gs, :1], True)
+            free = [g for g in gs if clip_of[g] is None]
+
+    refill(list(range(G)))
+    while any(c is not None for c in clip_of):
+        live = [c is not None for c in clip_of]
+        new = rows.gather(1, torch.tensor([max(ctx[g] - 1, 0) for g in range(G) for _ in range(beam)],
+                                          dtype=torch.long, device=dev).view(-1, 1))
+        logits = step(new, live)
+        gs = [g for g in range(G) if live[g]]
+        cand = (torch.log_softmax(logits.float(), dim=-1) + scores).view(G, -1)
+        perm = rank(gs, cand[gs] if len(gs) < G else cand, False)
+        reorder(perm)
+        refill([g for g in gs if clip_of[g] is None])
+    return out
+
+
+def streams_beam_search(prompt_lengths, beam_size, head_dim, device):
+    """Does DistributedGPT3.beam_search run these clips as one streaming search (run_beam_search_stream)?  Only where
+    it gains and its per-sequence decoding step exists: the clips need more than one chunk of the batched search (more
+    than 64 // beam_size clips, or several prompt lengths; one chunk has nothing to refill, and its step does less host
+    work), the decoder's head_dim has the per-sequence decode attention (64 / 80 / 96) and the tokens are on a CUDA
+    device, where those kernels run.  Otherwise the batched search over chunks, as before the streaming search."""
+    from ymp import ops
+    if torch.device(device).type != "cuda" or head_dim not in (64, 80, 96):
+        return False
+    return len(beam_search_chunks(prompt_lengths, beam_size, ops.SKINNY_WIDE_MAX_ROWS)) > 1
+
+
 def beam_search_chunks(prompt_lengths, beam_size, max_rows):
     """How a batched beam search splits its clips: clips grouped by prompt length (in order of first appearance),
     each group cut into chunks of at most max_rows // beam_size clips.  Returns [(prompt_length, [clip indices])]."""
@@ -771,13 +923,19 @@ class DistributedGPT3(nn.Module):
     def beam_search(self, tokens, query_embeds=None, beam_size=5, num_return_gen=1, stop_token=None, **kwargs):
         """Beam search (:1743-1875).  One sample (tokens [1, L]): Dict(sequences [n, len], scores [n]).
         B > 1 samples (prompt_length an int or a [B] tensor): a list of B such Dicts, each equal to the call for that
-        sample alone, computed by batched beam searches over chunks of samples that share a prompt length."""
+        sample alone.  Samples that need more than one chunk of the batched search run one streaming beam search
+        (run_beam_search_stream: a finished sample's beam slots take the next sample) where streams_beam_search says so;
+        otherwise batched beam searches over chunks of samples that share a prompt length."""
         cfg = self.config
         prompt_length = kwargs.pop('prompt_length', tokens.size(1))
         if stop_token is None:
             stop_token = cfg.eod_id
         if tokens.size(0) > 1:
-            return self._beam_search_batched(tokens, query_embeds, beam_size, num_return_gen, stop_token, prompt_length)
+            lengths = torch.as_tensor(prompt_length).reshape(-1).tolist()
+            lengths = lengths * tokens.size(0) if len(lengths) == 1 else lengths
+            stream = streams_beam_search(lengths, beam_size, cfg.hidden_size // cfg.num_attention_heads, tokens.device)
+            search = self._beam_search_stream if stream else self._beam_search_batched
+            return search(tokens, query_embeds, beam_size, num_return_gen, stop_token, prompt_length)
         prompt_length = int(prompt_length)
         nq = 0 if query_embeds is None else query_embeds.size(1)
         final_len = min(tokens.size(1) + cfg.tokens_to_generate, cfg.max_position_embeddings)
@@ -816,6 +974,63 @@ class DistributedGPT3(nn.Module):
             for i, o in zip(clips, outs):
                 res[i] = o
         return res
+
+    def _beam_search_stream(self, tokens, query_embeds, beam_size, num_return_gen, stop_token, prompt_length):
+        """run_beam_search_stream over one KV cache of G = 64 // beam_size groups in per-row mode: the single-token steps
+        replay one captured per-row TokenStep, a finished clip's group is refilled by a group prefill into its first
+        slot."""
+        from ymp import engine, ops
+        cfg = self.config
+        B = tokens.size(0)
+        lengths = torch.as_tensor(prompt_length).reshape(-1).tolist()
+        if len(lengths) == 1:
+            lengths = lengths * B
+        assert len(lengths) == B
+        G = min(ops.SKINNY_WIDE_MAX_ROWS // beam_size, B)
+        if G < 1:
+            raise ValueError(f"beam_size {beam_size} exceeds the {ops.SKINNY_WIDE_MAX_ROWS} rows of one decoding step")
+        nq = 0 if query_embeds is None else query_embeds.size(1)
+        final_len = min(tokens.size(1) + cfg.tokens_to_generate, cfg.max_position_embeddings)
+        rows, ML, dev = G * beam_size, final_len + nq, tokens.device
+        self.inference_params = None
+        key = (rows, ML, str(dev), "per_row")
+        pool = self.__dict__.setdefault("_decode_pool", {})
+        if key not in pool:
+            pool.clear()   # one resident cache, as in _decode
+            pool[key] = engine.KVCache(cfg.engine_cfg(), rows, ML, dev)
+        cache = pool[key]
+        cache.reset_rows()
+        keys, params = self._param_list()
+        W = {k: YF.as_bf16(p) for k, p in zip(keys, params)}
+        sig = (params[0].data_ptr(), params[-1].data_ptr(), sum(p._version for p in params))
+        emb = self.dist_model.language_model.embedding.word_embeddings
+        wemb, pos = W[engine.GPT + "embedding.word_embeddings.weight"], W[engine.GPT + "embedding.position_embeddings.weight"]
+        ts = cache.token
+        if ts is None or ts.sig != sig or not ts.per_row:
+            static = all(p.dtype == torch.bfloat16 or not p.requires_grad for p in params)
+            ts = cache.token = engine.TokenStep(cache, W, emb.weight.dtype, sig, static, per_row=True)
+        elif not ts.static:
+            ts.W = W
+
+        def step(new_tokens, live):
+            cache.set_live([x for x in live for _ in range(beam_size)])
+            _, logits = ts.run(emb(new_tokens).reshape(rows, -1))
+            return logits
+
+        def prefill(group0, group_stride, clips, n):
+            sel = torch.tensor(clips, dtype=torch.long, device=dev)
+            x = emb(tokens[sel, :n])
+            if query_embeds is not None:
+                x = torch.cat([query_embeds[sel].to(x.dtype), x], dim=1)
+            m = n + nq
+            x = (x.float() + pos[:m][None].float()).reshape(len(clips) * m, -1).contiguous()
+            hid = cache.prefill_groups(W, x, m, group0, group_stride, beam_size)
+            return ops.gemm(hid, wemb).float()
+
+        return run_beam_search_stream(step, prefill, cache.reindex_rows, tokens, lengths, nq, beam_size=beam_size,
+                                      num_return_gen=num_return_gen, stop_token=stop_token,
+                                      tokens_to_generate=cfg.tokens_to_generate,
+                                      max_position_embeddings=cfg.max_position_embeddings, groups=G)
 
     @torch.no_grad()
     def generate(self, tokens, do_sample=True, termination_id=None, *args, **kwargs):

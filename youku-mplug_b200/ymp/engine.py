@@ -834,7 +834,12 @@ class KVCache:
     its own slot b * max_len + p, and never changes; so a beam search permutes its beams with `reindex`, which gathers
     the table's cached columns and moves no K/V byte.  Columns >= len are never gathered and stay the identity
     b * max_len + p, so every entry always names a valid row (the decode kernel requests keys before it reads the
-    device-side count)."""
+    device-side count).
+
+    Per-sequence lengths (`lens` int64 [B]: position / cache row of each sequence's next token; `lens1` int32 [B]: keys
+    it attends to; host mirror `lens_host`) serve a decoding step whose sequences sit at different positions: a beam
+    search that starts a new clip in the beam slots of a finished one (prefill_groups, reindex_rows, set_live).  There
+    the table invariant holds per row: column p of row b is the identity b * max_len + p for every p >= lens[b]."""
 
     def __init__(self, gcfg, batch, max_len, device):
         g = GptDims(gcfg)
@@ -847,6 +852,12 @@ class KVCache:
         self.rows = self._identity.clone()
         self._indexed = False   # rows differs from the identity
         self.token = None   # TokenStep of the single-token steps (built by the caller that owns the weights)
+        self.lens = torch.zeros(batch, device=device, dtype=torch.int64)
+        self.lens1 = torch.ones(batch, device=device, dtype=torch.int32)
+        self.lens_host = [0] * batch
+        self.adv = torch.ones(batch, device=device, dtype=torch.int64)   # 1: the per-row step advances the row, 0: frozen
+        self.adv_host = [1] * batch
+        self._cols = torch.arange(max_len, device=device, dtype=torch.int64).view(1, max_len)
 
     def reset(self):
         """Forget the cached positions (the rows are overwritten by the next prefill; stale rows past `len` are never read)."""
@@ -892,6 +903,55 @@ class KVCache:
             v[:, :, :self.len].copy_(src.view(self.g.layers, self.B, self.len, -1))
         self._reset_rows()
 
+    def reset_rows(self):
+        """Per-row mode: forget every sequence's cached positions; every row is live."""
+        self.reset()
+        self.lens.zero_()
+        self.lens1.fill_(1)
+        self.lens_host = [0] * self.B
+        self.set_live([True] * self.B)
+
+    def set_live(self, live):
+        """Per-row mode: which rows the next single-token steps advance.  A frozen row keeps its length, so its step
+        writes its K/V row again at the same position of its own slot and never moves past max_len."""
+        live = [1 if x else 0 for x in live]
+        assert len(live) == self.B
+        if live != self.adv_host:
+            self.adv_host = live
+            self.adv.copy_(torch.tensor(live, dtype=torch.int64), non_blocking=False)
+
+    def reindex_rows(self, idx):
+        """Per-row mode reindex: row b takes old row idx[b]'s table columns p < lens[b] (idx[b] holds at least as many
+        positions: a beam search permutes rows within a group of equal lengths) and keeps the identity past them, so no
+        row ever reads another row's identity entries."""
+        assert idx.numel() == self.B
+        self.rows.copy_(torch.where(self._cols < self.lens.view(-1, 1), self.rows.index_select(0, idx), self._identity))
+        self._indexed = True
+
+    def prefill_groups(self, W, x, n, group0, group_stride, stride):
+        """Per-row mode: run k sequences of n positions (x [k*n, H] fp32, rows i*n + j at positions 0 .. n-1) into
+        the first slots of groups group0 + i * group_stride (group g = rows g*stride .. g*stride + stride - 1) while the
+        other groups keep their cached positions.  Each group's other rows read the new positions from its first slot
+        through the row table (reset to the identity first); the group's lengths become n.  Same kernels as gpt_decode's
+        first call, so the rows equal a fresh prefill of the sequence.  Returns the final hidden state of each
+        sequence's last position [k, H]."""
+        k = x.shape[0] // n
+        first = group0 * stride
+        assert x.shape[0] == k * n and 0 < n <= self.max_len and first + ((k - 1) * group_stride + 1) * stride <= self.B
+        x = _decode_layers(W, x, self, n, 0, k, self.max_len * stride * group_stride, first * self.max_len)
+        for i in range(k):
+            g0 = first + i * group_stride * stride
+            rows = self.rows[g0:g0 + stride]
+            rows.copy_(self._identity[g0:g0 + stride])
+            rows[:, :n] = self._identity[g0, :n]
+            self.lens_host[g0:g0 + stride] = [n] * stride
+        sel = torch.tensor([first + i * group_stride * stride + j for i in range(k) for j in range(stride)],
+                           dtype=torch.long)
+        self.lens.index_fill_(0, sel.to(self.lens.device), n)
+        self.lens1.index_fill_(0, sel.to(self.lens.device), n + 1)
+        self._indexed = True
+        return _last_hidden(W, x, self.g, k, n)
+
     def reorder(self, idx):
         """Row b of the cache becomes old row idx[b] (beam search, swap_key_value_dict :1460-1473), in place and for
         the cached positions only: two launches for all layers.  A table left by reindex / share_prefill is first
@@ -909,12 +969,15 @@ class TokenStep:
     CUDA graph: every linear is a skinny GEMM (one pass over its weights, csrc/gemv.cu), the new K/V row goes into the cache
     at the device-side position `len_idx`, attention reads `len1` keys (ymp_attn_args.s_kv_dev), and the graph ends by
     advancing both counters - so one captured graph serves every position of every generate() call that reuses this
-    cache.  ~8 kernels per layer; the latency floor is the weight stream (2.6 GB at 1.3B)."""
+    cache.  ~8 kernels per layer; the latency floor is the weight stream (2.6 GB at 1.3B).
+    per_row: every sequence at its own position (the cache's `lens` / `lens1`): position embeddings gathered per row,
+    the new K/V rows written at per-row offsets (ymp_gemm_skinny_rows), attention over per-sequence key counts
+    (ymp_attn_fwd_seq_lens), and the graph advances the rows the cache marks live (`adv`)."""
 
-    def __init__(self, cache, W, emb_dtype, sig=None, static=True):
+    def __init__(self, cache, W, emb_dtype, sig=None, static=True, per_row=False):
         """sig: anything that changes when the weight tensors behind W move; static: W may be captured (raw pointers)."""
         g, dev = cache.g, cache.store.device
-        self.cache, self.W, self.sig, self.static = cache, W, sig, static
+        self.cache, self.W, self.sig, self.static, self.per_row = cache, W, sig, static, per_row
         self.emb_in = torch.zeros((cache.B, g.H), device=dev, dtype=emb_dtype)
         self.stage = torch.zeros((cache.B, 3 * g.H), device=dev, dtype=bf16)   # the new token's [q|k|v] row per sequence
         self.graph = None
@@ -927,7 +990,10 @@ class TokenStep:
         g, B, ML = c.g, c.B, c.max_len
         H, hd = g.H, g.hd
         pos = W[GPT + "embedding.position_embeddings.weight"]
-        x = self.emb_in.float() + pos.index_select(0, c.len_idx).float()
+        x = self.emb_in.float() + pos.index_select(0, c.lens if self.per_row else c.len_idx).float()
+        # K/V row of the new token: at the shared device-side length, or at each row's own length
+        kv_out = dict(out2_row_off=c.lens) if self.per_row else dict(out2_off=c.len_idx)
+        kv_len = dict(kv_lens=c.lens1) if self.per_row else dict(s_kv_dev=c.len1)
         mkv = ops.dense_map(ML)
         # more rows than ymp_gemm_skinny takes (a batched beam search): the wide entry point, same per-row results
         skinny = ops.gemm_skinny if B <= ops.SKINNY_MAX_ROWS else ops.gemm_skinny_wide
@@ -945,27 +1011,33 @@ class TokenStep:
             buf = c.qkv[i]
             # [q|k|v] of the new token: into the staging rows (q for this step) and into cache row b*ML + len (k, v)
             skinny(ln1, W[pre + "self_attention.query_key_value.weight"], bias=W[pre + "self_attention.query_key_value.bias"],
-                   out=st, out2=buf, out2_row_stride=ML, out2_off=c.len_idx)
+                   out=st, out2=buf, out2_row_stride=ML, **kv_out)
             att = torch.empty((B, H), device=x.device, dtype=bf16)
             q = TView(st, 0, 3 * hd, ops.dense_map(1))
             k, v = TView(buf, hd, 3 * hd, mkv), TView(buf, 2 * hd, 3 * hd, mkv)
             ops.attn_fwd(q, k, v, TView(att, 0, hd, ops.dense_map(1)), n_seq=B, n_heads=g.heads, head_dim=hd, s_q=1, s_kv=ML,
-                         causal=False, scale=g.scale, s_kv_dev=c.len1, kv_rows=c.rows)
+                         causal=False, scale=g.scale, kv_rows=c.rows, **kv_len)
             x1, ln2 = gemm_ln(att, pre + "self_attention.dense", x, pre + "post_attention_layernorm")
             h = skinny(ln2, W[pre + "mlp.dense_h_to_4h.weight"], bias=W[pre + "mlp.dense_h_to_4h.bias"], act=ACT_GELU_TANH)
             nxt = f"{GPT}encoder.layers.{i + 1}.input_layernorm" if i + 1 < g.layers else GPT + "encoder.final_layernorm"
             x, ln1 = gemm_ln(h, pre + "mlp.dense_4h_to_h", x1, nxt)
         hid = ln1
         logits = skinny(hid, W[GPT + "embedding.word_embeddings.weight"], out_dtype=torch.float32)
-        c.len_idx += 1
-        c.len1 += 1
+        if self.per_row:
+            c.lens += c.adv
+            c.lens1.copy_(c.lens)
+            c.lens1 += 1
+        else:
+            c.len_idx += 1
+            c.len1 += 1
         return hid, logits
 
     def run(self, emb):
         c = self.cache
         use_graph = self.static and decode_graph_enabled()
-        if c.len + 1 > c.max_len:
-            raise ValueError(f"KV cache overflow: {c.len} + 1 > {c.max_len}")
+        n = max(l for l, a in zip(c.lens_host, c.adv_host) if a) if self.per_row and any(c.adv_host) else c.len
+        if n + 1 > c.max_len:
+            raise ValueError(f"KV cache overflow: {n} + 1 > {c.max_len}")
         self.emb_in.copy_(emb)
         if not use_graph or not self.warm:
             # the first step runs eagerly: it is also the warm-up the capture needs (lazy kernel attributes)
@@ -980,7 +1052,10 @@ class TokenStep:
                 self.graph = graph
             self.graph.replay()
             hid, logits = self.out[0].clone(), self.out[1].clone()
-        c.len += 1
+        if self.per_row:
+            c.lens_host = [l + a for l, a in zip(c.lens_host, c.adv_host)]
+        else:
+            c.len += 1
         return hid, logits
 
 
@@ -997,8 +1072,7 @@ def gpt_decode(W, x, cache, n, seq_stride=1):
     seq_stride > 1 (first call only): x holds B = cache.B / seq_stride sequences and sequence b goes into cache slot
     b * seq_stride (a batched beam search fills each clip's first beam slot); the row table then points the other
     slots of the group at it, so no cached row is copied.  The single-token steps read keys through the row table."""
-    g, ML, off = cache.g, cache.max_len, cache.len
-    H, hd = g.H, g.hd
+    ML, off = cache.max_len, cache.len
     assert cache.B % seq_stride == 0 and (seq_stride == 1 or off == 0)
     B = cache.B // seq_stride
     assert x.shape[0] == B * n
@@ -1007,11 +1081,22 @@ def gpt_decode(W, x, cache, n, seq_stride=1):
         raise ValueError(f"KV cache overflow: {off} + {n} > {ML}")
     if off > 0 and n != 1:
         raise NotImplementedError("multi-token continuation after the first block is not supported")
+    x = _decode_layers(W, x, cache, n, off, B, SL)
+    cache._set_len(off + n)
+    cache.share_prefill(seq_stride)
+    return _last_hidden(W, x, cache.g, B, n)
+
+
+def _decode_layers(W, x, cache, n, off, B, SL, row0=0):
+    """gpt_decode's layers: B sequences of n new positions from position off, position p of sequence b in cache row
+    row0 + b * SL + p.  Returns the last layer's output [B*n, H] fp32."""
+    g = cache.g
+    H, hd = g.H, g.hd
     for i in range(g.layers):
         pre = f"{GPT}encoder.layers.{i}."
         ln1, _, _ = ops.layernorm_fwd(x, W[pre + "input_layernorm.weight"], W[pre + "input_layernorm.bias"], g.eps, stats=False)
-        buf = cache.qkv[i]
-        new_rows = buf[off:]  # GEMM row (b, i) -> buffer row b*max_len + off + i
+        buf = cache.qkv[i][row0:]
+        new_rows = buf[off:]  # GEMM row (b, i) -> buffer row b*SL + off + i
         ops.gemm(ln1, W[pre + "self_attention.query_key_value.weight"], bias=W[pre + "self_attention.query_key_value.bias"],
                  out=new_rows, d_row_block=n, d_row_stride=SL)
         att = torch.empty((B * n, H), device=x.device, dtype=bf16)
@@ -1028,8 +1113,11 @@ def gpt_decode(W, x, cache, n, seq_stride=1):
         h = ops.gemm(ln2, W[pre + "mlp.dense_h_to_4h.weight"], bias=W[pre + "mlp.dense_h_to_4h.bias"], act=ACT_GELU_TANH)
         x = ops.gemm(h, W[pre + "mlp.dense_4h_to_h.weight"], bias=W[pre + "mlp.dense_4h_to_h.bias"], residual=x1,
                      out_dtype=torch.float32)
-    cache._set_len(off + n)
-    cache.share_prefill(seq_stride)
+    return x
+
+
+def _last_hidden(W, x, g, B, n):
+    """Final-LayerNorm hidden state of the last of each sequence's n rows of x [B*n, H]: [B, H]."""
     last = torch.arange(B, device=x.device, dtype=torch.int32) * n + (n - 1)
     hid, _, _ = ops.layernorm_fwd(x, W[GPT + "encoder.final_layernorm.weight"], W[GPT + "encoder.final_layernorm.bias"], g.eps,
                                   in_rows=last, stats=False)

@@ -183,6 +183,19 @@ _ln_bwd = _declare("ymp_layernorm_bwd", LayerNormBwdArgs)
 _attn_fwd = _declare("ymp_attn_fwd", AttnArgs)
 _attn_fwd_prefix_table = _declare("ymp_attn_fwd_prefix_table", AttnPrefixTableArgs)
 _attn_fwd_prefix_kv = _declare("ymp_attn_fwd_prefix_kv", AttnPrefixKvArgs)
+
+
+def _declare_array(name, argstruct):
+    """An entry point that takes an argument struct plus one device array: name(args, array, stream)."""
+    fn = getattr(lib, name)
+    fn.restype = C.c_int
+    fn.argtypes = [C.POINTER(argstruct), c_vp, c_vp]
+    return fn
+
+
+_attn_fwd_seq_lens = _declare_array("ymp_attn_fwd_seq_lens", AttnArgs)
+_gemm_skinny_rows = _declare_array("ymp_gemm_skinny_rows", GemmSkinnyArgs)
+_gemm_skinny_wide_rows = _declare_array("ymp_gemm_skinny_wide_rows", GemmSkinnyArgs)
 _attn_bwd = _declare("ymp_attn_bwd", AttnBwdArgs)
 _im2col = _declare("ymp_im2col", Im2colArgs)
 _clip = _declare("ymp_clip_normalize", ClipArgs)

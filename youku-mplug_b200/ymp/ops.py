@@ -125,23 +125,25 @@ SKINNY_WIDE_MAX_ROWS = 64  # rows of ymp_gemm_skinny_wide (a batched beam search
 
 
 def gemm_skinny(x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_dtype=bf16, out2=None, out2_row_stride=0,
-                out2_off=None):
+                out2_off=None, out2_row_off=None):
     """y[M, N] = act(x[M, K] @ w[N, K]^T + bias) + residual for M <= 8 rows (single-token decoding): one pass over
     the weights on the HBM-bound kernel of csrc/gemv.cu instead of a mostly empty 128-row tensor-core tile.
     out2 [R, N] bf16 with out2_off (int64 device scalar): result row m is also written to out2 row
-    m * out2_row_stride + out2_off (the KV-cache row at the device-side cache length)."""
-    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, wide=False)
+    m * out2_row_stride + out2_off (the KV-cache row at the device-side cache length).  out2_row_off instead (int64
+    device array [M], ymp_gemm_skinny_rows): row m goes to out2 row m * out2_row_stride + out2_row_off[m] (sequences at
+    different cache lengths)."""
+    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, out2_row_off, wide=False)
 
 
 def gemm_skinny_wide(x, w, *, bias=None, residual=None, act=ACT_NONE, out=None, out_dtype=bf16, out2=None, out2_row_stride=0,
-                     out2_off=None):
+                     out2_off=None, out2_row_off=None):
     """gemm_skinny for up to SKINNY_WIDE_MAX_ROWS = 64 rows (ymp_gemm_skinny_wide): M <= 8 runs gemm_skinny's launch,
     9 <= M <= 64 a kernel with the same per-element arithmetic, so row m of the result is bit-identical to the same row
     computed by gemm_skinny.  The library rejects any call with more than 64."""
-    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, wide=True)
+    return _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, out2_row_off, wide=True)
 
 
-def _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, wide):
+def _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_stride, out2_off, out2_row_off, wide):
     _chk2d(x, "x"); _chk2d(w, "w")
     assert x.dtype == bf16 and w.dtype == bf16 and x.shape[1] == w.shape[1] and (wide or x.shape[0] <= SKINNY_MAX_ROWS)
     M, K, N = x.shape[0], x.shape[1], w.shape[0]
@@ -160,10 +162,17 @@ def _gemm_skinny(x, w, bias, residual, act, out, out_dtype, out2, out2_row_strid
     a.out_dtype = DT_F32 if out.dtype == torch.float32 else DT_BF16
     if out2 is not None:
         _chk2d(out2, "out2")
-        assert out2.dtype == bf16 and out2.shape[1] == N and out2_off.dtype == torch.int64 and out2_off.numel() == 1
+        assert out2.dtype == bf16 and out2.shape[1] == N and (out2_off is None) != (out2_row_off is None)
         assert out2.shape[0] >= (M - 1) * out2_row_stride + 1
-        a.y2, a.y2_off_dev = out2.data_ptr(), out2_off.data_ptr()
-        a.ldy2, a.y2_off_stride = out2_row_stride * out2.stride(0), out2.stride(0)
+        a.y2, a.ldy2, a.y2_off_stride = out2.data_ptr(), out2_row_stride * out2.stride(0), out2.stride(0)
+        if out2_row_off is not None:
+            assert out2_row_off.dtype == torch.int64 and out2_row_off.is_cuda and out2_row_off.is_contiguous()
+            assert out2_row_off.numel() == M
+            fn, what = (L._gemm_skinny_wide_rows, "ymp_gemm_skinny_wide_rows") if wide else (L._gemm_skinny_rows, "ymp_gemm_skinny_rows")
+            L.check(fn(L.C.byref(a), out2_row_off.data_ptr(), L.cur_stream()), what)
+            return out
+        assert out2_off.dtype == torch.int64 and out2_off.numel() == 1
+        a.y2_off_dev = out2_off.data_ptr()
     if wide:
         L.call(L._gemm_skinny_wide, a, "ymp_gemm_skinny_wide")
     else:
@@ -280,7 +289,7 @@ def _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, sca
 
 
 def attn_fwd(q, k, v, o, *, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, lse=None, mask_block=0,
-             total_rows=0, drop=None, s_kv_dev=None, kv_rows=None, n_prefix=None, cache=None):
+             total_rows=0, drop=None, s_kv_dev=None, kv_rows=None, n_prefix=None, cache=None, kv_lens=None):
     """q,k,v,o: TView.  Returns lse [n_seq, n_heads, s_q] fp32.  s_kv_dev: int32 device scalar, only the first
     min(s_kv, s_kv_dev) keys exist (the captured decoding step).  kv_rows: int32 CUDA tensor [n_seq, >= s_kv], key j of
     sequence s is row kv_rows[s, j] of k's / v's tensor (their seqmap is not used; s_q == 1 only, the decode kernel).
@@ -289,11 +298,18 @@ def attn_fwd(q, k, v, o, *, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, 
     upper bound on n_prefix + s_q (k.m.n_prefix is not used).
     cache (with n_prefix): (kc, vc, n0), TViews of the prefix cache (their seqmaps are not used) and its keys per prefix
     (ymp_attn_fwd_prefix_kv): the first n0 of sequence s's n_prefix keys are rows (s // seq_div) * n0 + j of kc / vc,
-    the other n_prefix - n0 are k's / v's seqmap prefix rows."""
+    the other n_prefix - n0 are k's / v's seqmap prefix rows.
+    kv_lens: int32 CUDA tensor [n_seq] (ymp_attn_fwd_seq_lens): sequence s attends to its first min(s_kv, kv_lens[s])
+    keys (one decoding step over sequences at different cache lengths; s_q == 1, the decode kernel)."""
     if lse is None:
         lse = torch.empty((n_seq, n_heads, s_q), device=q.t.device, dtype=torch.float32)
     a = _attn_args(q, k, v, o, lse, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, mask_block, total_rows, drop, s_kv_dev,
                    kv_rows)
+    if kv_lens is not None:
+        assert n_prefix is None and kv_lens.dtype == torch.int32 and kv_lens.is_cuda and kv_lens.is_contiguous()
+        assert kv_lens.numel() == n_seq, (kv_lens.numel(), n_seq)
+        L.check(L._attn_fwd_seq_lens(L.C.byref(a), kv_lens.data_ptr(), L.cur_stream()), "ymp_attn_fwd_seq_lens")
+        return lse
     if n_prefix is None:
         L.call(L._attn_fwd, a, "ymp_attn_fwd")
         return lse
