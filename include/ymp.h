@@ -338,6 +338,24 @@ typedef struct ymp_attn_prefix_kv_args {
 } ymp_attn_prefix_kv_args;
 int ymp_attn_fwd_prefix_kv(const ymp_attn_prefix_kv_args* a, void* stream);
 
+/* Causal attention over variable-length sequences stored back to back, without padding rows (the retrieval
+ * evaluation's text features: texts of different lengths in one launch).  Sequence s is rows starts[s] ..
+ * starts[s + 1] - 1 of q, k, v and o (element = base[row * ld + head * head_stride + d], as for ymp_attn_args), so it
+ * has len_s = starts[s + 1] - starts[s] rows; row i of it attends to rows starts[s] .. starts[s] + i.  Query and key
+ * tiles are aligned to starts[s], so each row's O and lse are bit-identical to the same row of ymp_attn_fwd's square
+ * causal call on the sequences padded to a common length.  A sequence of length 0 writes nothing, and no row outside
+ * [starts[0], starts[n_seq]) is written.  attn.n_seq sequences; attn.mask must be YMP_MASK_CAUSAL; attn.s_q, attn.s_kv
+ * and the three seqmaps are not read.  lse (optional): fp32 [rows, n_heads], lse[row * n_heads + head].
+ * Preconditions, not checked: starts is non-decreasing and every len_s <= max_len.  Forward only, head_dim 64 / 80 /
+ * 88 / 96, no dropout, total_rows, s_kv_dev or kv_rows; served by the wgmma tiles. */
+typedef struct ymp_attn_packed_args {
+  ymp_attn_args attn;
+  const int32_t* starts;  /* DEVICE array [n_seq + 1]: first row of each sequence, then the end of the last one */
+  int32_t max_len;        /* >= every len_s: sizes the grid ((max_len + 63) / 64 query tiles per sequence); 0: no launch */
+  int32_t _pad;
+} ymp_attn_packed_args;
+int ymp_attn_fwd_packed(const ymp_attn_packed_args* a, void* stream);
+
 typedef struct ymp_attn_bwd_args {
   ymp_attn_args fwd;      /* the forward call's arguments (q,k,v,o,lse and maps) */
   const void* dout;       /* bf16, addressed by map_do / lddo / do_head_stride */

@@ -12,7 +12,8 @@
 // attention_small.cu (block-diagonal sequences of <= 16 rows: TimeSformer temporal attention) and to the
 // single-query decoding kernel, and run everything else here.  ymp_attn_fwd_prefix_table runs the wgmma forward's
 // TABLE variant: causal with a key prefix per sequence read from a device table; ymp_attn_fwd_prefix_kv its CACHE
-// variant, whose prefix starts with rows of a separate K / V tensor (a prefix's keys computed by an earlier call).
+// variant, whose prefix starts with rows of a separate K / V tensor (a prefix's keys computed by an earlier call);
+// ymp_attn_fwd_packed its PACKED variant: causal within each of many sequences stored back to back.
 //   forward   : CTA = 64 query rows x (seq, head); K/V tiles streamed with cp.async double buffering
 //   backward  : two kernels, no atomics, deterministic -
 //               dQ   kernel: CTA = 64 query rows, streams K/V   (also emits delta = rowsum(dO*O))
@@ -119,6 +120,7 @@ struct AttnKParams {
                        // keys before its s_q queries
   const __nv_bfloat16 *kc, *vc;  // prefix cache (CACHE variant): key j < n0 of sequence s is row (s / mkv.seq_div) * n0 + j
   int ldc, hsc, n0;
+  const int* starts;   // packed sequences (PACKED variant): sequence s is rows starts[s] .. starts[s + 1] - 1
 };
 
 // keep-or-drop of the two adjacent key columns col, col+1 (col even) of `row`: scale or zero in place
@@ -375,7 +377,8 @@ __device__ __forceinline__ void stage_dkdv_stats(const AttnKParams& p, size_t st
 
 // Epilogues of a warp's 16 rows (row_lo + g, + 8) from their C fragments; columns DIO..D-1 are never stored.
 // Forward: O = o_acc / l (after the quad sums this thread's partial l_i) and lse = m * scale + log(l).
-template <int D, int DIO>
+// PACKED: lse is [rows, n_heads], indexed by the output row.
+template <int D, int DIO, bool PACKED = false>
 __device__ __forceinline__ void store_o_lse(const AttnKParams& p, const float (&o_acc)[D / 8][4], const float (&m_i)[2],
                                             float (&l_i)[2], int row_lo, int sq, int s, int h, const RSeq& mo, int g,
                                             int t4) {
@@ -393,7 +396,10 @@ __device__ __forceinline__ void store_o_lse(const AttnKParams& p, const float (&
 #pragma unroll
     for (int nb = 0; nb < DIO / 8; ++nb)
       *reinterpret_cast<uint32_t*>(orow + nb * 8 + t4 * 2) = pack_bf16(o_acc[nb][2 * r] * inv, o_acc[nb][2 * r + 1] * inv);
-    if (p.lse && t4 == 0) p.lse[((size_t)s * p.n_heads + h) * p.s_q + qi] = m_i[r] * p.scale + logf(l_i[r]);
+    if (p.lse && t4 == 0) {
+      const size_t li = PACKED ? (size_t)rrow(mo, qi) * p.n_heads + h : ((size_t)s * p.n_heads + h) * p.s_q + qi;
+      p.lse[li] = m_i[r] * p.scale + logf(l_i[r]);
+    }
   }
 }
 // dQ = scale * dq_acc
@@ -878,11 +884,20 @@ __device__ __forceinline__ auto with_cache(const RMat& m, const __nv_bfloat16* c
   else return m;
 }
 
+// The rows of sequence s: through the seqmap m, or (PACKED) rows r0, r0 + 1, ... of a packed buffer.
+template <bool PACKED>
+__device__ __forceinline__ RSeq seq_rows(const SeqMap& m, int s, int r0) {
+  if constexpr (PACKED) return RSeq{r0, 1, 0, 0};
+  else return resolve(m, s);
+}
+
 // TABLE: causal with a key prefix per sequence (ymp_attn_fwd_prefix_table): sequence s has qoff = n_prefix[s / seq_div]
 // keys before its s_q queries, the first qoff taken from map_kv's prefix rows; s_kv only bounds the grid.
 // CACHE (with TABLE, ymp_attn_fwd_prefix_kv): the first n0 of those qoff keys come from the prefix cache, the other
 // qoff - n0 from map_kv's prefix rows.  The tile alignment and key range still follow qoff alone.
-template <int D, int DIO, bool TABLE = false, bool CACHE = false>
+// PACKED (ymp_attn_fwd_packed; square causal, qoff = 0): sequence s is rows starts[s] .. starts[s + 1] - 1 of q, k, v
+// and o, its tiles aligned to its first row; s_q only bounds the grid.
+template <int D, int DIO, bool TABLE = false, bool CACHE = false, bool PACKED = false>
 __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   constexpr int TB = WgTile<D>::BYTES;
   extern __shared__ uint8_t smem_wg[];
@@ -906,11 +921,16 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
   int sq, skv;
   eff_len(p, s, sq, skv);
   if constexpr (TABLE) skv = qoff + sq;
+  int r0 = 0;
+  if constexpr (PACKED) {
+    r0 = __ldg(p.starts + s);
+    sq = skv = __ldg(p.starts + s + 1) - r0;
+  }
   if (q0 >= sq) return;  // (TABLE: the grid has a tile for every alignment; the surplus ones end here)
-  RSeq mkv = resolve(p.mkv, s);
-  const RSeq mo = resolve(p.mo, s);
+  RSeq mkv = seq_rows<PACKED>(p.mkv, s, r0);
+  const RSeq mo = seq_rows<PACKED>(p.mo, s, r0);
   if constexpr (TABLE) mkv.n_prefix = CACHE ? qoff - p.n0 : qoff;
-  const RMat Mq = rmat(p.q, resolve(p.mq, s), p.ldq, h * p.hsq);
+  const RMat Mq = rmat(p.q, seq_rows<PACKED>(p.mq, s, r0), p.ldq, h * p.hsq);
   const auto Mk = with_cache<CACHE>(rmat(p.k, mkv, p.ldk, h * p.hsk), p.kc, p, s, h);
   const auto Mv = with_cache<CACHE>(rmat(p.v, mkv, p.ldv, h * p.hsv), p.vc, p, s, h);
   int kv_begin;
@@ -953,7 +973,7 @@ __global__ void __launch_bounds__(128) attn_wg_fwd_kernel(const AttnKParams p) {
     wg_pv<D>(o_acc, sc, smem_u32(Vs));
     __syncthreads();  // every warpgroup MMA of this stage has retired before it is refilled
   }
-  store_o_lse<D, DIO>(p, o_acc, m_i, l_i, q0 + warp * 16, sq, s, h, mo, g, t4);
+  store_o_lse<D, DIO, PACKED>(p, o_acc, m_i, l_i, q0 + warp * 16, sq, s, h, mo, g, t4);
 }
 
 // dQ (and delta = rowsum(dO * O) for the dK / dV kernel, which runs after this one)
@@ -1296,6 +1316,15 @@ static int launch_wg_fwd_table(const AttnKParams& p, int head_dim, cudaStream_t 
     return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO, true, CACHE>>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
   });
 }
+// Packed sequences: one query tile per 64 rows of the longest one (p.s_q = max_len); a sequence's surplus tiles end at
+// once.
+static int launch_wg_fwd_packed(const AttnKParams& p, int head_dim, cudaStream_t st) {
+  const dim3 grid((p.s_q + 63) / 64, p.n_heads, p.n_seq);
+  return for_head_dim<false>(head_dim, [&](auto hd) {
+    using H = decltype(hd);
+    return launch_attn<attn_wg_fwd_kernel<H::D, H::DIO, false, false, true>>(grid, 5 * WgTile<H::D>::BYTES + 1024, st, p);
+  });
+}
 static int launch_wg_bwd(const AttnKParams& p, int head_dim, cudaStream_t st) {
   return for_head_dim<false>(head_dim, [&](auto hd) {
     using H = decltype(hd);
@@ -1433,6 +1462,30 @@ extern "C" int ymp_attn_fwd_prefix_kv(const ymp_attn_prefix_kv_args* c, void* st
   p.ldc = c->ld_cache; p.hsc = c->cache_head_stride; p.n0 = c->n0;
   g_attn_path = YMP_ATTN_PATH_WGMMA;
   return launch_wg_fwd_table<true>(p, c->table.attn.head_dim, (cudaStream_t)stream);
+}
+
+extern "C" int ymp_attn_fwd_packed(const ymp_attn_packed_args* a, void* stream) {
+  using namespace ymp;
+  const char* who = "ymp_attn_fwd_packed";
+  YMP_CHECK_ARG(a != nullptr, "%s: null args", who);
+  YMP_CHECK_ARG(a->starts != nullptr, "%s: null starts", who);
+  YMP_CHECK_ARG(a->max_len >= 0, "%s: max_len must be >= 0", who);
+  ymp_attn_args t = a->attn;
+  t.s_q = t.s_kv = a->max_len > 0 ? a->max_len : 1;   // (only bounds the grid)
+  AttnKParams p = {};
+  const int rc = fill_params(&t, p, who);
+  if (rc) return rc;
+  YMP_CHECK_ARG(t.o && aligned16(t.o), "%s: bad o", who);
+  YMP_CHECK_ARG(t.mask == YMP_MASK_CAUSAL, "%s: the mask must be causal", who);
+  YMP_CHECK_ARG(t.head_dim != 128, "%s: needs head_dim 64, 80, 88 or 96", who);
+  YMP_CHECK_ARG(!p.has_drop, "%s: takes no dropout", who);
+  YMP_CHECK_ARG(!t.s_kv_dev, "%s: takes no s_kv_dev", who);
+  YMP_CHECK_ARG(!t.kv_rows, "%s: takes no kv_rows", who);
+  YMP_CHECK_ARG(t.total_rows == 0, "%s: takes no total_rows (starts gives every sequence's rows)", who);
+  p.starts = a->starts;
+  g_attn_path = YMP_ATTN_PATH_WGMMA;
+  if (a->max_len == 0) return YMP_OK;   // every sequence is empty: nothing to write
+  return launch_wg_fwd_packed(p, t.head_dim, (cudaStream_t)stream);
 }
 
 extern "C" int ymp_attn_bwd(const ymp_attn_bwd_args* b, void* stream) {

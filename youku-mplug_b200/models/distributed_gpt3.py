@@ -336,11 +336,8 @@ class _PromptClsBase(_PrefixModelBase):
     # computed once per video too (shared_text_columns).  The outputs are bit-identical to the passes above on the
     # repeated prefixes.
     def _shared_prefix_ok(self, query_features):
-        """True when the eval passes may share the prefixes: no backward can be needed (grad mode off, or neither the
-        query features nor any decoder parameter requires grad) and the decoder's dropout is inactive."""
-        needs_grad = torch.is_grad_enabled() and (query_features.requires_grad
-                                                  or any(p.requires_grad for p in self.text_decoder.parameters()))
-        return not needs_grad and not self.text_decoder.dropout_active()
+        """True when the eval passes may share the prefixes (decoder_forward_only with the query features as input)."""
+        return decoder_forward_only(self.text_decoder, query_features)
 
     # An eval call keeps the prefixes' keys and values of its first pass (a lazy DistributedGPT3.prefix_kv) and its
     # second pass reads them.
@@ -405,6 +402,15 @@ class _PromptClsBase(_PrefixModelBase):
         return self.cls_head(self.text_decoder.forward_shared_prefix(query_features, emb, hidden_rows=rows,
                                                                      shared_cols=shared, used_cols=used,
                                                                      prefix_kv=prefix_kv).hidden)
+
+
+def decoder_forward_only(decoder, *inputs):
+    """May a forward-only decoder pass (no saved activations, no dropout) replace the training-step pass: no backward
+    through the decoder can be needed (grad mode off, or neither an input nor any decoder parameter requires grad) and
+    the decoder's dropout is inactive."""
+    needs_grad = torch.is_grad_enabled() and (any(t.requires_grad for t in inputs)
+                                              or any(p.requires_grad for p in decoder.parameters()))
+    return not needs_grad and not decoder.dropout_active()
 
 
 def prefix_cache_hit(entry, image, weights, ok):
@@ -539,11 +545,26 @@ class DistributedGPT3_Retrieval(_PrefixModelBase):
         return F.normalize(self.vision_proj(pooled).float(), dim=-1)
 
     def extract_text_feature(self, text):
+        """Normalised projection of each text's decoder state at its last valid token.  When no backward through the
+        decoder can be needed and its dropout is off (the evaluation, or a training step with a frozen decoder and no
+        dropout), the texts run packed without padding rows and without the LM head (DistributedGPT3.text_features), with
+        bit-identical results.  A pass with the decoder's dropout active keeps the padded pass: its masks are keyed by the
+        padded row index.  So does a pass captured into a CUDA graph: the packed layout is read from the mask on the
+        host, and a replay would reuse the captured texts' layout for every later batch."""
+        capturing = text.input_ids.is_cuda and torch.cuda.is_current_stream_capturing()
+        if decoder_forward_only(self.text_decoder) and not capturing:
+            pooled = self.text_decoder.text_features(text.input_ids, text.attention_mask)
+        else:
+            pooled = self._pooled_text_padded(text)
+        return F.normalize(self.text_proj(pooled).float(), dim=-1)
+
+    def _pooled_text_padded(self, text):
+        """The decoder state at each text's last valid token from the training-step pass over the padded texts (LM head
+        and per-token CE included, reference :922-936)."""
         targets = torch.cat([text.input_ids[:, 1:], text.input_ids[:, 1:2]], dim=1)
         out = self.text_decoder(tokens=text.input_ids, loss_mask=text.attention_mask[:, 1:].clone(), labels=targets)
         hid = out.last_hidden_state
-        pooled = hid[torch.arange(hid.shape[0], device=hid.device), text.attention_mask.sum(dim=-1) - 1]
-        return F.normalize(self.text_proj(pooled).float(), dim=-1)
+        return hid[torch.arange(hid.shape[0], device=hid.device), text.attention_mask.sum(dim=-1) - 1]
 
     def forward(self, image, text, idx):
         image_feat = self.extract_vision_feature(image)

@@ -799,6 +799,16 @@ class DistributedGPT3(nn.Module):
         """Does a pass in the current mode draw dropout masks (train() mode and a non-zero probability)?"""
         return YF.gpt_dropout_active(self.config.engine_cfg(self.training))
 
+    def text_features(self, tokens, attention_mask):
+        """Pooled final hidden states [B, H] of the texts tokens [B, L]: for each text, the final-LayerNorm state of
+        column attention_mask.sum(-1) - 1, bit-identical to that row of forward(tokens=...).last_hidden_state.  The texts
+        are packed back to back without padding rows (ymp.functional.gpt_text_features) and no LM head is run.  Forward
+        only and without dropout."""
+        if self.dropout_active():
+            raise ValueError("text_features: the decoder's dropout is active (train() mode with p > 0)")
+        keys, params = self._param_list()
+        return YF.gpt_text_features(tokens, attention_mask, self.config.engine_cfg(self.training), keys, params)
+
     def prefix_kv(self, query_embeds, lazy=False):
         """Keys and values of the V prefixes query_embeds [V,Q,H] at every decoder layer (ymp.engine.PrefixKV, [layers,
         V*Q, 2H] bf16): pass it to forward_shared_prefix(prefix_kv=...) with the same query_embeds to score any number

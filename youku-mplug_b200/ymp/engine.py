@@ -793,6 +793,28 @@ def gpt_fwd_shared_prefix(W, x, gcfg, V, t, Q, L, out_rows=None, shared=None, pr
     return hid
 
 
+def gpt_fwd_packed(W, x, gcfg, starts, max_len, out_rows):
+    """Forward-only decoder pass over sequences stored back to back without padding rows (the retrieval text features).
+    x [T, H] fp32: sequence s is rows starts[s] .. starts[s+1]-1 (starts: int32 CUDA tensor [n_seq + 1]), row starts[s]
+    + j holding its embedding + position j; max_len bounds every length.  Each layer runs its LayerNorms and GEMMs over
+    the T rows and causal attention within each sequence (ops.attn_fwd_packed).  Every kernel computes each row on its
+    own, so each row is bit-identical to the same row of gpt_fwd on the sequences padded to a common length.  No dropout,
+    no LM head, nothing kept for a backward.  Returns the final-LayerNorm hidden states of out_rows (int32 indices into
+    x's rows), [len(out_rows), H] bf16."""
+    g = GptDims(gcfg)
+    assert x.dim() == 2 and x.shape[1] == g.H and x.dtype == torch.float32
+
+    def attend(qkv, att):
+        ops.attn_fwd_packed(*(TView(qkv, j * g.hd, 3 * g.hd, None) for j in range(3)), TView(att, 0, g.hd, None),
+                            starts=starts, max_len=max_len, n_heads=g.heads, head_dim=g.hd, scale=g.scale)
+
+    for i in range(g.layers):
+        x, _ = gpt_layer_fwd(W, f"{GPT}encoder.layers.{i}.", x, g, None, None, attend=attend)
+    hid, _, _ = ops.layernorm_fwd(x, W[GPT + "encoder.final_layernorm.weight"], W[GPT + "encoder.final_layernorm.bias"], g.eps,
+                                  in_rows=out_rows)
+    return hid
+
+
 def gpt_layer_saved(W, c, i):
     """What layer i's backward reads: the activations kept by gpt_fwd, or in recompute mode the same tensors rebuilt
     from the layer's saved input (deterministic kernels, counter-based dropout masks: bit-identical to the kept ones)."""

@@ -529,6 +529,49 @@ def gpt_prefix_kv(query_embeds, gcfg, keys, params):
         return engine.gpt_prefix_kv(W, query_embeds, gcfg)
 
 
+def packed_text_rows(attention_mask):
+    """Host-side layout of gpt_text_features' packed rows, from one host read of the mask [B, L]: (starts, lengths,
+    pooled), int64 CPU tensors [B + 1], [B], [B].  The pooled column of text b is attention_mask[b].sum() - 1, the
+    reference's pooling index (read as Python indexes it: -1 is column L - 1).  Text b keeps its columns 0 ..
+    lengths[b] - 1 with lengths[b] = 1 + max(last attended column, pooled column), which holds for a mask with holes
+    too; under the causal mask no kept column sees a dropped one.  starts[b] is its first packed row and pooled[b] =
+    starts[b] + pooled column its pooled row."""
+    att = attention_mask.detach().to("cpu", torch.int64)
+    B, L = att.shape
+    col = att.sum(-1) - 1
+    if bool(((col < -L) | (col >= L)).any()):
+        raise ValueError(f"packed_text_rows: pooled columns {col.tolist()} outside a mask of {L} columns")
+    col = torch.where(col < 0, col + L, col)
+    last = torch.where(att.ne(0), torch.arange(L), -1).amax(-1) if L else torch.full((B,), -1)
+    lengths = 1 + torch.maximum(last, col)
+    starts = torch.zeros(B + 1, dtype=torch.int64)
+    starts[1:] = lengths.cumsum(0)
+    return starts, lengths, starts[:-1] + col
+
+
+def gpt_text_features(tokens, attention_mask, gcfg, keys, params):
+    """Final hidden state of each text's pooled column (attention_mask.sum(-1) - 1) for tokens [B, L], from one
+    forward-only decoder pass over the texts packed back to back (engine.gpt_fwd_packed; packed_text_rows gives the
+    rows): no padding rows, no LM head, no dropout.  The input rows use GptFn's dtype chain (the word embedding in its
+    parameter's dtype, then + the position of the column within its text, in fp32), so the result [B, H] bf16 is
+    bit-identical to the same rows of GptFn's hidden states on the padded tokens."""
+    _require_cuda(tokens, "gpt_text_features")
+    if gpt_dropout_active(gcfg):
+        raise ValueError("gpt_text_features: the decoder's dropout is active; the packed pass is forward only")
+    W = {k: as_bf16(p) for k, p in zip(keys, params)}
+    word = dict(zip(keys, params))[engine.GPT + "embedding.word_embeddings.weight"]
+    dev = tokens.device
+    starts, lengths, pooled = packed_text_rows(attention_mask)
+    text = torch.repeat_interleave(torch.arange(len(lengths)), lengths)
+    col = torch.arange(int(starts[-1])) - starts[:-1][text]
+    text, col = text.to(dev), col.to(dev)
+    pos = W[engine.GPT + "embedding.position_embeddings.weight"]
+    with torch.no_grad():
+        x = (torch.nn.functional.embedding(tokens[text, col], word).float() + pos[col].float()).contiguous()
+        return engine.gpt_fwd_packed(W, x, gcfg, starts.to(device=dev, dtype=torch.int32), int(lengths.max()),
+                                     pooled.to(device=dev, dtype=torch.int32))
+
+
 def gpt_shared_prefix(query_embeds, input_embeds, labels, hidden_rows, gcfg, keys, params, shared=None, used=None,
                       prefix_kv=None):
     """Forward-only decoder pass over [prefix v | text n] for N = V*t texts, text n after prefix v = n // t, with each

@@ -98,6 +98,10 @@ class AttnPrefixKvArgs(C.Structure):
                 ("cache_head_stride", c_i32), ("n0", c_i32), ("_pad", c_i32)]
 
 
+class AttnPackedArgs(C.Structure):
+    _fields_ = [("attn", AttnArgs), ("starts", c_vp), ("max_len", c_i32), ("_pad", c_i32)]
+
+
 class GemmSkinnyArgs(C.Structure):
     _fields_ = [("x", c_vp), ("w", c_vp), ("bias", c_vp), ("residual", c_vp), ("y", c_vp),
                 ("M", c_i32), ("N", c_i32), ("K", c_i32), ("ldx", c_i32), ("ldw", c_i32), ("ldr", c_i32), ("ldy", c_i32),
@@ -183,6 +187,7 @@ _ln_bwd = _declare("ymp_layernorm_bwd", LayerNormBwdArgs)
 _attn_fwd = _declare("ymp_attn_fwd", AttnArgs)
 _attn_fwd_prefix_table = _declare("ymp_attn_fwd_prefix_table", AttnPrefixTableArgs)
 _attn_fwd_prefix_kv = _declare("ymp_attn_fwd_prefix_kv", AttnPrefixKvArgs)
+_attn_fwd_packed = _declare("ymp_attn_fwd_packed", AttnPackedArgs)
 
 
 def _declare_array(name, argstruct):

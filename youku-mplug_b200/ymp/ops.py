@@ -329,6 +329,26 @@ def attn_fwd(q, k, v, o, *, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale, 
     return lse
 
 
+def attn_fwd_packed(q, k, v, o, *, starts, max_len, n_heads, head_dim, scale, lse=None):
+    """Causal attention within each of n_seq sequences stored back to back in q / k / v / o (TViews; their seqmaps are
+    not used), ymp_attn_fwd_packed: sequence s is rows starts[s] .. starts[s + 1] - 1 (starts: int32 CUDA tensor
+    [n_seq + 1]) and max_len bounds every length.  Each row is bit-identical to the same row of attn_fwd's square causal
+    call on the sequences padded to a common length; no row outside [starts[0], starts[-1]) is written.
+    lse: fp32 [rows, n_heads] CUDA tensor that receives lse[row, head], or None."""
+    assert starts.dtype == torch.int32 and starts.is_cuda and starts.is_contiguous() and starts.dim() == 1, starts
+    assert starts.numel() >= 2, "attn_fwd_packed: starts needs n_seq + 1 >= 2 entries"
+    if lse is not None:
+        assert lse.dtype == torch.float32 and lse.is_cuda and lse.is_contiguous() and lse.dim() == 2 and lse.shape[1] == n_heads
+    rows = seqmap()   # (not read: starts gives every sequence's rows)
+    q, k, v, o = (TView(t.t, t.col, t.hs, rows) for t in (q, k, v, o))
+    a = L.AttnPackedArgs()
+    a.attn = _attn_args(q, k, v, o, lse, starts.numel() - 1, n_heads, head_dim, max(1, max_len), max(1, max_len), MASK_CAUSAL,
+                        scale)
+    a.starts, a.max_len = starts.data_ptr(), max_len
+    L.call(L._attn_fwd_packed, a, "ymp_attn_fwd_packed")
+    return lse
+
+
 def attn_bwd(q, k, v, o, lse, dout, dq, dk, dv, *, n_seq, n_heads, head_dim, s_q, s_kv, causal, scale,
              mask_block=0, total_rows=0, drop=None):
     """dout,dq,dk,dv: TView (dk and dv share dk's seqmap)."""
