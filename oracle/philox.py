@@ -27,24 +27,40 @@ def philox4x32_10(c0, c1, c2, c3, k0, k1):
     return tuple(c.astype(np.uint32) for c in (c0, c1, c2, c3))
 
 
-def keep_mask(seed, offset, site, rows, cols, p):
-    """Boolean keep-mask [len(rows), cols] for logical rows `rows` (1-D integer array) and columns 0..cols-1:
-    counter = (col >> 2, row, site, offset), key = seed; keep iff word[col & 3] >= floor(p * 2^32)."""
+def threshold(p):
+    """The keep threshold of drop_state (philox.cuh): the kernels receive p as an fp32, so floor(fl32(p) * 2^32)
+    (exact in double), saturating at 0xFFFFFFFF.  At p = 0.1 this is 429496736, not the 429496729 of the double p."""
+    t = float(np.float32(p)) * 4294967296.0
+    return 0xFFFFFFFF if t >= 4294967295.0 else int(t)
+
+
+def scale(p):
+    """The kept-value multiplier of drop_state: 1.0f / (1.0f - fl32(p)), every step in fp32."""
+    one = np.float32(1.0)
+    return float(one / (one - np.float32(p)))
+
+
+def words(seed, offset, site, rows, cols):
+    """uint32 [len(rows), cols]: the Philox word of every (row, column), counter = (col >> 2, row, site, offset),
+    key = seed, word col & 3 of the four."""
     rows = np.asarray(rows, dtype=np.uint64).reshape(-1, 1)
     c4 = (np.arange((cols + 3) // 4, dtype=np.uint64)).reshape(1, -1)
     w = philox4x32_10(np.broadcast_to(c4, (rows.shape[0], c4.shape[1])), np.broadcast_to(rows, (rows.shape[0], c4.shape[1])),
                       np.uint64(site), np.uint64(int(offset) & 0xFFFFFFFF), int(seed) & 0xFFFFFFFF, (int(seed) >> 32) & 0xFFFFFFFF)
-    words = np.stack(w, axis=-1).reshape(rows.shape[0], -1)[:, :cols]
-    t = p * 4294967296.0
-    thresh = 0xFFFFFFFF if t >= 4294967295.0 else int(t)
-    return words >= np.uint32(thresh)
+    return np.stack(w, axis=-1).reshape(rows.shape[0], -1)[:, :cols]
+
+
+def keep_mask(seed, offset, site, rows, cols, p):
+    """Boolean keep-mask [len(rows), cols] for logical rows `rows` (1-D integer array) and columns 0..cols-1:
+    keep iff word(row, col) >= threshold(p)."""
+    return words(seed, offset, site, rows, cols) >= np.uint32(threshold(p))
 
 
 def dropout(x, seed, offset, site, p, rows=None):
-    """torch tensor [R, C] -> dropout(x) with the kernels' mask; rows default to 0..R-1."""
+    """torch tensor [R, C] -> dropout(x) with the kernels' mask and scale; rows default to 0..R-1."""
     import torch
     if p <= 0.0:
         return x
     R, C = x.shape
     m = keep_mask(seed, offset, site, np.arange(R) if rows is None else rows, C, p)
-    return x * torch.from_numpy(m).to(x.dtype) * (1.0 / (1.0 - p))
+    return x * torch.from_numpy(m).to(x.dtype) * scale(p)

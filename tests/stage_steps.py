@@ -95,8 +95,7 @@ def drop_mult(spec, rows, cols, dev):
     from oracle import philox
     seed, off, site, p = spec
     keep = philox.keep_mask(seed, off, site, np.asarray(rows, dtype=np.int64), cols, p)
-    k = f32(1.0 / (1.0 - f32(p)))
-    return torch.from_numpy(keep).to(dev).to(F64) * k
+    return torch.from_numpy(keep).to(dev).to(F64) * philox.scale(p)
 
 
 def _same(a, b):

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import attn_bounds as AB
+from oracle import philox
 
 bf16 = torch.bfloat16
 
@@ -142,7 +143,7 @@ def test_geometric_values_expose_a_late_causal_leak():
 def _mult(n, H, sq, skv, p, seed):
     g = torch.Generator().manual_seed(seed)
     keep = torch.rand(n, H, sq, skv, generator=g) >= p
-    return keep.double() * float(torch.tensor(1.0 / (1.0 - p), dtype=torch.float32))
+    return keep.double() * philox.scale(p)
 
 
 @pytest.mark.parametrize("mask,sq,skv", [(AB.MASK_CAUSAL, 70, 70), (AB.MASK_NONE, 33, 97)])

@@ -13,7 +13,9 @@ Each case
     a key that leaks through the mask moves O by more than the bound;
   - tests the backward in isolation (given the reference O rounded to bf16 and the reference lse), and for one case
     per family chained to the kernel's own forward (with the forward's bounds as the input error).
-Set YMP_ATTN_BOUNDS_REPORT=<file> to write the largest err / bound per family and tensor as JSON.
+Under dropout on the probabilities the reference and the bounds take the oracle's multiplier keep / (1 - p).
+Set YMP_ATTN_BOUNDS_REPORT=<file> to write the largest err / bound per family and tensor as JSON (the families under
+dropout as "<family>+drop", and "mma_sync+drop(per-element)" for the dK / dV kernel's per-element Philox calls).
 """
 import json
 import math
@@ -23,6 +25,7 @@ import pytest
 import torch
 
 import attn_bounds as AB
+import stage_steps as SS
 
 pytestmark = pytest.mark.gpu
 bf16 = torch.bfloat16
@@ -31,6 +34,7 @@ SENT16 = 0x7FA5          # bf16 NaN bit pattern of untouched output memory
 SENT32 = 0x7FA0BEEF      # fp32 NaN bit pattern of untouched lse memory
 POISON = 3.0e4           # finite poison of input memory no kernel may read
 ROW0 = 2                 # rows of every buffer before the addressed view
+DROP_SEED, DROP_OFFSET, DROP_SITE = 0x1234567812345, 7, 4 * 5 + 1
 RATIOS = {}
 
 
@@ -49,23 +53,24 @@ def _report():
             json.dump(RATIOS, f, indent=1, sort_keys=True)
 
 
-def fwd_family(hd, s_q, s_kv, mask, mask_block=0, total_rows=0, kv_dev=False):
-    """The family ymp.h documents for a forward call (no dropout, dense seqmaps under block masks)."""
+def fwd_family(hd, s_q, s_kv, mask, mask_block=0, total_rows=0, kv_dev=False, drop=False):
+    """The family ymp.h documents for a forward call (dense seqmaps under block masks).  Under dropout neither the
+    decode kernel nor the warp-per-sequence kernel runs."""
     from ymp import lib
     if mask == AB.MASK_CAUSAL and s_q < s_kv:
         return lib.ATTN_PATH_WGMMA
-    if s_q == 1 and mask == AB.MASK_NONE and not total_rows and hd not in (88, 128):
+    if s_q == 1 and mask == AB.MASK_NONE and not total_rows and hd not in (88, 128) and not drop:
         return lib.ATTN_PATH_DECODE
-    if mask == AB.MASK_BLOCK and mask_block <= 16 and hd != 88 and not kv_dev:
+    if mask == AB.MASK_BLOCK and mask_block <= 16 and hd != 88 and not kv_dev and not drop:
         return lib.ATTN_PATH_SMALL
     if hd == 128 or mask == AB.MASK_BLOCK or kv_dev or (s_q < 16 and s_kv > 256):
         return lib.ATTN_PATH_MMA_SYNC
     return lib.ATTN_PATH_WGMMA
 
 
-def bwd_family(hd, mask, mask_block=0):
+def bwd_family(hd, mask, mask_block=0, drop=False):
     from ymp import lib
-    if mask == AB.MASK_BLOCK and mask_block <= 16 and hd != 88:
+    if mask == AB.MASK_BLOCK and mask_block <= 16 and hd != 88 and not drop:
         return lib.ATTN_PATH_SMALL
     if hd == 128 or mask == AB.MASK_BLOCK:
         return lib.ATTN_PATH_MMA_SYNC
@@ -155,10 +160,19 @@ def _check(fam, what, got, want, bound, where):
                              f"bound {bound.flatten()[idx].item():.3g}")
 
 
+def _drop_name(name, hd, drop, bwd=False):
+    """Report name of a family under dropout; the mma.sync dK / dV kernel draws one Philox call per element at head_dim
+    88 and 96 and shares calls within a quad of lanes otherwise."""
+    if not drop:
+        return name
+    return name + ("+drop(per-element)" if bwd and name == "mma_sync" and hd in (88, 96) else "+drop")
+
+
 def run(cuda, *, hd, s_q, s_kv, n=2, H=2, mask=AB.MASK_NONE, mask_block=0, total_rows=0, kv_count=None, maps=None,
-        fwd_path, bwd_path=None, chained=False, probe=None, seed=0):
+        fwd_path, bwd_path=None, chained=False, probe=None, seed=0, drop=None):
     """One forward (and, with bwd_path, one isolated backward; with chained, also one backward from the kernel's own
-    O and lse) checked element-wise, with sentinels and the served family."""
+    O and lse) checked element-wise, with sentinels and the served family.  drop: the probability of dropout on the
+    attention probabilities (the reference and the bounds take the oracle's keep / (1 - p))."""
     from ymp import lib, ops
     gen = torch.Generator().manual_seed(seed)
     maps = dict(dict(q=AB.dense(s_q), kv=AB.dense(s_kv), o=AB.dense(s_q)), **(maps or {}))
@@ -180,11 +194,16 @@ def run(cuda, *, hd, s_q, s_kv, n=2, H=2, mask=AB.MASK_NONE, mask_block=0, total
     q, k, v, do = Q.gather(), K.gather(), V.gather(), dO.gather()
     vis = AB.visible(n, s_q, s_kv, mask, mask_block, total_rows, kv_count)
     scale = hd ** -0.5
-    ref = AB.reference(q, k, v, vis.to(cuda), scale, do)
+    mult = dspec = None
+    if drop:
+        dspec = ops.Drop(torch.tensor([DROP_SEED, DROP_OFFSET], dtype=torch.int64, device=cuda), DROP_SITE, drop)
+        mult = SS.drop_mult((DROP_SEED, DROP_OFFSET, DROP_SITE, drop), range(n * H * s_q), s_kv, cuda)
+        mult = mult.view(n, H, s_q, s_kv)
+    ref = AB.reference(q, k, v, vis.to(cuda), scale, do, mult=mult)
     rows = ref["vis"].any(-1)                                  # [n, 1, s_q]: query rows that exist
     keys = ref["vis"].any(-2)                                  # [n, 1, s_kv]: keys some query sees
     kw = dict(n_seq=n, n_heads=H, head_dim=hd, s_q=s_q, s_kv=s_kv, causal=mask, scale=scale, mask_block=mask_block,
-              total_rows=total_rows)
+              total_rows=total_rows, drop=dspec)
     dev = None if kv_count is None else torch.tensor([kv_count], dtype=torch.int32, device=cuda)
 
     O = Operand(cuda, maps["o"], n, s_q, H, hd, lq, True)
@@ -193,7 +212,7 @@ def run(cuda, *, hd, s_q, s_kv, n=2, H=2, mask=AB.MASK_NONE, mask_block=0, total
     fam = lib.attn_last_path()
     assert fam == fwd_path, f"forward served by {_family_name(fam)}, expected {_family_name(fwd_path)}"
     torch.cuda.synchronize()
-    name = _family_name(fam)
+    name = _drop_name(_family_name(fam), hd, drop)
     O.check_untouched(f"{name} O")
     lse.check_untouched()
     e_o, e_lse = AB.fwd_bounds(q, k, v, scale, ref)
@@ -215,7 +234,7 @@ def run(cuda, *, hd, s_q, s_kv, n=2, H=2, mask=AB.MASK_NONE, mask_block=0, total
         fam = lib.attn_last_path()
         assert fam == bwd_path, f"{tag}backward served by {_family_name(fam)}, expected {_family_name(bwd_path)}"
         torch.cuda.synchronize()
-        bname = _family_name(fam)
+        bname = _drop_name(_family_name(fam), hd, drop, bwd=True)
         for t, w in ((dQ, "dQ"), (dK, "dK"), (dV, "dV")):
             t.check_untouched(f"{tag}{bname} {w}")
         e_dq, e_dk, e_dv = AB.bwd_bounds(q, k, v, do, scale, ref, eo, el)
@@ -391,3 +410,22 @@ def test_mma_sync_chained(cuda, kind):
     else:
         run(cuda, hd=64, n=3, s_q=80, s_kv=80, mask=AB.MASK_BLOCK, mask_block=20, fwd_path=lib.ATTN_PATH_MMA_SYNC,
             bwd_path=lib.ATTN_PATH_MMA_SYNC, chained=True, probe="block", seed=14)
+
+
+# ---------------------------------------------------------------------------------- dropout on the probabilities
+# One isolated and one chained case for each family and keep-bit path: wgmma (s_q == 1 included: no decode kernel
+# under dropout; cross attention; total_rows), the mma.sync kernels with the quad exchange (head_dim 64, 128) and with
+# one Philox call per element in the dK / dV kernel (88, 96), and the mma.sync forward with the wgmma backward.
+@pytest.mark.parametrize("hd,s_q,s_kv,n,mask,mb,total,p,chained", [
+    (64, 129, 129, 2, AB.MASK_CAUSAL, 0, 0, 0.1, False), (96, 63, 129, 2, AB.MASK_NONE, 0, 0, 0.3, False),
+    (64, 1, 70, 2, AB.MASK_NONE, 0, 0, 0.1, False), (64, 100, 100, 3, AB.MASK_CAUSAL, 0, 250, 0.3, False),
+    (80, 129, 129, 2, AB.MASK_CAUSAL, 0, 0, 0.1, True),
+    (128, 70, 200, 2, AB.MASK_NONE, 0, 0, 0.3, False), (64, 80, 80, 3, AB.MASK_BLOCK, 20, 0, 0.1, False),
+    (128, 130, 130, 2, AB.MASK_CAUSAL, 0, 0, 0.1, True),
+    (96, 96, 96, 3, AB.MASK_BLOCK, 24, 0, 0.3, False), (88, 80, 80, 3, AB.MASK_BLOCK, 8, 0, 0.3, True),
+    (80, 7, 1000, 2, AB.MASK_NONE, 0, 0, 0.3, False), (96, 15, 257, 2, AB.MASK_NONE, 0, 0, 0.1, True)])
+def test_dropout(cuda, hd, s_q, s_kv, n, mask, mb, total, p, chained):
+    run(cuda, hd=hd, n=n, s_q=s_q, s_kv=s_kv, mask=mask, mask_block=mb, total_rows=total,
+        fwd_path=fwd_family(hd, s_q, s_kv, mask, mb, total, drop=True), bwd_path=bwd_family(hd, mask, mb, drop=True),
+        chained=chained, probe="causal" if mask == AB.MASK_CAUSAL else "block" if mask == AB.MASK_BLOCK else None,
+        seed=hd + s_q + s_kv, drop=p)

@@ -35,8 +35,8 @@ def test_elementwise_dropout_mask_bit_exact(cuda, dtype):
     y = ops.dropout(x.clone(), ops.Drop(_rng(cuda), site, p), row0=1000)
     keep = philox.keep_mask(SEED, OFFSET, site, np.arange(1000, 1000 + R), C, p)
     assert torch.equal((y != 0).cpu(), torch.from_numpy(keep))
-    kept = y[y != 0].float()
-    assert torch.allclose(kept, torch.full_like(kept, 1.0 / (1.0 - p)), rtol=4e-3 if dtype == bf16 else 1e-6)
+    kept = y[y != 0]
+    assert torch.equal(kept, torch.full_like(kept, philox.scale(p)))       # 1 * scale, rounded once to the dtype
 
 
 @pytest.mark.parametrize("M,N,K,tile_n", [(300, 320, 256, 0), (512, 768, 768, 512), (1000, 2048, 2048, 512), (130, 264, 72, 128)])
