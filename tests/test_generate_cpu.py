@@ -11,15 +11,24 @@ GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 class _OracleDecoder:
-    """Decode callbacks with the same contract as DistributedGPT3._decode_callbacks, full recompute inside."""
+    """Decode callbacks over the oracle's fp32 full recompute: run_sample's step(new_tokens, first), and run_beam_search's
+    prefill / beam_step / reorder over one clip (ids [1, L]) in `rows` identical beams, with the contract of the model's
+    fixed-length decode state (beam_step ignores `live`)."""
 
-    def __init__(self, qf, sd, gcfg):
-        self.qf, self.sd, self.gcfg, self.hist = qf, sd, gcfg, None
+    def __init__(self, qf, sd, gcfg, ids=None, rows=1):
+        self.qf, self.sd, self.gcfg, self.ids, self.rows, self.hist = qf, sd, gcfg, ids, rows, None
 
     def step(self, new_tokens, first):
         self.hist = new_tokens.clone() if first else torch.cat([self.hist, new_tokens], dim=1)
         with torch.no_grad():
             return port.next_token_logits(self.qf, self.hist, self.sd, self.gcfg)
+
+    def prefill(self, group0, group_stride, clips, n):
+        assert (group0, group_stride, list(clips)) == (0, 1, [0])
+        return self.step(self.ids[:, :n].repeat(self.rows, 1), True)[:1]
+
+    def beam_step(self, new_tokens, live):
+        return self.step(new_tokens, False)
 
     def reorder(self, idx):
         self.hist = self.hist[idx]
@@ -45,15 +54,15 @@ def test_oracle_generation_matches_reference_fixture():
     assert torch.equal(greedy, fx["greedy"])
 
 
-def test_product_host_logic_with_oracle_logits():
+def test_product_loops_with_oracle_logits():
     import models.modeling_distributed_gpt3 as M
     fx, sd = _fixture()
     g, eod, qf, Q = fx["gcfg"], fx["eod"], fx["query_features"], fx["Q"]
     for i in range(fx["B"]):
-        dec = _OracleDecoder(qf[i:i + 1].repeat(fx["beam_size"], 1, 1), sd, g)
-        out = M.run_beam_search(dec.step, dec.reorder, fx["ids"][i:i + 1], int(fx["prompt_length"][i]), Q, beam_size=fx["beam_size"],
-                                num_return_gen=1, stop_token=eod, tokens_to_generate=fx["n_new"],
-                                max_position_embeddings=g["max_position_embeddings"])
+        dec = _OracleDecoder(qf[i:i + 1].repeat(fx["beam_size"], 1, 1), sd, g, fx["ids"][i:i + 1], fx["beam_size"])
+        out, = M.run_beam_search(dec.beam_step, dec.prefill, dec.reorder, fx["ids"][i:i + 1], [int(fx["prompt_length"][i])], Q,
+                                 groups=1, beam_size=fx["beam_size"], num_return_gen=1, stop_token=eod,
+                                 tokens_to_generate=fx["n_new"], max_position_embeddings=g["max_position_embeddings"])
         assert torch.equal(out.sequences, fx["beam_sequences"][i])
         assert (out.scores.reshape(-1) - fx["beam_scores"][i]).abs().max() < 1e-4
     dec = _OracleDecoder(qf, sd, g)

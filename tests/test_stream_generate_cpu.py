@@ -1,6 +1,6 @@
-"""CPU: the host logic of the streaming beam search (models.modeling_distributed_gpt3.run_beam_search_stream: a finished
-clip's slot group takes the next clip), the routing of DistributedGPT3.beam_search with B > 1, and the per-row table
-bookkeeping of ymp.engine.KVCache."""
+"""CPU: the host logic of the streaming beam search (models.modeling_distributed_gpt3.run_beam_search over a per-row
+decode state: a finished clip's slot group takes the next clip), the routing of DistributedGPT3.beam_search with B > 1,
+and the per-row table bookkeeping of ymp.engine.KVCache."""
 import os
 
 import pytest
@@ -32,22 +32,30 @@ def _clips(fx, n):
 
 
 class _OneClip:
-    """run_beam_search callbacks of one clip over the oracle's fp32 full recompute."""
+    """Fixed-length run_beam_search callbacks of one clip (ids [1, L], groups = 1) over the oracle's fp32 full
+    recompute; step ignores `live`."""
 
-    def __init__(self, qf, sd, gcfg, beam):
-        self.qf, self.sd, self.gcfg, self.beam, self.hist = qf, sd, gcfg, beam, None
+    def __init__(self, qf, sd, gcfg, ids, beam):
+        self.qf, self.sd, self.gcfg, self.ids, self.beam, self.hist = qf, sd, gcfg, ids, beam, None
 
-    def step(self, new_tokens, first):
-        self.hist = new_tokens.clone() if first else torch.cat([self.hist, new_tokens], dim=1)
+    def _logits(self):
         with torch.no_grad():
             return port.next_token_logits(self.qf.repeat(self.beam, 1, 1), self.hist, self.sd, self.gcfg)
+
+    def prefill(self, group0, group_stride, clips, n):
+        self.hist = self.ids[:, :n].repeat(self.beam, 1)
+        return self._logits()[:1]
+
+    def step(self, new_tokens, live):
+        self.hist = torch.cat([self.hist, new_tokens], dim=1)
+        return self._logits()
 
     def reorder(self, idx):
         self.hist = self.hist[idx]
 
 
 class _StreamDecoder:
-    """run_beam_search_stream callbacks over the oracle: each group keeps its own clip's token history, so a group's
+    """Per-row run_beam_search callbacks over the oracle: each group keeps its own clip's token history, so a group's
     logits are those of its clip alone.  Records the prefill calls and each group's cache length (prefix + tokens)."""
 
     def __init__(self, qf, sd, gcfg, ids, groups, beam, max_len):
@@ -97,7 +105,7 @@ class _StreamDecoder:
 
 
 @pytest.mark.parametrize("beam,groups,n_ret", [(3, 2, 2), (5, 3, 1), (3, 4, 3)])
-def test_stream_equals_per_clip(beam, groups, n_ret):
+def test_per_row_groups_equal_per_clip_search(beam, groups, n_ret):
     """More clips than groups, mixed prompt lengths: each clip's sequences and scores equal run_beam_search on that clip
     alone, and groups are refilled mid-run."""
     import models.modeling_distributed_gpt3 as M
@@ -110,11 +118,11 @@ def test_stream_equals_per_clip(beam, groups, n_ret):
               max_position_embeddings=g["max_position_embeddings"])
     final_len = min(ids.shape[1] + fx["n_new"], g["max_position_embeddings"])
     dec = _StreamDecoder(qf, sd, g, ids, groups, beam, final_len + Q)
-    res = M.run_beam_search_stream(dec.step, dec.prefill, dec.reorder, ids.clone(), plens, Q, groups=groups, **kw)
+    res = M.run_beam_search(dec.step, dec.prefill, dec.reorder, ids.clone(), plens, Q, groups=groups, **kw)
     assert len(res) == N
     for c in range(N):
-        one = _OneClip(qf[c:c + 1], sd, g, beam)
-        ref = M.run_beam_search(one.step, one.reorder, ids[c:c + 1].clone(), plens[c], Q, **kw)
+        one = _OneClip(qf[c:c + 1], sd, g, ids[c:c + 1], beam)
+        ref, = M.run_beam_search(one.step, one.prefill, one.reorder, ids[c:c + 1].clone(), [plens[c]], Q, groups=1, **kw)
         assert torch.equal(res[c].sequences, ref.sequences), c
         assert torch.equal(res[c].scores, ref.scores), c
     started = [c for _, _, cs, _ in dec.prefills for c in cs]
@@ -124,7 +132,7 @@ def test_stream_equals_per_clip(beam, groups, n_ret):
     assert any(not all(live) for live in dec.live_log) or len(dec.prefills) > len({p for *_, p in dec.prefills})
 
 
-def test_stream_refills_at_different_steps():
+def test_per_row_groups_refill_at_different_steps():
     """Clips whose captions end at different steps: groups are refilled at several distinct steps, and a group with no
     clip left is frozen (not live) for the remaining steps."""
     import models.modeling_distributed_gpt3 as M
@@ -141,9 +149,9 @@ def test_stream_refills_at_different_steps():
     def counted(new_tokens, live):
         steps_at.append(len(dec.prefills))
         return step(new_tokens, live)
-    M.run_beam_search_stream(counted, dec.prefill, dec.reorder, ids.clone(), plens, Q, beam_size=beam, num_return_gen=1,
-                             stop_token=fx["eod"], tokens_to_generate=fx["n_new"],
-                             max_position_embeddings=g["max_position_embeddings"], groups=G)
+    M.run_beam_search(counted, dec.prefill, dec.reorder, ids.clone(), plens, Q, beam_size=beam, num_return_gen=1,
+                      stop_token=fx["eod"], tokens_to_generate=fx["n_new"],
+                      max_position_embeddings=g["max_position_embeddings"], groups=G)
     assert len(set(steps_at)) >= 3           # prefills land between different decoding steps
     assert not all(dec.live_log[-1])         # the tail runs with frozen groups
 
@@ -170,31 +178,40 @@ def test_streaming_is_chosen_where_it_gains_and_runs():
     assert not M.streams_beam_search([4] * 25, 3, 64, cpu)
 
 
-def test_decoder_beam_search_routes_to_stream_in_input_order(monkeypatch):
-    """DistributedGPT3.beam_search with B > 1 where streams_beam_search says so: one streaming search over 64 // beam
-    groups (at most B), every clip's own prompt length, results in input order; otherwise the chunked search."""
+def test_decoder_beam_search_streams_on_per_row_state_in_input_order(monkeypatch):
+    """DistributedGPT3.beam_search with B > 1 where streams_beam_search says so: one streaming search over a per-row
+    decode state of 64 // beam groups (at most B), every clip's own prompt length, results in input order; otherwise
+    the chunked search over fixed-length decode states."""
     import models.modeling_distributed_gpt3 as M
     from helpers import make_model_dir
     os.environ["YMP_ALLOW_RANDOM_INIT"] = "1"
     gcfg = dict(port.GCFG_TINY)
     dec = M.DistributedGPT3(model_dir=make_model_dir(port.VCFG_TINY, gcfg))
-    calls, chunked, decided = [], [], []
+    calls, chunked, decided, made = [], [], [], {}
+    adapters = {k: getattr(M.DistributedGPT3, k) for k in ("_per_row_decoder", "_fixed_len_decoder")}
+
+    def spy(kind):
+        def build(self, *a, **k):
+            made[kind] = adapters[kind](self, *a, **k)
+            return made[kind]
+        return build
 
     def fake(step, prefill, reorder, tokens, plens, nq, **kw):
-        calls.append((tokens.shape[0], list(plens), nq, kw["groups"], kw["beam_size"]))
-        return [M.AttrDict(sequences=tokens[i:i + 1].clone(), scores=torch.tensor([float(plens[i])]))
-                for i in range(tokens.shape[0])]
-
-    def fake_chunk(step, reorder, tokens, plen, nq, **kw):
-        chunked.append((tokens.shape[0], plen))
+        if (step, prefill, reorder) == made.pop("_per_row_decoder", None):
+            calls.append((tokens.shape[0], list(plens), nq, kw["groups"], kw["beam_size"]))
+            return [M.AttrDict(sequences=tokens[i:i + 1].clone(), scores=torch.tensor([float(plens[i])]))
+                    for i in range(tokens.shape[0])]
+        assert (step, prefill, reorder) == made.pop("_fixed_len_decoder") and len(set(plens)) == 1
+        chunked.append((tokens.shape[0], plens[0]))
         return [M.AttrDict(sequences=tokens[i:i + 1].clone(), scores=torch.tensor([0.0])) for i in range(tokens.shape[0])]
     decide = M.streams_beam_search
 
     def on_device(lengths, beam, hd, device):   # the CPU tensors stand in for CUDA ones
         decided.append((list(lengths), beam, hd, torch.device(device).type))
         return decide(lengths, beam, hd, "cuda")
-    monkeypatch.setattr(M, "run_beam_search_stream", fake)
-    monkeypatch.setattr(M, "run_beam_search_batched", fake_chunk)
+    for k in adapters:
+        monkeypatch.setattr(M.DistributedGPT3, k, spy(k))
+    monkeypatch.setattr(M, "run_beam_search", fake)
     monkeypatch.setattr(M, "streams_beam_search", on_device)
     B, beam, Q = 25, 3, 4
     ids = torch.arange(B * 6).view(B, 6)

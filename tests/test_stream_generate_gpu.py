@@ -242,17 +242,21 @@ def _generate_both(model, video, text, beam):
     """(model.generate's list on the streaming path, its AttrDicts, the per-clip beam searches' AttrDicts)."""
     import models.modeling_distributed_gpt3 as M
     dec = model.text_decoder
-    orig, calls = M.run_beam_search_stream, []
+    orig, calls, got = M.DistributedGPT3._per_row_decoder, [], []
 
-    def counted(*a, **k):
-        out = orig(*a, **k)
-        calls.append(out)
-        return out
-    M.run_beam_search_stream = counted
+    def counted(self, *a, **k):
+        calls.append(a)
+        return orig(self, *a, **k)
+    M.DistributedGPT3._per_row_decoder = counted
     bs = dec.beam_search
-    dec.beam_search = lambda *a, **k: bs(*a, **dict(k, beam_size=beam))
+
+    def beam_search(*a, **k):
+        got.append(bs(*a, **dict(k, beam_size=beam)))
+        return got[-1]
+    dec.beam_search = beam_search
     try:
         res = model.generate(video, text)
+        stream = got[0]
         eos = dec.config.eod_id
         per = []
         with torch.no_grad():
@@ -261,10 +265,10 @@ def _generate_both(model, video, text, beam):
                 per.append(dec.generate(text.input_ids[i:i + 1], query_embeds=qf[i:i + 1], termination_id=eos,
                                         do_sample=False, prompt_length=text.attention_mask.sum(-1)[i] - 1))
     finally:
-        M.run_beam_search_stream = orig
+        M.DistributedGPT3._per_row_decoder = orig
         del dec.beam_search
     assert len(calls) == 1
-    return res, calls[0], per
+    return res, stream, per
 
 
 def _check(res, stream, per, B):
@@ -282,7 +286,7 @@ def _mixed_text(M, ids, dev, plens):
     return M.BatchEncoding(dict(input_ids=ids.to(dev), attention_mask=att.to(dev)))
 
 
-def test_caption_generate_stream_equals_per_clip_tiny(cuda):
+def test_caption_generate_per_row_state_equals_per_clip_tiny(cuda):
     """30 clips at beam 5 on the tiny fixture (its weights make beams finish early), prompt lengths 3 .. 6."""
     import models.modeling_distributed_gpt3 as M
     fx, model = _tiny(cuda)
@@ -296,7 +300,7 @@ def test_caption_generate_stream_equals_per_clip_tiny(cuda):
 
 
 @pytest.mark.parametrize("width", ["1.3B", "2.7B"])
-def test_caption_generate_stream_equals_per_clip_wide(cuda, width):
+def test_caption_generate_per_row_state_equals_per_clip_wide(cuda, width):
     """2-layer decoders at the 1.3B / 2.7B widths, 30 clips at beam 5 (12 groups: 18 refills), mixed prompt lengths,
     the stop token's embedding row scaled so that captions end at varying steps."""
     import models.modeling_distributed_gpt3 as M

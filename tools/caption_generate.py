@@ -11,8 +11,8 @@ each, every call ending in a device synchronise; the median of --rounds calls is
   batched_moving - the chunked batched search with the beams permuted by moving the cached K/V rows (KVCache.reorder);
   batched        - the chunked batched search (chunks of 64 // beam clips per decode step, each running until its
                    slowest clip is done), beams permuted through the cache's row table (KVCache.reindex);
-  stream         - model.generate(video, text): the streaming search (run_beam_search_stream), a finished clip's
-                   beam slots take the next clip while the others keep decoding.
+  stream         - model.generate(video, text): the streaming search (run_beam_search over the per-row decode state),
+                   a finished clip's beam slots take the next clip while the others keep decoding.
 Two workloads: `full` (random weights almost never emit the stop token, so every caption runs all 100 tokens: the
 stream arm must do the batched arm's steps) and `varied` (the stop token's row of the tied word embedding scaled by
 --stop-scale, so captions end at varying steps: where the stream arm saves steps).
@@ -25,6 +25,7 @@ events over many launches, weights rotated through copies larger than L2): micro
 SXM data sheet's 3.35 TB/s.  --counts prints the weight and KV-cache bytes counted from shapes, without a GPU.
 """
 import argparse
+import gc
 import json
 import os
 import statistics
@@ -156,13 +157,15 @@ def inputs(vis, name, B):
 
 
 def chunked_generate(model, video, text, moving=False):
-    """model.generate through the chunked batched beam search (DistributedGPT3._beam_search_batched)."""
-    dec = model.text_decoder
-    dec._beam_search_stream = dec._beam_search_batched
+    """model.generate through the chunked batched beam search: streams_beam_search answers no, so beam_search runs
+    its chunks over fixed-length decode states."""
+    import models.modeling_distributed_gpt3 as G
+    streams = G.streams_beam_search
+    G.streams_beam_search = lambda *a: False
     try:
         return moving_generate(model, video, text) if moving else model.generate(video, text)
     finally:
-        del dec._beam_search_stream
+        G.streams_beam_search = streams
 
 
 def run(model, vis, name, rounds, workload="full", stop_scale=4.0):
@@ -215,6 +218,7 @@ def run(model, vis, name, rounds, workload="full", stop_scale=4.0):
             # the decoder pools one KV cache + captured step per shape on the model: every arm allocates (and counts in
             # its peak) and captures its own, rather than one arm inheriting the cache of the arm before it
             dec.__dict__.pop("_decode_pool", None)
+            gc.collect()   # a dropped cache and its captured step reference each other: free them before the next arm
             torch.cuda.synchronize()
             base = torch.cuda.memory_allocated()
             torch.cuda.reset_peak_memory_stats()

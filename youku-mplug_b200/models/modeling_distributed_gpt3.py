@@ -410,131 +410,6 @@ def run_sample(step, tokens, lengths, n_query, *, tokens_to_generate, eod_id, ma
     return tokens[:, :ctx + n_query + 1]
 
 
-def run_beam_search(step, reorder, tokens, prompt_length, n_query, *, beam_size, num_return_gen, stop_token,
-                    tokens_to_generate, max_position_embeddings):
-    """DistributedGPT3.beam_search's loop (:1743-1875), batch size 1, over a decode callback.
-    step(new_tokens [beam, n], first) -> logits [beam, V]; reorder(idx) permutes the callback's KV cache."""
-    assert tokens.size(0) == 1
-    dev = tokens.device
-    tokens = torch.cat((tokens, torch.full((1, tokens_to_generate), stop_token, dtype=torch.long, device=dev)), dim=-1)
-    final_len = min(tokens.size(1), max_position_embeddings)
-    if prompt_length >= final_len:
-        raise ValueError('context length + tokens_to_generate too large')
-    pool = BeamHypotheses(beam_size)
-    scores = torch.zeros(beam_size, 1, dtype=torch.float32, device=dev)
-    tokens = tokens.repeat(beam_size, 1)
-    done = False
-    prev = 0
-    ctx = prompt_length
-    for ctx in range(prompt_length, final_len):
-        logits = step(tokens[:, prev:ctx], ctx == prompt_length)
-        vocab = logits.size(-1)
-        cand = torch.log_softmax(logits.float(), dim=-1) + scores
-        flat = cand[0] if ctx == prompt_length else cand.view(-1)  # identical beams at the first step
-        ranked_scores, ranked = torch.sort(flat, descending=True)
-        ranked, ranked_scores = ranked[:2 * beam_size], ranked_scores[:2 * beam_size]
-        beam_of, word_of = torch.div(ranked, vocab, rounding_mode='floor').tolist(), (ranked % vocab).tolist()
-        survivors = []
-        for rank, (word, beam) in enumerate(zip(word_of, beam_of)):
-            if word == stop_token:
-                if rank >= beam_size:  # a finished hypothesis outside the top beam_size candidates is dropped
-                    continue
-                pool.add(tokens[beam].clone(), ranked_scores[rank], ctx + 1 - prompt_length)
-            else:
-                survivors.append((word, ranked_scores[rank], beam))
-            if len(survivors) == beam_size:
-                break
-        if pool.is_done(ranked_scores.max().item(), ctx + 1 - prompt_length):
-            done = True
-            break
-        keep = torch.tensor([b for _, _, b in survivors], dtype=torch.long, device=dev)
-        tokens = tokens[keep, :]
-        tokens[:, ctx] = torch.tensor([w for w, _, _ in survivors], dtype=torch.long, device=dev)
-        scores = torch.stack([sc for _, sc, _ in survivors]).reshape(-1, 1).float()
-        reorder(keep)
-        prev = ctx
-    if not done:
-        for b in range(beam_size):
-            pool.add(tokens[b].clone(), scores[b], ctx + 1 - prompt_length)
-    best = sorted(pool.beams, key=lambda x: float(x[0]), reverse=True)[:min(num_return_gen, len(pool.beams))]
-    return AttrDict(sequences=torch.stack([h for _, h, _ in best], dim=0),
-                    scores=torch.stack([torch.as_tensor(sc, device=dev).reshape(-1)[0] for sc, _, _ in best], dim=0))
-
-def run_beam_search_batched(step, reorder, tokens, prompt_length, n_query, *, beam_size, num_return_gen, stop_token,
-                            tokens_to_generate, max_position_embeddings):
-    """run_beam_search for B clips at once (tokens [B, L], one prompt length) over one decode callback with B*beam rows:
-    clip c owns rows c*beam .. c*beam + beam - 1.  Each clip keeps its own ranking, BeamHypotheses and stopping rule,
-    so its result equals run_beam_search on that clip alone.  A step sorts every clip's candidates in one device sort
-    and copies the top 2*beam of all clips to the host in one transfer.  Rows of a finished clip keep stepping and are
-    never read; the loop ends when every clip is done or the length limit is reached.
-    step(new_tokens [B*beam, n], first) -> logits [B*beam, V] (the first call may return one row per clip, [B, V]);
-    reorder(idx [B*beam]) permutes the callback's KV cache.  Returns a list of B AttrDict(sequences, scores)."""
-    B, dev = tokens.size(0), tokens.device
-    tokens = torch.cat((tokens, torch.full((B, tokens_to_generate), stop_token, dtype=torch.long, device=dev)), dim=-1)
-    final_len = min(tokens.size(1), max_position_embeddings)
-    if prompt_length >= final_len:
-        raise ValueError('context length + tokens_to_generate too large')
-    pools = [BeamHypotheses(beam_size) for _ in range(B)]
-    done = [False] * B
-    scores = torch.zeros(B * beam_size, 1, dtype=torch.float32, device=dev)
-    tokens = tokens.repeat_interleave(beam_size, dim=0)
-    top = 2 * beam_size
-    prev = 0
-    ctx = prompt_length
-    for ctx in range(prompt_length, final_len):
-        first = ctx == prompt_length
-        logits = step(tokens[:, prev:ctx], first)
-        vocab = logits.size(-1)
-        if first:  # identical beams: only the first beam of every clip is ranked
-            cand = torch.log_softmax(logits.view(B, -1, vocab)[:, 0].float(), dim=-1) + scores.view(B, beam_size)[:, :1]
-        else:
-            cand = (torch.log_softmax(logits.float(), dim=-1) + scores).view(B, -1)
-        ranked_scores, ranked = torch.sort(cand, dim=-1, descending=True)
-        ranked, ranked_scores = ranked[:, :top], ranked_scores[:, :top]
-        host = torch.cat((ranked.double(), ranked_scores.double()), dim=1).cpu()   # indices < 2**53 and fp32 are exact
-        idx = host[:, :top].long()
-        beam_of, word_of = torch.div(idx, vocab, rounding_mode='floor').tolist(), (idx % vocab).tolist()
-        best_score = host[:, top:].max(dim=1).values.tolist()
-        keep, words, picked = [], [], []
-        for c in range(B):
-            base = c * beam_size
-            if not done[c]:
-                survivors = []
-                for rank, (word, beam) in enumerate(zip(word_of[c], beam_of[c])):
-                    if word == stop_token:
-                        if rank >= beam_size:  # a finished hypothesis outside the top beam_size candidates is dropped
-                            continue
-                        pools[c].add(tokens[base + beam].clone(), ranked_scores[c, rank], ctx + 1 - prompt_length)
-                    else:
-                        survivors.append((word, rank, beam))
-                    if len(survivors) == beam_size:
-                        break
-                done[c] = pools[c].is_done(best_score[c], ctx + 1 - prompt_length)
-            if done[c]:  # rows that are never read again: keep them in place
-                survivors = [(stop_token, b, b) for b in range(beam_size)]
-            keep += [base + b for _, _, b in survivors]
-            words += [w for w, _, _ in survivors]
-            picked += [c * top + r for _, r, _ in survivors]
-        if all(done):
-            break
-        keep = torch.tensor(keep, dtype=torch.long, device=dev)
-        tokens = tokens[keep, :]
-        tokens[:, ctx] = torch.tensor(words, dtype=torch.long, device=dev)
-        scores = ranked_scores.reshape(-1)[torch.tensor(picked, dtype=torch.long, device=dev)].reshape(-1, 1).float()
-        reorder(keep)
-        prev = ctx
-    out = []
-    for c in range(B):
-        pool, base = pools[c], c * beam_size
-        if not done[c]:
-            for b in range(beam_size):
-                pool.add(tokens[base + b].clone(), scores[base + b], ctx + 1 - prompt_length)
-        best = sorted(pool.beams, key=lambda x: float(x[0]), reverse=True)[:min(num_return_gen, len(pool.beams))]
-        out.append(AttrDict(sequences=torch.stack([h for _, h, _ in best], dim=0),
-                            scores=torch.stack([torch.as_tensor(sc, device=dev).reshape(-1)[0] for sc, _, _ in best], dim=0)))
-    return out
-
-
 def _prefill_runs(groups, plens):
     """Refills of one step that can share a prefill launch: groups whose clips have one prompt length and whose slots
     are equally spaced.  groups ascending; returns [(prompt_length, first_group, group_stride, [groups])]."""
@@ -554,22 +429,24 @@ def _prefill_runs(groups, plens):
     return [(p, r[0], r[1] - r[0] if len(r) > 1 else 1, r) for p, r in runs]
 
 
-def run_beam_search_stream(step, prefill, reorder, tokens, prompt_lengths, n_query, *, beam_size, num_return_gen, stop_token,
-                           tokens_to_generate, max_position_embeddings, groups):
-    """run_beam_search for N clips (tokens [N, L], one prompt length per clip) over `groups` slot groups of beam_size
-    rows each (group g owns rows g*beam .. g*beam + beam - 1), filled with clips in input order.  Each clip keeps its
-    own context length, ranking, BeamHypotheses and stopping rule, so its result equals run_beam_search on that clip
-    alone.  When a group's clip is done (its pool is done or its own last position is reached) the next waiting clip is
-    prefilled into that group while the other groups keep decoding; a group with no successor is frozen.
-      step(new_tokens [groups*beam, 1], live [groups] bools) -> logits [groups*beam, V] of one single-token step of the
-        live groups (a frozen group's rows are not read and must not advance);
+def run_beam_search(step, prefill, reorder, tokens, prompt_lengths, n_query, *, groups, beam_size, num_return_gen,
+                    stop_token, tokens_to_generate, max_position_embeddings):
+    """DistributedGPT3.beam_search's loop (:1743-1875) for N clips (tokens [N, L], one prompt length per clip) over a
+    decode state of `groups` slot groups of beam_size rows each (group g owns rows g*beam .. g*beam + beam - 1), filled
+    with clips in input order.  Each clip keeps its own context length, ranking, BeamHypotheses and stopping rule, so
+    its result does not depend on the other clips or on `groups`.  When a group's clip is done (its pool is done or its
+    own last position is reached) the next waiting clip is prefilled into that group while the other groups keep
+    decoding; a group with no successor is frozen.
       prefill(first_group, group_stride, clips, n) -> logits [len(clips), V]: clip clips[i]'s [prefix | tokens[:n]] into
         group first_group + i * group_stride (refills of one step with one prompt length and equally spaced groups
         share a call);
+      step(new_tokens [groups*beam, 1], live [groups] bools) -> logits [groups*beam, V] of one single-token step (the
+        rows of a group that is not live are never read);
       reorder(idx [groups*beam]) permutes the decode state's rows (within groups).
-    A decoding step ranks every live group's candidates in one device sort and copies them to the host in one
-    transfer; the step that starts clips ranks their first candidates in one more sort and transfer.  Returns a list of
-    N AttrDict(sequences, scores) in input order."""
+    A decoding step ranks every live group's candidates in one device sort, copies them to the host in one transfer and
+    applies the survivors with one host-to-device copy; the step that starts clips ranks their first candidates (one
+    beam per clip: its beams are identical) in one more of each.  Returns a list of N AttrDict(sequences, scores) in
+    input order."""
     N, dev = tokens.size(0), tokens.device
     plens = [int(p) for p in prompt_lengths]
     assert len(plens) == N
@@ -577,13 +454,14 @@ def run_beam_search_stream(step, prefill, reorder, tokens, prompt_lengths, n_que
     final_len = min(tokens.size(1), max_position_embeddings)
     if max(plens) >= final_len:
         raise ValueError('context length + tokens_to_generate too large')
-    G, beam, top = groups, beam_size, 2 * beam_size
+    G, beam, top, width = groups, beam_size, 2 * beam_size, tokens.size(1)
     clip_of = [None] * G        # clip decoding in group g (None: free / frozen)
-    ctx = [0] * G               # the group's next context position (run_beam_search's ctx)
+    ctx = [0] * G               # the group's next context position
     pools = [None] * G
     out = [None] * N
-    rows = torch.full((G * beam, tokens.size(1)), stop_token, dtype=torch.long, device=dev)
+    rows = torch.full((G * beam, width), stop_token, dtype=torch.long, device=dev)
     scores = torch.zeros(G * beam, 1, dtype=torch.float32, device=dev)
+    new = torch.full((G * beam, 1), stop_token, dtype=torch.long, device=dev)   # each row's next input token
     waiting = list(range(N))
 
     def finish(g, add):
@@ -596,17 +474,20 @@ def run_beam_search_stream(step, prefill, reorder, tokens, prompt_lengths, n_que
                           scores=torch.stack([torch.as_tensor(sc, device=dev).reshape(-1)[0] for sc, _, _ in best], dim=0))
         clip_of[g] = None
 
-    def rank(gs, cand, first):
-        """Rank groups gs from cand [len(gs), width] (one sort, one transfer), apply the survivors to rows / scores,
-        advance or finish each group.  Returns keep (row -> source row) for the reorder."""
+    def rank(gs, cand, vocab, gather):
+        """Rank the clips of groups gs from cand [len(gs), width] (one sort, one transfer), write the survivors of the
+        groups that go on into rows / scores / new (one transfer), advance or finish each group.  gather: the survivors
+        may come from any beam of their group (a decoding step; otherwise they all come from the group's identical
+        beams): every row is gathered from its source row first, and that index (identity for the other groups) is
+        returned for the reorder."""
+        nonlocal rows
         ranked_scores, ranked = torch.sort(cand, dim=-1, descending=True)
         ranked, ranked_scores = ranked[:, :top], ranked_scores[:, :top]
         host = torch.cat((ranked.double(), ranked_scores.double()), dim=1).cpu()   # indices < 2**53 and fp32 are exact
-        vocab = cand.size(1) if first else cand.size(1) // beam
         idx = host[:, :top].long()
         beam_of, word_of = torch.div(idx, vocab, rounding_mode='floor').tolist(), (idx % vocab).tolist()
         best_score = host[:, top:].max(dim=1).values.tolist()
-        keep, at, words, picked, ended = [], [], [], [], []
+        keep, going, words, picked = list(range(G * beam)), [], [], []
         for i, g in enumerate(gs):
             c, base = clip_of[g], g * beam
             survivors = []
@@ -620,26 +501,29 @@ def run_beam_search_stream(step, prefill, reorder, tokens, prompt_lengths, n_que
                 if len(survivors) == beam:
                     break
             if pools[g].is_done(best_score[i], ctx[g] + 1 - plens[c]):
-                ended.append((g, False))
+                finish(g, False)
                 continue
-            keep += [base + b for _, _, b in survivors]
-            at += [(base + j, ctx[g]) for j in range(beam)]
+            going.append(g)
+            keep[base:base + beam] = [base + b for _, _, b in survivors]
             words += [w for w, _, _ in survivors]
             picked += [i * top + r for _, r, _ in survivors]
+        if not going:
+            return None
+        dst = [g * beam + j for g in going for j in range(beam)]
+        at = [r * width + ctx[r // beam] for r in dst]
+        head = keep if gather else []
+        keep, dst, words, picked, at = torch.tensor(head + dst + words + picked + at, dtype=torch.long,
+                                                    device=dev).split([len(head)] + [len(dst)] * 4)
+        if gather:
+            rows = rows.index_select(0, keep)
+        rows.view(-1).index_copy_(0, at, words)   # not put_: it fails under torch.use_deterministic_algorithms
+        scores.index_copy_(0, dst, ranked_scores.take(picked).view(-1, 1))
+        new.index_copy_(0, dst, words.view(-1, 1))
+        for g in going:
             if ctx[g] + 1 == final_len:
-                ended.append((g, True))
-        perm = torch.arange(G * beam, device=dev)
-        if keep:
-            dst = torch.tensor([r for r, _ in at], dtype=torch.long, device=dev)
-            perm[dst] = torch.tensor(keep, dtype=torch.long, device=dev)
-            rows[dst] = rows[perm[dst]]
-            rows[dst, torch.tensor([p for _, p in at], dtype=torch.long, device=dev)] = torch.tensor(words, dtype=torch.long, device=dev)
-            scores[dst] = ranked_scores.reshape(-1)[torch.tensor(picked, dtype=torch.long, device=dev)].reshape(-1, 1).float()
-        for g, add in ended:
-            finish(g, add)
-        for g in gs:
+                finish(g, True)
             ctx[g] += 1
-        return perm
+        return keep if gather else None
 
     def refill(free):
         """Start waiting clips in the free groups (ascending) and rank their first candidates; repeat for clips that
@@ -650,37 +534,35 @@ def run_beam_search_stream(step, prefill, reorder, tokens, prompt_lengths, n_que
             for g, c in zip(gs, cs):
                 clip_of[g], ctx[g], pools[g] = c, plens[c], BeamHypotheses(beam)
                 rows[g * beam:(g + 1) * beam] = tokens[c]
-                scores[g * beam:(g + 1) * beam] = 0
             first = [None] * len(gs)
             for p, g0, gstride, run in _prefill_runs(gs, [plens[c] for c in cs]):
                 lg = prefill(g0, gstride, [clip_of[g] for g in run], p)
                 for j, g in enumerate(run):
                     first[gs.index(g)] = lg[j:j + 1]
             lg = torch.cat(first)
-            # identical beams: only the first beam of every clip is ranked
-            rank(gs, torch.log_softmax(lg.float(), dim=-1) + scores.view(G, beam)[gs, :1], True)
+            rank(gs, torch.log_softmax(lg.float(), dim=-1), lg.size(1), False)
             free = [g for g in gs if clip_of[g] is None]
 
     refill(list(range(G)))
     while any(c is not None for c in clip_of):
         live = [c is not None for c in clip_of]
-        new = rows.gather(1, torch.tensor([max(ctx[g] - 1, 0) for g in range(G) for _ in range(beam)],
-                                          dtype=torch.long, device=dev).view(-1, 1))
         logits = step(new, live)
         gs = [g for g in range(G) if live[g]]
         cand = (torch.log_softmax(logits.float(), dim=-1) + scores).view(G, -1)
-        perm = rank(gs, cand[gs] if len(gs) < G else cand, False)
-        reorder(perm)
+        keep = rank(gs, cand if len(gs) == G else cand[gs], logits.size(-1), True)
+        if keep is not None:
+            reorder(keep)
         refill([g for g in gs if clip_of[g] is None])
     return out
 
 
 def streams_beam_search(prompt_lengths, beam_size, head_dim, device):
-    """Does DistributedGPT3.beam_search run these clips as one streaming search (run_beam_search_stream)?  Only where
-    it gains and its per-sequence decoding step exists: the clips need more than one chunk of the batched search (more
-    than 64 // beam_size clips, or several prompt lengths; one chunk has nothing to refill, and its step does less host
-    work), the decoder's head_dim has the per-sequence decode attention (64 / 80 / 96) and the tokens are on a CUDA
-    device, where those kernels run.  Otherwise the batched search over chunks, as before the streaming search."""
+    """Does DistributedGPT3.beam_search run these clips as one streaming search (run_beam_search over the per-row decode
+    state, a finished clip's group refilled)?  Only where it gains and its per-sequence decoding step exists: the clips
+    need more than one chunk of the batched search (more than 64 // beam_size clips, or several prompt lengths; one
+    chunk has nothing to refill), the decoder's head_dim has the per-sequence decode attention (64 / 80 / 96) and the
+    tokens are on a CUDA device, where those kernels run.  Otherwise one search per chunk over the fixed-length decode
+    state."""
     from ymp import ops
     if torch.device(device).type != "cuda" or head_dim not in (64, 80, 96):
         return False
@@ -864,14 +746,7 @@ class DistributedGPT3(nn.Module):
             return AttrDict(logits=logits.view(B, 1, -1), loss=None, losses=None, last_hidden_state=hid.view(B, 1, H))
         keys, params = self._param_list()
         if ip.cache is None:
-            # one cache (and one captured token step) per (batch, length) is kept on the model and reused by later
-            # sample() / beam_search() calls: caption evaluation decodes thousands of clips with the same shape
-            key = (ip.max_batch_size, ip.max_sequence_len, str(input_embeds.device))
-            pool = self.__dict__.setdefault("_decode_pool", {})
-            if key not in pool:
-                pool.clear()   # keep one shape resident (a 1.3B cache at beam 5 x 400 positions is 0.6 GB)
-                pool[key] = engine.KVCache(self.config.engine_cfg(), ip.max_batch_size, ip.max_sequence_len, input_embeds.device)
-            ip.cache = pool[key]
+            ip.cache = self._resident_cache(ip.max_batch_size, ip.max_sequence_len, input_embeds.device, per_row=False)
             ip.cache.reset()
             ip.key_value_memory_dict = {i + 1: t for i, t in enumerate(ip.cache.qkv)}
         off = ip.sequence_len_offset
@@ -879,16 +754,7 @@ class DistributedGPT3(nn.Module):
         assert off == ip.cache.len and B * stride == ip.cache.B
         if n == 1 and off > 0 and B <= (ops.SKINNY_WIDE_MAX_ROWS if ip.wide_step else ops.SKINNY_MAX_ROWS):
             # single-token step: skinny GEMMs + device-side cache length, replayed as one CUDA graph
-            sig = (params[0].data_ptr(), params[-1].data_ptr(), sum(p._version for p in params))
-            ts = ip.cache.token
-            if ts is None or ts.sig != sig:
-                # weights the graph may hold raw pointers to: bf16 parameters (used in place) and frozen fp32 ones
-                # (their bf16 copy is cached until the version changes); trainable fp32 ones are re-cast every step
-                static = all(p.dtype == torch.bfloat16 or not p.requires_grad for p in params)
-                ts = ip.cache.token = engine.TokenStep(ip.cache, {k: YF.as_bf16(p) for k, p in zip(keys, params)},
-                                                       input_embeds.dtype, sig, static)
-            elif not ts.static:
-                ts.W = {k: YF.as_bf16(p) for k, p in zip(keys, params)}
+            ts = self._token_step(ip.cache, keys, params, input_embeds.dtype, per_row=False)
             if ts.static:
                 ip.token_step = ts
             hid, logits = ts.run(input_embeds.reshape(B, H))
@@ -901,6 +767,34 @@ class DistributedGPT3(nn.Module):
         ip.sequence_len_offset += n  # tokens.size(1) + query_embeds.size(1) of the reference
         return AttrDict(logits=logits.view(B, 1, -1), loss=None, losses=None, last_hidden_state=hid.view(B, 1, H))
 
+    def _resident_cache(self, batch, max_len, device, per_row):
+        """The KV cache of `batch` sequences x max_len positions for one length mode (per_row: ymp.engine.KVCache's
+        per-sequence lengths, else its one scalar length).  It is kept on the model with its captured token step and
+        reused by later sample() / beam_search() calls: caption evaluation decodes thousands of clips with the same
+        shape.  One shape stays resident (a 1.3B cache at beam 5 x 400 positions is 0.6 GB)."""
+        from ymp import engine
+        key = (batch, max_len, str(device), per_row)
+        pool = self.__dict__.setdefault("_decode_pool", {})
+        if key not in pool:
+            pool.clear()
+            pool[key] = engine.KVCache(self.config.engine_cfg(), batch, max_len, device)
+        return pool[key]
+
+    def _token_step(self, cache, keys, params, emb_dtype, per_row):
+        """cache's single-token step (ymp.engine.TokenStep) for the weights `params`: rebuilt when they moved or changed
+        version.  The graph may hold raw pointers to bf16 parameters (used in place) and frozen fp32 ones (their bf16
+        copy is cached until the version changes); trainable fp32 ones are re-cast on every call."""
+        from ymp import engine
+        sig = (params[0].data_ptr(), params[-1].data_ptr(), sum(p._version for p in params))
+        ts = cache.token
+        if ts is None or ts.sig != sig or ts.per_row != per_row:
+            static = all(p.dtype == torch.bfloat16 or not p.requires_grad for p in params)
+            ts = cache.token = engine.TokenStep(cache, {k: YF.as_bf16(p) for k, p in zip(keys, params)}, emb_dtype, sig,
+                                                static, per_row=per_row)
+        elif not ts.static:
+            ts.W = {k: YF.as_bf16(p) for k, p in zip(keys, params)}
+        return ts
+
     def _decode_callbacks(self, query_embeds):
         def step(new_tokens, first):
             out = self(tokens=new_tokens, query_embeds=query_embeds if first else None)
@@ -911,6 +805,58 @@ class DistributedGPT3(nn.Module):
             # row (swap_key_value_dict keeps the reference's physical permutation)
             self.inference_params.cache.reindex(idx)
         return step, reorder
+
+    def _fixed_len_decoder(self, tokens, query_embeds, groups, beam_size, max_len, wide):
+        """run_beam_search's decode state over a KV cache with one length for all rows (InferenceParams + _decode,
+        through _decode_callbacks): the clips tokens [groups, L] start together at one prompt length and step together;
+        a finished clip's rows keep stepping unread.  wide: the chunked search's form (the prefill runs each clip's
+        [prefix | prompt] once, into its first beam slot, and the cache's row table points the clip's other beams at it;
+        single-token steps of up to 64 rows take the captured step); otherwise one clip whose prefill runs beam_size
+        identical rows.  Returns (step, prefill, reorder)."""
+        assert wide or groups == 1
+        ip = self.inference_params = InferenceParams(groups * beam_size, max_len)
+        ip.wide_step, ip.prefill_stride = wide, beam_size if wide else 1
+        qe = query_embeds if wide or query_embeds is None else query_embeds.repeat(beam_size, 1, 1)
+        step, reorder = self._decode_callbacks(qe)
+
+        def prefill(group0, group_stride, clips, n):
+            assert ip.sequence_len_offset == 0, "the fixed-length decode state is prefilled once"
+            assert group0 == 0 and group_stride == 1 and list(clips) == list(range(groups))
+            if wide:
+                return step(tokens[:, :n], True)
+            return step(tokens[:, :n].repeat(beam_size, 1), True)[:1]
+        return (lambda new_tokens, live: step(new_tokens, False)), prefill, reorder
+
+    def _per_row_decoder(self, tokens, query_embeds, groups, beam_size, max_len):
+        """run_beam_search's decode state over a KV cache in per-row mode: each group at its own length, the
+        single-token steps replay one captured per-row TokenStep that advances the live groups' rows only, and a
+        finished clip's group is refilled by a group prefill into its first slot.  Returns (step, prefill, reorder)."""
+        from ymp import engine, ops
+        rows, dev = groups * beam_size, tokens.device
+        nq = 0 if query_embeds is None else query_embeds.size(1)
+        self.inference_params = None
+        cache = self._resident_cache(rows, max_len, dev, per_row=True)
+        cache.reset_rows()
+        emb = self.dist_model.language_model.embedding.word_embeddings
+        ts = self._token_step(cache, *self._param_list(), emb.weight.dtype, per_row=True)
+        W = ts.W
+        wemb, pos = W[engine.GPT + "embedding.word_embeddings.weight"], W[engine.GPT + "embedding.position_embeddings.weight"]
+
+        def step(new_tokens, live):
+            cache.set_live([x for x in live for _ in range(beam_size)])
+            _, logits = ts.run(emb(new_tokens).reshape(rows, -1))
+            return logits
+
+        def prefill(group0, group_stride, clips, n):
+            sel = torch.tensor(clips, dtype=torch.long, device=dev)
+            x = emb(tokens[sel, :n])
+            if query_embeds is not None:
+                x = torch.cat([query_embeds[sel].to(x.dtype), x], dim=1)
+            m = n + nq
+            x = (x.float() + pos[:m][None].float()).reshape(len(clips) * m, -1).contiguous()
+            hid = cache.prefill_groups(W, x, m, group0, group_stride, beam_size)
+            return ops.gemm(hid, wemb).float()
+        return step, prefill, cache.reindex_rows
 
     @torch.no_grad()
     def sample(self, tokens, query_embeds=None, temperature=1.0, use_eod_token_for_early_termination=True,
@@ -931,116 +877,61 @@ class DistributedGPT3(nn.Module):
 
     @torch.no_grad()
     def beam_search(self, tokens, query_embeds=None, beam_size=5, num_return_gen=1, stop_token=None, **kwargs):
-        """Beam search (:1743-1875).  One sample (tokens [1, L]): Dict(sequences [n, len], scores [n]).
-        B > 1 samples (prompt_length an int or a [B] tensor): a list of B such Dicts, each equal to the call for that
-        sample alone.  Samples that need more than one chunk of the batched search run one streaming beam search
-        (run_beam_search_stream: a finished sample's beam slots take the next sample) where streams_beam_search says so;
-        otherwise batched beam searches over chunks of samples that share a prompt length."""
+        """Beam search (:1743-1875) through run_beam_search.  One sample (tokens [1, L]): Dict(sequences [n, len],
+        scores [n]), over the fixed-length decode state.  B > 1 samples (prompt_length an int or a [B] tensor): a list
+        of B such Dicts, each equal to the call for that sample alone.  Samples that need more than one chunk run one
+        streaming search over the per-row decode state (_beam_search_stream: a finished sample's beam slots take the
+        next sample) where streams_beam_search says so; otherwise one search per chunk of samples that share a prompt
+        length (_beam_search_batched)."""
         cfg = self.config
         prompt_length = kwargs.pop('prompt_length', tokens.size(1))
         if stop_token is None:
             stop_token = cfg.eod_id
         if tokens.size(0) > 1:
-            lengths = torch.as_tensor(prompt_length).reshape(-1).tolist()
-            lengths = lengths * tokens.size(0) if len(lengths) == 1 else lengths
+            lengths, _, _, _ = self._beam_search_args(tokens, query_embeds, prompt_length, beam_size, num_return_gen, stop_token)
             stream = streams_beam_search(lengths, beam_size, cfg.hidden_size // cfg.num_attention_heads, tokens.device)
             search = self._beam_search_stream if stream else self._beam_search_batched
             return search(tokens, query_embeds, beam_size, num_return_gen, stop_token, prompt_length)
-        prompt_length = int(prompt_length)
+        lengths, nq, max_len, kw = self._beam_search_args(tokens, query_embeds, prompt_length, beam_size, num_return_gen,
+                                                          stop_token)
+        dec = self._fixed_len_decoder(tokens, query_embeds, 1, beam_size, max_len, wide=False)
+        return run_beam_search(*dec, tokens, lengths, nq, groups=1, **kw)[0]
+
+    def _beam_search_args(self, tokens, query_embeds, prompt_length, beam_size, num_return_gen, stop_token):
+        """(one prompt length per sample, prefix length, KV-cache length, run_beam_search's keyword arguments)."""
+        cfg = self.config
+        lengths = torch.as_tensor(prompt_length).reshape(-1).tolist()
+        lengths = lengths * tokens.size(0) if len(lengths) == 1 else lengths
+        assert len(lengths) == tokens.size(0)
         nq = 0 if query_embeds is None else query_embeds.size(1)
-        final_len = min(tokens.size(1) + cfg.tokens_to_generate, cfg.max_position_embeddings)
-        self.inference_params = InferenceParams(beam_size, final_len + nq)
-        qe = None if query_embeds is None else query_embeds.repeat(beam_size, 1, 1)
-        step, reorder = self._decode_callbacks(qe)
-        return run_beam_search(step, reorder, tokens, prompt_length, nq, beam_size=beam_size, num_return_gen=num_return_gen,
-                               stop_token=stop_token, tokens_to_generate=cfg.tokens_to_generate,
-                               max_position_embeddings=cfg.max_position_embeddings)
+        max_len = min(tokens.size(1) + cfg.tokens_to_generate, cfg.max_position_embeddings) + nq
+        return lengths, nq, max_len, dict(beam_size=beam_size, num_return_gen=num_return_gen, stop_token=stop_token,
+                                          tokens_to_generate=cfg.tokens_to_generate,
+                                          max_position_embeddings=cfg.max_position_embeddings)
 
     def _beam_search_batched(self, tokens, query_embeds, beam_size, num_return_gen, stop_token, prompt_length):
+        """run_beam_search per chunk of beam_search_chunks (clips of one prompt length), one group per clip of a
+        fixed-length decode state."""
         from ymp import ops
-        cfg = self.config
-        B = tokens.size(0)
-        lengths = torch.as_tensor(prompt_length).reshape(-1).tolist()
-        if len(lengths) == 1:
-            lengths = lengths * B
-        assert len(lengths) == B
-        nq = 0 if query_embeds is None else query_embeds.size(1)
-        final_len = min(tokens.size(1) + cfg.tokens_to_generate, cfg.max_position_embeddings)
-        res = [None] * B
+        lengths, nq, max_len, kw = self._beam_search_args(tokens, query_embeds, prompt_length, beam_size, num_return_gen,
+                                                          stop_token)
+        res = [None] * tokens.size(0)
         for plen, clips in beam_search_chunks(lengths, beam_size, ops.SKINNY_WIDE_MAX_ROWS):
             sel = torch.tensor(clips, dtype=torch.long, device=tokens.device)
-            ip = self.inference_params = InferenceParams(len(clips) * beam_size, final_len + nq)
-            ip.wide_step, ip.prefill_stride = True, beam_size
-            step, reorder = self._decode_callbacks(None if query_embeds is None else query_embeds[sel])
-
-            def first_beams(new_tokens, first, step=step):
-                # the prefill runs each clip's [prefix | prompt] once, into its first beam slot; the cache's row table
-                # points the clip's other beams at it
-                return step(new_tokens[::beam_size] if first else new_tokens, first)
-            outs = run_beam_search_batched(first_beams, reorder, tokens[sel], plen, nq, beam_size=beam_size,
-                                           num_return_gen=num_return_gen, stop_token=stop_token,
-                                           tokens_to_generate=cfg.tokens_to_generate,
-                                           max_position_embeddings=cfg.max_position_embeddings)
-            for i, o in zip(clips, outs):
+            toks, qe = tokens[sel], None if query_embeds is None else query_embeds[sel]
+            dec = self._fixed_len_decoder(toks, qe, len(clips), beam_size, max_len, wide=True)
+            for i, o in zip(clips, run_beam_search(*dec, toks, [plen] * len(clips), nq, groups=len(clips), **kw)):
                 res[i] = o
         return res
 
     def _beam_search_stream(self, tokens, query_embeds, beam_size, num_return_gen, stop_token, prompt_length):
-        """run_beam_search_stream over one KV cache of G = 64 // beam_size groups in per-row mode: the single-token steps
-        replay one captured per-row TokenStep, a finished clip's group is refilled by a group prefill into its first
-        slot."""
-        from ymp import engine, ops
-        cfg = self.config
-        B = tokens.size(0)
-        lengths = torch.as_tensor(prompt_length).reshape(-1).tolist()
-        if len(lengths) == 1:
-            lengths = lengths * B
-        assert len(lengths) == B
-        G = min(ops.SKINNY_WIDE_MAX_ROWS // beam_size, B)
-        if G < 1:
-            raise ValueError(f"beam_size {beam_size} exceeds the {ops.SKINNY_WIDE_MAX_ROWS} rows of one decoding step")
-        nq = 0 if query_embeds is None else query_embeds.size(1)
-        final_len = min(tokens.size(1) + cfg.tokens_to_generate, cfg.max_position_embeddings)
-        rows, ML, dev = G * beam_size, final_len + nq, tokens.device
-        self.inference_params = None
-        key = (rows, ML, str(dev), "per_row")
-        pool = self.__dict__.setdefault("_decode_pool", {})
-        if key not in pool:
-            pool.clear()   # one resident cache, as in _decode
-            pool[key] = engine.KVCache(cfg.engine_cfg(), rows, ML, dev)
-        cache = pool[key]
-        cache.reset_rows()
-        keys, params = self._param_list()
-        W = {k: YF.as_bf16(p) for k, p in zip(keys, params)}
-        sig = (params[0].data_ptr(), params[-1].data_ptr(), sum(p._version for p in params))
-        emb = self.dist_model.language_model.embedding.word_embeddings
-        wemb, pos = W[engine.GPT + "embedding.word_embeddings.weight"], W[engine.GPT + "embedding.position_embeddings.weight"]
-        ts = cache.token
-        if ts is None or ts.sig != sig or not ts.per_row:
-            static = all(p.dtype == torch.bfloat16 or not p.requires_grad for p in params)
-            ts = cache.token = engine.TokenStep(cache, W, emb.weight.dtype, sig, static, per_row=True)
-        elif not ts.static:
-            ts.W = W
-
-        def step(new_tokens, live):
-            cache.set_live([x for x in live for _ in range(beam_size)])
-            _, logits = ts.run(emb(new_tokens).reshape(rows, -1))
-            return logits
-
-        def prefill(group0, group_stride, clips, n):
-            sel = torch.tensor(clips, dtype=torch.long, device=dev)
-            x = emb(tokens[sel, :n])
-            if query_embeds is not None:
-                x = torch.cat([query_embeds[sel].to(x.dtype), x], dim=1)
-            m = n + nq
-            x = (x.float() + pos[:m][None].float()).reshape(len(clips) * m, -1).contiguous()
-            hid = cache.prefill_groups(W, x, m, group0, group_stride, beam_size)
-            return ops.gemm(hid, wemb).float()
-
-        return run_beam_search_stream(step, prefill, cache.reindex_rows, tokens, lengths, nq, beam_size=beam_size,
-                                      num_return_gen=num_return_gen, stop_token=stop_token,
-                                      tokens_to_generate=cfg.tokens_to_generate,
-                                      max_position_embeddings=cfg.max_position_embeddings, groups=G)
+        """One run_beam_search over all clips in G = 64 // beam_size groups of a per-row decode state."""
+        from ymp import ops
+        lengths, nq, max_len, kw = self._beam_search_args(tokens, query_embeds, prompt_length, beam_size, num_return_gen,
+                                                          stop_token)
+        G = min(ops.SKINNY_WIDE_MAX_ROWS // beam_size, tokens.size(0))
+        dec = self._per_row_decoder(tokens, query_embeds, G, beam_size, max_len)
+        return run_beam_search(*dec, tokens, lengths, nq, groups=G, **kw)
 
     @torch.no_grad()
     def generate(self, tokens, do_sample=True, termination_id=None, *args, **kwargs):
